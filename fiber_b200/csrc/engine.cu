@@ -618,7 +618,33 @@ static void worker_destroy(Worker& w) {
 // Claim-unit size: near the body's preferred size, a multiple of the API chunksize when the chunk
 // is smaller (so chunk boundaries coincide with unit boundaries), and a multiple of 16/R tasks so
 // every full slot is 16 B aligned on both sides of the gather.
+//
+// Record bodies (FBR_BODY_RECORD): unit_tasks is what one shared-memory stage of dispatch_record_kernel holds, so the
+// unit never exceeds it (rounded DOWN to the chunk and alignment multiples), and the alignment is
+// lcm(16/gcd(16,R), 16/gcd(16,A)) tasks: every full slot AND every unit's argument offset is 16 B aligned, which
+// keeps both sides of the unit on the bulk-copy path (R = 12, 24, 40 need 4, 2, 2 tasks; 16/R would not do).
+// Chunk boundaries coincide with unit boundaries only while lcm(chunksize, align) fits the stage: pick_unit may grow a
+// unit to 2*pref for that, a record unit cannot, so with e.g. chunksize 1023 and align 4 the unit is the stage-sized
+// pref and a chunk may straddle two units (which only changes how tasks are grouped, never a result).
+static uint32_t gcd_u32(uint32_t a, uint32_t b) { while (b) { const uint32_t t = a % b; a = b; b = t; } return a; }
+static uint32_t pick_unit_record(const BodyEntry& b, uint32_t chunksize, uint64_t n_tasks, int sm_count, uint64_t ring_bytes) {
+    uint32_t pref = b.unit_tasks;
+    if (const char* e = getenv("FBR_UNIT_TASKS")) pref = std::min<uint32_t>(pref, (uint32_t)std::max(16, atoi(e)));
+    const uint64_t per_task = std::max(b.result_bytes, b.arg_bytes);
+    while (pref > 1 && (uint64_t)pref * per_task > ring_bytes / 2) pref >>= 1;
+    while (pref > 256 && (uint64_t)pref * (uint64_t)sm_count > n_tasks) pref >>= 1;
+    const uint32_t ar = 16u / gcd_u32(16u, b.result_bytes), aa = 16u / gcd_u32(16u, b.arg_bytes);
+    const uint32_t align = ar / gcd_u32(ar, aa) * aa;                       // lcm of two powers of two
+    uint32_t unit = pref;
+    if (chunksize <= pref) {
+        const uint32_t m = chunksize / gcd_u32(chunksize, align) * align;   // lcm(chunksize, align)
+        if (m <= pref) unit = pref / m * m;
+    }
+    return std::max(align, unit / align * align);
+}
+
 static uint32_t pick_unit(const BodyEntry& b, uint32_t chunksize, uint64_t n_tasks, int sm_count, uint64_t ring_bytes) {
+    if (b.flags & FBR_BODY_RECORD) return pick_unit_record(b, chunksize, n_tasks, sm_count, ring_bytes);
     uint32_t pref = b.unit_tasks;
     if (pref == 1) return 1;
     if (const char* e = getenv("FBR_UNIT_TASKS")) pref = (uint32_t)std::max(16, atoi(e));   // tuning knob (profiles/pi_perf.py)
@@ -979,6 +1005,8 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
     cx.unit = pick_unit(body, cs, part.count, w.sm_count, p->ring_bytes);
     cx.slot_stride = (uint32_t)round_up((uint64_t)cx.unit * cx.R, 16);
     const uint32_t unit = cx.unit, R = cx.R;
+    if ((body.flags & FBR_BODY_RECORD) && unit > body.unit_tasks)   // a unit must fit the kernel's shared-memory stage
+        return fail(FBR_EINVAL, "record body %s: a claim unit of %u tasks exceeds its stage of %u", body.name.c_str(), unit, body.unit_tasks);
 
     // control block
     if (w.ctrl_free.empty()) return fail(FBR_ENOMEM, "more than %d maps in flight on worker %d", kCtrlSlots, part.worker);
@@ -1426,7 +1454,20 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
         dlclose(h);
         return fail(FBR_EINVAL, "module %s exports body '%s', not '%s'", module_path, m->name, name);
     }
-    if (m->result_bytes == 0 || m->unit_tasks == 0 || (m->arg_bytes % 8) != 0 || m->result_kind > FBR_RES_BITS8) {
+    if (m->flags & FBR_BODY_RECORD) {
+        // staged through shared memory by dispatch_record_kernel: sizes are free within its stages
+        const char* why = nullptr;
+        if (m->arg_bytes == 0 || m->result_bytes == 0 || m->arg_bytes % 4 || m->result_bytes % 4) why = "argument and result bytes must be non-zero multiples of 4";
+        else if (m->arg_bytes > 4096 || m->result_bytes > 4096) why = "argument and result records are at most 4096 bytes";
+        else if (m->result_kind != FBR_RES_BYTES) why = "the result kind must be FBR_RES_BYTES (no bit-packed twin)";
+        else if (m->flags & FBR_BODY_SUMMABLE) why = "results cannot be folded on the device (FBR_BODY_SUMMABLE)";
+        else if (m->flags & FBR_BODY_NEEDS_SHARED) why = "dispatch_record_kernel passes no broadcast block (FBR_BODY_NEEDS_SHARED)";
+        else if (m->unit_tasks == 0) why = "unit_tasks is 0";
+        if (why) {
+            dlclose(h);
+            return fail(FBR_EINVAL, "module %s: record body '%s': %s", module_path, name, why);
+        }
+    } else if (m->result_bytes == 0 || m->unit_tasks == 0 || (m->arg_bytes % 8) != 0 || m->result_kind > FBR_RES_BITS8) {
         dlclose(h);
         return fail(FBR_EINVAL, "module %s: body '%s' has an invalid record layout", module_path, name);
     }
@@ -1635,6 +1676,12 @@ int fbr_map_submit(fbr_pool_t* p, const fbr_map_desc_t* d, uint64_t* seq_out) {
             return fail(FBR_EINVAL, "body %s needs explicit argument records (arg_stride=0)", body.name.c_str());
     } else if (body.flags & FBR_BODY_INDEX_ONLY) {
         return fail(FBR_EINVAL, "body %s takes range() arguments only (arg_stride must be 0)", body.name.c_str());
+    } else if (body.flags & FBR_BODY_RECORD) {
+        // dispatch_record_kernel copies argument records of any 4 B aligned layout (bulk loads where 16 B aligned)
+        if (d->arg_stride < body.arg_bytes || (d->arg_stride % 4) != 0)
+            return fail(FBR_EINVAL, "arg_stride %u invalid for body %s (arg_bytes %u)", d->arg_stride, body.name.c_str(), body.arg_bytes);
+        if (d->n_tasks && !d->args) return fail(FBR_EINVAL, "args is NULL");
+        if ((uintptr_t)d->args % 4) return fail(FBR_EINVAL, "argument records of body %s must be 4-byte aligned", body.name.c_str());
     } else {
         if (d->arg_stride < body.arg_bytes || (d->arg_stride % 8) != 0)
             return fail(FBR_EINVAL, "arg_stride %u invalid for body %s (arg_bytes %u)", d->arg_stride, body.name.c_str(), body.arg_bytes);

@@ -903,6 +903,207 @@ __global__ void __launch_bounds__(160) dispatch_payload_map_tma_kernel(const Wav
 }
 
 // ================================================================================================
+// dispatch: record bodies (FBR_BODY_RECORD) -- any trivially copyable Arg / Res of 4..4096 bytes (multiples
+// of 4), staged through shared memory (warp-specialised, like dispatch_payload_map_tma_kernel):
+//   warp 0 (one elected lane)  waits for an EMPTY IN stage, claims a unit by ticket and bulk-loads the unit's
+//                              count * A argument bytes into it (cp.async.bulk + FULL mbarrier complete_tx);
+//                              with two IN stages the next unit's load overlaps this unit's compute;
+//   warps 1-8 (256 consumers)  copy whatever the bulk load could not take (see below), run B::run one task per
+//                              thread from the IN stage into an OUT stage, then -- after a proxy fence and a
+//                              named barrier -- one of them bulk-stores the unit's count * R result bytes to
+//                              wp.ring + t * slot_stride (the ring slot, or the final index: direct placement).
+// Fallbacks, chosen at run time per unit: argument bytes that are not contiguous (arg_stride != A), not 16 B
+// aligned in global memory, or past the last multiple of 16 are copied by the consumers (16 B vectors where
+// both sides allow it, else 4 B words); the same holds for the result bytes of an unaligned destination or a
+// tail that is not a multiple of 16.  The body sees its argument and result as references into shared memory,
+// so a 1 KB record is never copied into registers.  Known costs (DESIGN.md section 4): records are packed, so lane
+// i's record starts at i * A -- a body that walks a large record word by word has every lane on the same bank
+// (A = 1024: 32-way); reading it in 16 B vectors cuts that to 8-way.  A stage holds kStageBytes of the larger
+// record, so for large records most consumers are idle during B::run (A = 1024: 32 tasks per unit).
+// ================================================================================================
+namespace record {
+constexpr int kConsumers = 256;
+constexpr int kThreads = 32 + kConsumers;
+constexpr int kInStages = 2, kOutStages = 2;
+constexpr uint32_t kStageBytes = 32768;   // per stage, for the larger of A and R
+constexpr uint32_t kMaxUnit = 1024;       // tasks per unit: 4 per consumer thread
+
+template <class B>
+struct Layout {
+    static constexpr uint32_t A = (uint32_t)sizeof(typename B::Arg), R = (uint32_t)sizeof(typename B::Res);
+    static_assert(A % 4 == 0 && R % 4 == 0 && A >= 4 && R >= 4 && A <= 4096 && R <= 4096,
+                  "record bodies: sizeof(Arg) and sizeof(Res) are multiples of 4 between 4 and 4096");
+    // tasks per unit that make count * A and count * R multiples of 16 (A and R are multiples of 4)
+    static constexpr uint32_t kAlign = ((A % 16 == 0) && (R % 16 == 0)) ? 1u : ((A % 8 == 0) && (R % 8 == 0)) ? 2u : 4u;
+    static constexpr uint32_t unit() {
+        const uint32_t w = A > R ? A : R;
+        uint32_t u = kMaxUnit;
+        while (u > kAlign && u * w > kStageBytes) u >>= 1;
+        return u;
+    }
+    static constexpr uint32_t kUnit = unit();
+    static constexpr uint32_t kInBytes = kUnit * A, kOutBytes = kUnit * R;   // multiples of 16
+    // dynamic shared memory of an instantiation: range() maps (index) read no argument bytes and have no IN stages
+    static constexpr size_t smem(bool index) {
+        return (index ? 0 : (size_t)kInStages * kInBytes) + (size_t)kOutStages * kOutBytes;
+    }
+    static_assert(kInBytes % 16 == 0 && kOutBytes % 16 == 0 && smem(false) <= (200u << 10), "record stage layout");
+};
+
+// contiguous copy by `n` threads; 16 B vectors while both sides are 16 B aligned, then 4 B words, then bytes
+__device__ __forceinline__ void coop_copy(uint8_t* dst, const uint8_t* src, uint32_t bytes, uint32_t tid, uint32_t n) {
+    const uintptr_t al = reinterpret_cast<uintptr_t>(dst) | reinterpret_cast<uintptr_t>(src);
+    uint32_t off = 0;
+    if ((al & 15) == 0) {
+        const uint32_t nv = bytes >> 4;
+        for (uint32_t v = tid; v < nv; v += n)
+            reinterpret_cast<uint4*>(dst)[v] = reinterpret_cast<const uint4*>(src)[v];
+        off = nv << 4;
+    }
+    if ((al & 3) == 0) {
+        const uint32_t w1 = bytes >> 2;
+        for (uint32_t w = (off >> 2) + tid; w < w1; w += n)
+            reinterpret_cast<uint32_t*>(dst)[w] = reinterpret_cast<const uint32_t*>(src)[w];
+        off = w1 << 2;
+    }
+    for (uint32_t b = off + tid; b < bytes; b += n) dst[b] = src[b];
+}
+
+// `count` records of A bytes, `stride` bytes apart in global memory (4 B aligned), packed into `dst`
+template <uint32_t A>
+__device__ __forceinline__ void gather_records(uint8_t* dst, const uint8_t* src, uint32_t stride, uint32_t count,
+                                               uint32_t tid, uint32_t n) {
+    constexpr uint32_t W = A / 4;
+    for (uint32_t w = tid; w < count * W; w += n) {
+        const uint32_t i = w / W, k = w - i * W;
+        reinterpret_cast<uint32_t*>(dst)[w] = *reinterpret_cast<const uint32_t*>(src + (size_t)i * stride + 4 * k);
+    }
+}
+}  // namespace record
+
+template <class B, bool kIndex>
+__global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const WaveParams wp) {
+    using namespace bulk;
+    using L = record::Layout<B>;
+    using Arg = typename B::Arg;
+    using Res = typename B::Res;
+    constexpr int kIn = record::kInStages, kOut = record::kOutStages;
+    constexpr uint32_t C = record::kConsumers;
+    extern __shared__ __align__(128) uint8_t smem[];
+    __shared__ uint64_t full[kIn], empty[kIn];
+    __shared__ TaskRecord s_rec[kIn];
+    __shared__ uint32_t s_ticket[kIn];
+    __shared__ uint32_t s_bulk[kIn];      // argument bytes of the unit the bulk load brings (the rest: consumers)
+    __shared__ int s_fault[2];
+    uint8_t* const in_stage = smem;
+    uint8_t* const out_stage = smem + (kIndex ? 0 : (size_t)kIn * L::kInBytes);   // L::smem(kIndex) bytes in all
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < kIn; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], C); }
+        s_fault[0] = 0; s_fault[1] = 0;
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    if (threadIdx.x < 32) {
+        if (threadIdx.x != 0) return;
+        // ---------------- producer ----------------
+        for (uint32_t seq = 0;; ++seq) {
+            const int sg = seq % kIn;
+            mbar_wait(&empty[sg], ((seq / kIn) & 1) ^ 1);      // fresh barrier: passes immediately
+            const uint32_t t = atomicAdd(wp.ticket, 1u);
+            if (t >= wp.n_units) {
+                // each CTA draws exactly one ticket >= n_units; the highest re-arms the counter
+                if (t == wp.n_units + gridDim.x - 1u) *wp.ticket = 0u;
+                s_rec[sg].count = 0u;                            // end marker
+                asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&full[sg])) : "memory");
+                return;
+            }
+            const TaskRecord rec = wave_record(wp, t);
+            s_rec[sg] = rec;
+            s_ticket[sg] = t;
+            uint32_t nb = 0;
+            if constexpr (!kIndex) {
+                const uint8_t* src = wp.args + rec.arg_off;
+                if (wp.arg_stride == L::A && (reinterpret_cast<uintptr_t>(src) & 15) == 0) nb = (rec.count * L::A) & ~15u;
+                s_bulk[sg] = nb;
+                if (nb) {
+                    mbar_expect_tx(&full[sg], nb);
+                    bulk_load(in_stage + (size_t)sg * L::kInBytes, src, nb, &full[sg]);
+                }
+            }
+            if (nb == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&full[sg])) : "memory");
+        }
+    }
+
+    // ---------------- consumers (threads 32..287) ----------------
+    const uint32_t ct = threadIdx.x - 32;
+    for (uint32_t seq = 0;; ++seq) {
+        const int sg = seq % kIn, og = seq % kOut;
+        mbar_wait(&full[sg], (seq / kIn) & 1);
+        const TaskRecord rec = s_rec[sg];
+        if (rec.count == 0) break;
+        const uint32_t t = s_ticket[sg];
+        const uint8_t* in = in_stage + (size_t)sg * L::kInBytes;
+        uint8_t* out = out_stage + (size_t)og * L::kOutBytes;
+        if constexpr (!kIndex) {
+            const uint8_t* src = wp.args + rec.arg_off;
+            uint8_t* stage = in_stage + (size_t)sg * L::kInBytes;
+            if (wp.arg_stride == L::A) {
+                const uint32_t nb = s_bulk[sg];
+                record::coop_copy(stage + nb, src + nb, rec.count * L::A - nb, ct, C);
+            } else {
+                record::gather_records<L::A>(stage, src, wp.arg_stride, rec.count, ct, C);
+            }
+        }
+        // the bulk store that last read OUT stage `og` (unit seq - kOut) must be done with it.  Thread 0 commits exactly
+        // one bulk group per unit (see below), so "at most kOut - 1 groups still reading" means units seq-kOut+1 .. seq-1
+        if (ct == 0 && seq >= (uint32_t)kOut) bulk_wait_read<kOut - 1>();
+        asm volatile("bar.sync 1, %0;" ::"n"(C) : "memory");
+
+        int* const unit_fault = &s_fault[seq & 1];
+        const ErrSink es{wp.err_word, unit_fault};
+        const uint64_t g0 = wp.index_base + rec.first;
+        for (uint32_t i = ct; i < rec.count; i += C) {
+            Res& r = *reinterpret_cast<Res*>(out + (size_t)i * L::R);
+            if constexpr (kIndex) {
+                const Arg a = (Arg)(wp.index_start + (int64_t)(rec.first + i) * wp.index_step);
+                B::run(a, r, g0 + i, es, rec.attempt);
+            } else {
+                B::run(*reinterpret_cast<const Arg*>(in + (size_t)i * L::A), r, g0 + i, es, rec.attempt);
+            }
+        }
+        // generic-proxy writes of this unit's stages become visible to the async proxy (the bulk store below, the
+        // next bulk load into the IN stage); then the IN stage goes back to the producer
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&empty[sg])) : "memory");
+        asm volatile("bar.sync 1, %0;" ::"n"(C) : "memory");
+
+        uint8_t* dst = wp.ring + (size_t)t * wp.slot_stride;
+        const uint32_t bytes = rec.count * L::R;
+        const uint32_t nbs = (reinterpret_cast<uintptr_t>(dst) & 15) == 0 ? (bytes & ~15u) : 0u;
+        if (ct == 0) {
+            // one group per unit, empty when the unit's results are all copied by hand (fewer than 16 bytes, or an
+            // unaligned destination): the wait above counts groups, and must count units
+            if (nbs) bulk_store(dst, out, nbs);
+            else asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        }
+        if (nbs < bytes) record::coop_copy(dst + nbs, out + nbs, bytes - nbs, ct, C);
+        if (ct == 0) {
+            bool lost = false;
+            if constexpr (B::kCanFault) {
+                lost = *unit_fault != 0;                  // every consumer's reports for this unit are in (barrier above)
+                s_fault[(seq + 1) & 1] = 0;               // re-arm the next unit's flag: its writers start after the next barrier
+            }
+            // the thread kernel's protocol: a lost unit is re-dispatched (resilient) or a task error
+            if (lost && !wp.resilient)
+                atomicMin(wp.err_word, (unsigned long long)(((wp.index_base + rec.first) << 8) | TASK_FAULT));
+            put_header(wp, t, SlotHeader{rec.seq, rec.count | ((lost && wp.resilient) ? kUnitLost : 0u), rec.first});
+        }
+    }
+    if (ct == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+}
+
+// ================================================================================================
 // payload_fill: w[t][j] = low32(splitmix64(SEED ^ (t*1024 + j))); each thread emits 16 B.
 // ================================================================================================
 __global__ void __launch_bounds__(kThreads) payload_fill_kernel(uint4* out, uint64_t t0, uint64_t n_vec) {

@@ -198,12 +198,7 @@ class ResultArray(collections.abc.Sequence):
             return self._sum
         if self._bits is not None:
             return int(np.unpackbits(self._bits).sum())   # the bits past n are zero
-        if self._a.dtype.kind in "iu" and self._a.dtype.itemsize == 8:
-            # int64 results: NumPy's sum wraps silently, Python's sum of the reference's list does not
-            lo = int((self._a.view(np.uint64) & np.uint64(0xFFFFFFFF)).sum(dtype=np.uint64))
-            hi = int((self._a.view(np.int64) >> np.int64(32)).sum(dtype=np.int64))
-            return hi * (1 << 32) + lo
-        return int(self._a.sum())
+        return self._spec.sum_rows(self._a)              # what sum() of the reference's list gives, per result layout
 
     def sort(self):
         raise TypeError("ResultArray is read-only; use sorted(result) or result.tolist()")

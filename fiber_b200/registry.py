@@ -21,7 +21,7 @@ from . import _abi
 _BOUND = {}  # callables that cannot carry attributes (builtins) -> body name
 
 
-def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entry=None, **meta):
+def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entry=None, result=None, **meta):
     """Decorator: ``@device_body("pi_inside_det")`` binds ``func`` to the device body ``name`` and sets
     ``func.__fiber_meta__`` (``gpu=1`` unless overridden), like ``fiber.meta``.
 
@@ -33,7 +33,12 @@ def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entr
     how a callable that is not compiled into libfiber_b200 gets its device code there.  ``args`` names the
     argument record layout: ``"i64"`` (one int) or ``"i64x2"`` (two ints).  A bool body may also export its
     bit-packed twin (``FBR_EXPORT_BOOL_BODY_BITS(Body, "<name>_bits8", <bits_entry>, flags)``): pass ``bits_entry``
-    and its results travel one bit each, like the compiled-in bool body's."""
+    and its results travel one bit each, like the compiled-in bool body's.
+
+    A RECORD body (``FBR_EXPORT_RECORD_BODY``: any fixed-size argument and result structs) describes both records
+    with NumPy dtypes: ``args`` and ``result`` take anything ``np.dtype()`` accepts, e.g. ``"<f8"`` or
+    ``[("x", "<f8"), ("y", "<f8")]``, sub-array fields included.  The field names are the function's parameter
+    names; a one-field (or plain scalar) result is returned as that value, several fields as a tuple."""
     from .meta import VALID_META_KEYS
     for k in meta:
         assert k in VALID_META_KEYS, "Invalid meta argument \"{}\"".format(k)
@@ -41,7 +46,7 @@ def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entr
     md.update(meta)
     if source is not None:
         from . import bodies
-        register_module(name, bodies.compile_module(name, source), entry, args, bits_entry)
+        register_module(name, bodies.compile_module(name, source), entry, args, bits_entry, result)
 
     def decorator(func):
         bind(func, name, **md)
@@ -49,7 +54,7 @@ def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entr
     return decorator
 
 
-_MODULES = {}   # body name -> (module path, entry, argument layout) of bodies registered from their own module
+_MODULES = {}   # body name -> (module path, entry, argument layout, bits entry, result layout) of bodies registered from their own module
 
 
 def module_of(name):
@@ -57,11 +62,12 @@ def module_of(name):
     return _MODULES.get(name)
 
 
-def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_entry=None):
+def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_entry=None, result=None):
     """``fbr_register_body`` + the host-side encoder for the body's argument records (and, with ``bits_entry``, the
-    body's bit-packed twin ``<name>_bits8``)."""
+    body's bit-packed twin ``<name>_bits8``).  Record bodies (``FBR_BODY_RECORD``) take NumPy dtypes for ``args`` and
+    ``result``; their sizes must be the module's ``arg_bytes`` / ``result_bytes`` (``ValueError`` otherwise)."""
     import ctypes
-    _MODULES[name] = (str(module_path), entry, args, bits_entry)
+    specs = _load_specs()           # the table as it was: the body registered below gets the encoder its layout asks for
     if bits_entry is not None:
         twin = name + "_bits8"
         register_module(twin, module_path, bits_entry, "bits8")
@@ -70,11 +76,26 @@ def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_
     L = _abi.load()
     fid = ctypes.c_int(-1)
     _abi.check(L.fbr_register_body(name.encode(), str(module_path).encode(), entry.encode(), ctypes.byref(fid)))
-    specs = _load_specs()
+    info = _abi.BodyInfo()
+    _abi.check(L.fbr_body_info(fid.value, ctypes.byref(info)))
+    record = None
+    if info.flags & _abi.FBR_BODY_RECORD:
+        if result is None:
+            raise ValueError("record body %s: pass result=<dtype> (its %d-byte result record)" % (name, info.result_bytes))
+        record = _Record(info, args, result)        # validates both layouts against the module
+        args, result = record.arg_dtype, record.res_dtype
+    elif result is not None:
+        raise ValueError("body %s is not a record body (FBR_EXPORT_RECORD_BODY): its result layout is fixed" % name)
+    old = specs.get(name)
+    if record is not None and isinstance(old, _Record) and (old.arg_dtype, old.res_dtype) != (record.arg_dtype, record.res_dtype):
+        raise ValueError("record body %s is registered already with args=%s, result=%s; a name keeps its layouts"
+                         % (name, old.arg_dtype, old.res_dtype))
+    # the engine keeps the first module registered under a name (fbr_register_body is idempotent): so do worker processes
+    _MODULES.setdefault(name, (str(module_path), entry, args, bits_entry, result))
     if name not in specs:
-        info = _abi.BodyInfo()
-        _abi.check(L.fbr_body_info(fid.value, ctypes.byref(info)))
-        if args == "i64":
+        if record is not None:
+            specs[name] = record
+        elif args == "i64":
             specs[name] = _UnaryI64(info)
         elif args == "i64x2":
             specs[name] = _BinaryI64(info)
@@ -253,6 +274,15 @@ class BodySpec:
             return [tuple(r) for r in arr.tolist()]
         return arr.tolist()
 
+    def sum_rows(self, arr):
+        """``sum()`` of the reference's result list, from the result array."""
+        if arr.dtype.kind in "iu" and arr.dtype.itemsize == 8:
+            # int64 results: NumPy's sum wraps silently, Python's sum of the reference's list does not
+            lo = int((arr.view(np.uint64) & np.uint64(0xFFFFFFFF)).sum(dtype=np.uint64))
+            hi = int((arr.view(np.int64) >> np.int64(32)).sum(dtype=np.int64))
+            return hi * (1 << 32) + lo
+        return int(arr.sum())
+
 
 class _UnaryI64(BodySpec):
     """f(x) with one int argument: square_i64, identity_i64, pi_inside_det, fault_identity_i64."""
@@ -352,6 +382,145 @@ class _BinaryI64(BodySpec):
             rows.append((vals["x"], vals["y"]))
         a = _as_i64(rows, self.name).reshape(len(rows), 2)
         return Encoded(len(rows), args=a, arg_stride=16)
+
+
+_LAYOUT_ALIASES = {"i64": "<i8", "i64x2": [("x", "<i8"), ("y", "<i8")]}
+
+
+def _record_dtype(layout, what, name):
+    """``np.dtype(layout)``, refused when a field holds Python objects (``TypeError``) or is big-endian (the device is
+    little-endian: ``TypeError``)."""
+    dt = np.dtype(_LAYOUT_ALIASES.get(layout, layout) if isinstance(layout, str) else layout)
+
+    def check(d):
+        if d.hasobject:
+            raise TypeError("%s: the %s layout %s holds Python objects; records are fixed-size bytes" % (name, what, dt))
+        if d.names is not None:
+            for f in d.names:
+                check(d.fields[f][0])
+        elif d.subdtype is not None:
+            check(d.subdtype[0])
+        elif d.byteorder == ">" or (d.byteorder == "=" and np.little_endian is False):
+            raise TypeError("%s: the %s layout %s is big-endian; the device reads little-endian records" % (name, what, dt))
+    check(dt)
+    return dt
+
+
+_MISSING = object()
+
+
+class _Record(BodySpec):
+    """A record body (``FBR_BODY_RECORD``): argument and result records described by NumPy dtypes.
+
+    The argument dtype's field names are the function's parameter names (a dtype without fields is one positional
+    parameter).  ``map(f, array)`` with exactly the argument dtype -- or, for a one-parameter body, an array of the
+    parameter's own dtype and shape -- is passed to the engine without a copy; lists, ``starmap`` tuples and
+    ``apply_async(args, kwds)`` are bound to the fields the way Python binds a call.  Results come back as a structured
+    view of the pinned segment; one value per task (a scalar or one-field dtype) reads as that value, several fields
+    as a tuple."""
+
+    def __init__(self, info, args, result):
+        super().__init__(info)
+        self.arg_dtype = _record_dtype(args, "argument", self.name)
+        self.res_dtype = _record_dtype(result, "result", self.name)
+        if self.arg_dtype.itemsize != self.arg_bytes:
+            raise ValueError("%s: argument dtype %s is %d bytes, the body's argument record is %d"
+                             % (self.name, self.arg_dtype, self.arg_dtype.itemsize, self.arg_bytes))
+        if self.res_dtype.itemsize != self.result_bytes:
+            raise ValueError("%s: result dtype %s is %d bytes, the body's result record is %d"
+                             % (self.name, self.res_dtype, self.res_dtype.itemsize, self.result_bytes))
+        self.params = self.arg_dtype.names                 # None: one positional-only parameter
+        # the argument records as a structured array with named fields (one field "_0" when the dtype has none)
+        self._sdt = self.arg_dtype if self.params else np.dtype([("_0", self.arg_dtype)])
+        self._fields = self._sdt.names
+
+    # ---- arguments ------------------------------------------------------------------------------------------------
+    def _fast_map_ok(self, items):
+        return True
+
+    def _bind(self, args, kwds):
+        """Field values of one call ``f(*args, **kwds)``, with Python's TypeErrors for a bad argument list."""
+        names = self.params or ("",)
+        if len(args) > len(names):
+            raise TypeError("%s() takes %d positional argument%s but %d %s given"
+                            % (self.name, len(names), "" if len(names) == 1 else "s", len(args), "was" if len(args) == 1 else "were"))
+        vals = list(args) + [_MISSING] * (len(names) - len(args))
+        for k, v in kwds.items():
+            if self.params is None or k not in self.params:
+                raise TypeError("%s() got an unexpected keyword argument %r" % (self.name, k))
+            j = self.params.index(k)
+            if vals[j] is not _MISSING:
+                raise TypeError("%s() got multiple values for argument %r" % (self.name, k))
+            vals[j] = v
+        missing = [repr(names[j]) for j, v in enumerate(vals) if v is _MISSING]
+        if missing:
+            listed = missing[0] if len(missing) == 1 else "%s and %s" % (", ".join(missing[:-1]) + ("," if len(missing) > 2 else ""), missing[-1])
+            raise TypeError("%s() missing %d required positional argument%s: %s"
+                            % (self.name, len(missing), "" if len(missing) == 1 else "s", listed))
+        return vals
+
+    def _columns(self, columns):
+        arr = np.empty(len(columns[0]) if columns else 0, self._sdt)
+        for f, col in zip(self._fields, columns):
+            arr[f] = col
+        return Encoded(len(arr), args=arr, arg_stride=self.arg_bytes)
+
+    def _encode(self, items, fast, apply=False):
+        if fast:
+            if isinstance(items, range) and self.flags & _abi.FBR_BODY_INDEX_ARG:
+                if len(items) and not (-2 ** 63 <= items[0] <= 2 ** 63 - 1 and -2 ** 63 <= items[-1] <= 2 ** 63 - 1):
+                    raise OverflowError("range() bounds exceed the int64 task record")
+                return Encoded(len(items), index_start=items.start, index_step=items.step)
+            if isinstance(items, np.ndarray):
+                if items.ndim == 1 and items.dtype == self.arg_dtype:
+                    a = np.ascontiguousarray(items)         # zero-copy when it already is
+                    return Encoded(len(a), args=a, arg_stride=self.arg_bytes)
+                one = self._sdt.fields[self._fields[0]][0]
+                if len(self._fields) == 1 and items.ndim >= 1 and items.dtype == one.base and items.shape[1:] == one.shape:
+                    a = np.ascontiguousarray(items)
+                    return Encoded(len(a), args=a.reshape(len(a), -1).view(self._sdt).reshape(len(a)), arg_stride=self.arg_bytes)
+            if len(self._fields) == 1:
+                return self._columns([list(items)])
+            items = [(it,) for it in items]                 # map() passes one argument: f(item) must bind
+        rows = [self._bind(*self._split(it, apply)) for it in items]
+        return self._columns([list(c) for c in zip(*rows)] if rows else [[] for _ in self._fields])
+
+    # ---- results --------------------------------------------------------------------------------------------------
+    def result_dtype(self):
+        d = self.res_dtype
+        if d.names is None and d.subdtype is not None:
+            return d.subdtype[0], d.subdtype[1]
+        return d, ()
+
+    def to_python(self, row):
+        names = self.res_dtype.names
+        if names is None:
+            return row.tolist()
+        if len(names) == 1:
+            return row[names[0]].tolist()
+        return tuple(row[n].tolist() for n in names)
+
+    def rows_to_list(self, arr):
+        names = self.res_dtype.names
+        if names is None:
+            return arr.tolist()
+        if len(names) == 1:
+            return arr[names[0]].tolist()
+        return list(zip(*(arr[n].tolist() for n in names)))
+
+    def unpack_result(self, raw):
+        return self.to_python(np.frombuffer(raw, self.res_dtype)[0])
+
+    def sum_rows(self, arr):
+        names = self.res_dtype.names
+        if names is not None and len(names) > 1:
+            raise TypeError("unsupported operand type(s) for +: 'int' and 'tuple' (%s returns %d fields)" % (self.name, len(names)))
+        vals = arr[names[0]] if names else arr
+        if vals.ndim > 1:
+            raise TypeError("unsupported operand type(s) for +: 'int' and 'list' (%s returns an array per task)" % self.name)
+        if vals.dtype.kind in "iub" and vals.dtype.itemsize <= 4:
+            return int(vals.sum(dtype=np.int64))         # exact: fewer than 2^31 values of at most 32 bits
+        return sum(vals.tolist())                        # Python's left-to-right sum, as over the reference's list
 
 
 class _SleepF64(BodySpec):

@@ -22,9 +22,32 @@
 // (fiber_b200.device_body(name, source=...) does the last two steps from Python.)  The body is instantiated
 // into the same persistent-CTA dispatch kernel template the compiled-in bodies use, so it gets the ticket
 // claim, record synthesis, direct placement / result ring, sum fold and resilient re-dispatch for free.
+//
+// A ThreadBody returns a 1- or 8-byte value.  A function over other fixed-size records -- f(x: float) -> float,
+// f(x, y) -> (r, theta), a row of 256 uint32 -> a few statistics -- is a RECORD body: Arg and Res are any
+// trivially copyable structs (sizeof a multiple of 4, at most 4096 bytes), and run() writes the result in place:
+//
+//     struct Polar {
+//         struct Arg { double x, y; }; struct Res { double r2, r; };
+//         static constexpr bool kIndexArg = false;       // true: Arg = int64_t, range() maps need no argument bytes
+//         static constexpr bool kCanFault = false;
+//         __device__ static void run(const Arg& a, Res& r, uint64_t task_index, const fbr::ErrSink& es, uint32_t attempt) {
+//             r.r2 = __dadd_rn(__dmul_rn(a.x, a.x), __dmul_rn(a.y, a.y)); r.r = __dsqrt_rn(r.r2);
+//         }
+//     };
+//     FBR_EXPORT_RECORD_BODY(Polar, "polar_f64", polar_entry, 0)
+//
+// `a` and `r` refer to shared memory: dispatch_record_kernel bulk-loads each claim unit's argument records into a
+// shared-memory stage and bulk-stores the unit's results from another, so a large record is never copied into
+// registers.  From Python: fiber_b200.device_body("polar_f64", source=..., entry="polar_entry",
+// args=[("x", "<f8"), ("y", "<f8")], result=[("r2", "<f8"), ("r", "<f8")]) -- the NumPy dtypes describe the
+// two structs byte for byte (INTEGRATION.md).  Record bodies cannot fold sums on the device and have no
+// bit-packed twin.
 #pragma once
 #include "fiber_b200.h"
 #include "kernels.cuh"      // fiber_b200/csrc: dispatch_thread_kernel, WaveParams, ErrSink, TaskError
+
+#include <type_traits>
 
 namespace fbr_body_export {
 template <class B>
@@ -90,6 +113,66 @@ int occupancy_bits(int index_mode) {
                                             8u * (uint32_t)sizeof(typename Body::Arg), 1u, (uint32_t)FBR_RES_BITS8, \
                                             (uint32_t)(body_flags), 512u,                                        \
                                             fbr_body_export::launch_bits<Body>, fbr_body_export::occupancy_bits<Body>}; \
+        return &m;                                                                                               \
+    }
+
+namespace fbr_body_export {
+// record bodies: dispatch_record_kernel, dynamic shared memory of Layout<B>::smem(index) bytes
+template <class B>
+void launch_record(const void* wpv, int grid, void* sv) {
+    const fbr::WaveParams& wp = *(const fbr::WaveParams*)wpv;
+    cudaStream_t s = (cudaStream_t)sv;
+    using L = fbr::record::Layout<B>;
+    if constexpr (B::kIndexArg) {
+        if (wp.arg_stride == 0) {
+            fbr::dispatch_record_kernel<B, true><<<grid, fbr::record::kThreads, L::smem(true), s>>>(wp);
+            return;
+        }
+    }
+    fbr::dispatch_record_kernel<B, false><<<grid, fbr::record::kThreads, L::smem(false), s>>>(wp);
+}
+// Also raises the kernels' dynamic shared-memory limit on the current device; the engine asks for the occupancy on
+// every device before the body's first launch there.
+template <class B>
+int occupancy_record(int index_mode) {
+    using L = fbr::record::Layout<B>;
+    const void* k = (const void*)fbr::dispatch_record_kernel<B, false>;
+    size_t smem = L::smem(false);
+    cudaFuncSetAttribute(fbr::dispatch_record_kernel<B, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L::smem(false));
+    if constexpr (B::kIndexArg) {
+        cudaFuncSetAttribute(fbr::dispatch_record_kernel<B, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L::smem(true));
+        if (index_mode) {
+            k = (const void*)fbr::dispatch_record_kernel<B, true>;
+            smem = L::smem(true);
+        }
+    }
+    int occ = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k, fbr::record::kThreads, smem) != cudaSuccess) { cudaGetLastError(); return 1; }
+    return occ > 0 ? occ : 1;
+}
+template <class B>
+constexpr bool record_body_ok() {
+    static_assert(std::is_trivially_copyable<typename B::Arg>::value && std::is_trivially_copyable<typename B::Res>::value,
+                  "record bodies: Arg and Res are trivially copyable");
+    static_assert(!B::kIndexArg || std::is_same<typename B::Arg, int64_t>::value, "record bodies with kIndexArg take Arg = int64_t");
+    return true;
+}
+}  // namespace fbr_body_export
+
+// Body: a RecordBody -- Arg and Res are trivially copyable, sizeof a multiple of 4 and at most 4096 (see the header
+// comment).  The result kind is FBR_RES_BYTES; FBR_BODY_RECORD is added to body_flags, which carry FBR_BODY_INDEX_ARG
+// exactly when Body::kIndexArg is true (a range() map of a body without the index instantiation would read no
+// arguments).  unit_tasks is the number of tasks whose records fill one shared-memory stage of dispatch_record_kernel.
+#define FBR_EXPORT_RECORD_BODY(Body, body_name, entry, body_flags)                                                \
+    static_assert(fbr_body_export::record_body_ok<Body>(), "record body");                                       \
+    static_assert((((body_flags) & FBR_BODY_INDEX_ARG) != 0) == Body::kIndexArg,                                 \
+                  "record bodies: FBR_BODY_INDEX_ARG in the flags if and only if kIndexArg");                     \
+    extern "C" const fbr_body_module_t* entry(void) {                                                            \
+        static const fbr_body_module_t m = {FBR_BODY_MODULE_ABI, (uint32_t)sizeof(fbr::WaveParams), body_name,   \
+                                            fbr::record::Layout<Body>::A, fbr::record::Layout<Body>::R,          \
+                                            (uint32_t)FBR_RES_BYTES, (uint32_t)(body_flags) | FBR_BODY_RECORD,    \
+                                            fbr::record::Layout<Body>::kUnit,                                    \
+                                            fbr_body_export::launch_record<Body>, fbr_body_export::occupancy_record<Body>}; \
         return &m;                                                                                               \
     }
 
