@@ -18,7 +18,8 @@ FBR_OK, FBR_EINVAL, FBR_ECUDA, FBR_ENOMEM, FBR_ESTATE, FBR_ETIMEOUT, FBR_ETASK, 
 # fbr_result_kind
 FBR_RES_BYTES, FBR_RES_BOOL, FBR_RES_I64, FBR_RES_U32, FBR_RES_F64X2, FBR_RES_NONE, FBR_RES_BITS8 = range(7)
 # body flags
-FBR_BODY_INDEX_ARG, FBR_BODY_NEEDS_SHARED, FBR_BODY_SUMMABLE, FBR_BODY_INDEX_ONLY, FBR_BODY_RECORD = 0x1, 0x2, 0x4, 0x8, 0x10
+FBR_BODY_INDEX_ARG, FBR_BODY_NEEDS_SHARED, FBR_BODY_SUMMABLE, FBR_BODY_INDEX_ONLY, FBR_BODY_RECORD, FBR_BODY_BROADCAST = \
+    0x1, 0x2, 0x4, 0x8, 0x10, 0x20
 # pool flags
 FBR_POOL_TIMING, FBR_POOL_OVERLAP = 0x1, 0x2
 # map flags
@@ -31,7 +32,7 @@ FBR_TASK_OK, FBR_TASK_OVERFLOW, FBR_TASK_BADARG, FBR_TASK_FAULT = range(4)
 # every symbol include/fiber_b200.h declares (tests check the .so exports each of them)
 SYMBOLS = [
     "fbr_abi_version", "fbr_last_error", "fbr_device_count",
-    "fbr_body_count", "fbr_body_info", "fbr_body_lookup", "fbr_register_body",
+    "fbr_body_count", "fbr_body_info", "fbr_body_lookup", "fbr_register_body", "fbr_body_shared_info",
     "fbr_pool_create", "fbr_pool_close", "fbr_pool_terminate", "fbr_pool_join", "fbr_pool_destroy",
     "fbr_pool_n_workers", "fbr_pool_worker_device",
     "fbr_map_submit", "fbr_shared_put", "fbr_shared_drop", "fbr_plan_query",
@@ -136,6 +137,7 @@ def load():
         "fbr_body_info": (i32, [i32, P(BodyInfo)]),
         "fbr_body_lookup": (i32, [ctypes.c_char_p, P(i32)]),
         "fbr_register_body": (i32, [ctypes.c_char_p, ctypes.c_char_p, ctypes.c_char_p, P(i32)]),
+        "fbr_body_shared_info": (i32, [i32, P(u32), P(u32)]),
         "fbr_pool_create": (i32, [i32, P(i32), u64, u32, P(vp)]),
         "fbr_pool_close": (i32, [vp]),
         "fbr_pool_terminate": (i32, [vp]),

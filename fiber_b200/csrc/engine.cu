@@ -181,6 +181,7 @@ struct BodyEntry {
     occupancy_fn occupancy = nullptr;
     int max_ctas_per_sm = 0;   // 0 = as many as fit; streaming read+write bodies run best with few, fat streams
     void* module = nullptr;    // dlopen handle of a registered body (never closed: kernels may be in flight)
+    uint32_t shared_elem_bytes = 0, shared_stage_bytes = 0;   // FBR_BODY_BROADCAST record bodies
 };
 
 static std::mutex g_body_mu;
@@ -1021,8 +1022,17 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
             auto it = p->shared.find((uint64_t)(uintptr_t)d.shared);
             if (it == p->shared.end()) return fail(FBR_ENOENT, "unknown shared handle");
             cx.d_shared = (const uint8_t*)it->second.d_ptr[part.worker];
-        } else if (cx.args_dev) {
+        } else if (cx.args_dev && !((uintptr_t)d.shared & 15)) {
             cx.d_shared = (const uint8_t*)d.shared;
+        } else if (cx.args_dev && (body.flags & FBR_BODY_BROADCAST) && d.shared_bytes <= body.shared_stage_bytes) {
+            // staged: the kernel copies whatever is not 16 B aligned into shared memory by hand
+            cx.d_shared = (const uint8_t*)d.shared;
+        } else if (cx.args_dev) {
+            // a caller's device block at a base that is not 16 B aligned, read in place by the kernel: a body may load its
+            // elements as 8 or 16 B vectors (an alignas(16) struct, doubles), which would fault there.  Read an aligned copy.
+            CK(cudaMallocAsync(&part.d_shared_tmp, d.shared_bytes, w.s_in));
+            CK(cudaMemcpyAsync(part.d_shared_tmp, d.shared, d.shared_bytes, cudaMemcpyDefault, w.s_in));
+            cx.d_shared = (const uint8_t*)part.d_shared_tmp;
         } else {
             CK(cudaMallocAsync(&part.d_shared_tmp, d.shared_bytes, w.s_in));
             CK(cudaMemcpyAsync(part.d_shared_tmp, d.shared, d.shared_bytes, cudaMemcpyHostToDevice, w.s_in));
@@ -1426,6 +1436,14 @@ int fbr_body_info(int func_id, fbr_body_info_t* info) {
     return FBR_OK;
 }
 
+int fbr_body_shared_info(int func_id, uint32_t* elem_bytes, uint32_t* stage_bytes) {
+    const BodyEntry* bp = body_of(func_id);
+    if (!elem_bytes || !stage_bytes || !bp) return fail(FBR_EINVAL, "bad func_id %d", func_id);
+    *elem_bytes = bp->shared_elem_bytes;
+    *stage_bytes = bp->shared_stage_bytes;
+    return FBR_OK;
+}
+
 int fbr_body_lookup(const char* name, int* func_id) {
     if (!name || !func_id) return fail(FBR_EINVAL, "NULL argument");
     for (int f = 0, n = body_count(); f < n; ++f)
@@ -1454,6 +1472,15 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
         dlclose(h);
         return fail(FBR_EINVAL, "module %s exports body '%s', not '%s'", module_path, m->name, name);
     }
+    const bool bcast = (m->flags & FBR_BODY_BROADCAST) != 0;
+    if (!bcast && (m->shared_elem_bytes || m->shared_stage_bytes)) {
+        dlclose(h);
+        return fail(FBR_EINVAL, "module %s: body '%s' describes a broadcast element but lacks FBR_BODY_BROADCAST", module_path, name);
+    }
+    if (bcast && !(m->flags & FBR_BODY_RECORD)) {
+        dlclose(h);
+        return fail(FBR_EINVAL, "module %s: body '%s': only record bodies take a broadcast block (FBR_BODY_BROADCAST)", module_path, name);
+    }
     if (m->flags & FBR_BODY_RECORD) {
         // staged through shared memory by dispatch_record_kernel: sizes are free within its stages
         const char* why = nullptr;
@@ -1461,8 +1488,16 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
         else if (m->arg_bytes > 4096 || m->result_bytes > 4096) why = "argument and result records are at most 4096 bytes";
         else if (m->result_kind != FBR_RES_BYTES) why = "the result kind must be FBR_RES_BYTES (no bit-packed twin)";
         else if (m->flags & FBR_BODY_SUMMABLE) why = "results cannot be folded on the device (FBR_BODY_SUMMABLE)";
-        else if (m->flags & FBR_BODY_NEEDS_SHARED) why = "dispatch_record_kernel passes no broadcast block (FBR_BODY_NEEDS_SHARED)";
+        else if ((m->flags & FBR_BODY_NEEDS_SHARED) && !bcast)
+            why = "a body without a Shared element type receives no broadcast block (FBR_BODY_NEEDS_SHARED without FBR_BODY_BROADCAST)";
+        else if (bcast && !(m->flags & FBR_BODY_NEEDS_SHARED)) why = "FBR_BODY_BROADCAST needs FBR_BODY_NEEDS_SHARED (its maps must pass a block)";
+        else if (bcast && (m->shared_elem_bytes == 0 || m->shared_elem_bytes % 4 || m->shared_elem_bytes > 4096))
+            why = "the broadcast element must be a non-zero multiple of 4 bytes up to 4096";
+        else if (bcast && m->shared_stage_bytes % 16) why = "the broadcast staging budget must be a multiple of 16 bytes";
         else if (m->unit_tasks == 0) why = "unit_tasks is 0";
+        // dispatch_record_kernel's shared memory: two IN and two OUT stages of one unit each, then the broadcast region
+        else if (2ull * m->unit_tasks * (m->arg_bytes + m->result_bytes) + m->shared_stage_bytes > (200ull << 10))
+            why = "the stages and the broadcast staging budget exceed 200 KB of shared memory";
         if (why) {
             dlclose(h);
             return fail(FBR_EINVAL, "module %s: record body '%s': %s", module_path, name, why);
@@ -1484,6 +1519,7 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
     b.name = name;
     b.arg_bytes = m->arg_bytes; b.result_bytes = m->result_bytes; b.result_kind = m->result_kind;
     b.flags = m->flags; b.unit_tasks = m->unit_tasks;
+    b.shared_elem_bytes = m->shared_elem_bytes; b.shared_stage_bytes = m->shared_stage_bytes;
     b.launch = m->launch; b.occupancy = m->occupancy;
     b.module = h;
     g_bodies.push_back(b);
@@ -1689,8 +1725,24 @@ int fbr_map_submit(fbr_pool_t* p, const fbr_map_desc_t* d, uint64_t* seq_out) {
         if (body.arg_bytes >= 16 && body.result_kind != FBR_RES_BITS8 && (d->arg_stride % 16 || ((uintptr_t)d->args % 16)))
             return fail(FBR_EINVAL, "argument records of body %s must be 16-byte aligned", body.name.c_str());
     }
-    if ((body.flags & FBR_BODY_NEEDS_SHARED) && (!d->shared || d->shared_bytes < sizeof(ParzenShared)))
+    if (body.flags & FBR_BODY_BROADCAST) {
+        // run() iterates over shared_bytes / elem_bytes elements: the block must hold exactly that many
+        if (!d->shared || d->shared_bytes == 0)
+            return fail(FBR_EINVAL, "body %s needs a broadcast block", body.name.c_str());
+        if (d->shared_bytes % body.shared_elem_bytes)
+            return fail(FBR_EINVAL, "body %s: broadcast block of %llu bytes is not a whole number of %u-byte elements", body.name.c_str(),
+                        (unsigned long long)d->shared_bytes, body.shared_elem_bytes);
+    } else if ((body.flags & FBR_BODY_NEEDS_SHARED) && (!d->shared || d->shared_bytes < sizeof(ParzenShared))) {
         return fail(FBR_EINVAL, "body %s needs a shared argument block", body.name.c_str());
+    }
+    if (d->shared && d->shared_bytes && (d->flags & FBR_SHARED_HANDLE)) {
+        // a kernel reads shared_bytes from the handle's allocation: it must not claim more than fbr_shared_put uploaded
+        auto it = p->shared.find((uint64_t)(uintptr_t)d->shared);
+        if (it == p->shared.end()) return fail(FBR_ENOENT, "unknown shared handle");
+        if (d->shared_bytes > it->second.bytes)
+            return fail(FBR_EINVAL, "shared_bytes %llu exceeds the %llu bytes of shared handle %llu", (unsigned long long)d->shared_bytes,
+                        (unsigned long long)it->second.bytes, (unsigned long long)(uintptr_t)d->shared);
+    }
     if ((d->flags & FBR_OUT_DEVICE) && !d->out) return fail(FBR_EINVAL, "FBR_OUT_DEVICE without out");
     if ((d->flags & FBR_RESULTS_ON_DEVICE) && ((d->flags & FBR_OUT_DEVICE) || d->out))
         return fail(FBR_EINVAL, "FBR_RESULTS_ON_DEVICE owns its output buffer: do not pass out / FBR_OUT_DEVICE");

@@ -920,7 +920,17 @@ __global__ void __launch_bounds__(160) dispatch_payload_map_tma_kernel(const Wav
 // i's record starts at i * A -- a body that walks a large record word by word has every lane on the same bank
 // (A = 1024: 32-way); reading it in 16 B vectors cuts that to 8-way.  A stage holds kStageBytes of the larger
 // record, so for large records most consumers are idle during B::run (A = 1024: 32 tasks per unit).
+// Bodies with a Shared element type also receive the map's broadcast block: one within the body's kSharedStage is
+// bulk-loaded once per CTA into a region after the stages (DESIGN.md section 4 has the staged vs global measurement).
 // ================================================================================================
+// The map's broadcast block as a record body with a Shared element type sees it: n = shared_bytes / sizeof(T) elements,
+// read-only, in shared memory when the block fits the body's kSharedStage, else in global memory.
+template <class T>
+struct Broadcast {
+    const T* data;
+    uint64_t n;
+};
+
 namespace record {
 constexpr int kConsumers = 256;
 constexpr int kThreads = 32 + kConsumers;
@@ -928,11 +938,30 @@ constexpr int kInStages = 2, kOutStages = 2;
 constexpr uint32_t kStageBytes = 32768;   // per stage, for the larger of A and R
 constexpr uint32_t kMaxUnit = 1024;       // tasks per unit: 4 per consumer thread
 
+// A record body opts into the broadcast block with `using Shared = <element>;` and `static constexpr uint32_t
+// kSharedStage = <bytes>;`; its run() then takes a const Broadcast<Shared>& after the result.
+template <class B, class = void>
+struct BroadcastOf {
+    static constexpr bool kOn = false;
+    static constexpr uint32_t kElem = 0, kStage = 0;
+};
+template <class B>
+struct BroadcastOf<B, std::void_t<typename B::Shared>> {
+    using T = typename B::Shared;
+    static constexpr bool kOn = true;
+    static constexpr uint32_t kElem = (uint32_t)sizeof(T), kStage = B::kSharedStage;
+    static_assert(std::is_trivially_copyable<T>::value, "broadcast bodies: Shared is trivially copyable");
+    static_assert(kElem % 4 == 0 && kElem <= 4096, "broadcast bodies: sizeof(Shared) is a multiple of 4 up to 4096");
+    static_assert(kStage % 16 == 0, "broadcast bodies: kSharedStage is a multiple of 16 (0: never stage)");
+};
+
 template <class B>
 struct Layout {
     static constexpr uint32_t A = (uint32_t)sizeof(typename B::Arg), R = (uint32_t)sizeof(typename B::Res);
     static_assert(A % 4 == 0 && R % 4 == 0 && A >= 4 && R >= 4 && A <= 4096 && R <= 4096,
                   "record bodies: sizeof(Arg) and sizeof(Res) are multiples of 4 between 4 and 4096");
+    // the broadcast region after the IN / OUT stages (0 bytes for bodies without a Shared type)
+    static constexpr uint32_t kShared = BroadcastOf<B>::kStage;
     // tasks per unit that make count * A and count * R multiples of 16 (A and R are multiples of 4)
     static constexpr uint32_t kAlign = ((A % 16 == 0) && (R % 16 == 0)) ? 1u : ((A % 8 == 0) && (R % 8 == 0)) ? 2u : 4u;
     static constexpr uint32_t unit() {
@@ -944,9 +973,10 @@ struct Layout {
     static constexpr uint32_t kUnit = unit();
     static constexpr uint32_t kInBytes = kUnit * A, kOutBytes = kUnit * R;   // multiples of 16
     // dynamic shared memory of an instantiation: range() maps (index) read no argument bytes and have no IN stages
-    static constexpr size_t smem(bool index) {
+    static constexpr size_t stages(bool index) {
         return (index ? 0 : (size_t)kInStages * kInBytes) + (size_t)kOutStages * kOutBytes;
     }
+    static constexpr size_t smem(bool index) { return stages(index) + kShared; }
     static_assert(kInBytes % 16 == 0 && kOutBytes % 16 == 0 && smem(false) <= (200u << 10), "record stage layout");
 };
 
@@ -997,8 +1027,22 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
     __shared__ int s_fault[2];
     uint8_t* const in_stage = smem;
     uint8_t* const out_stage = smem + (kIndex ? 0 : (size_t)kIn * L::kInBytes);   // L::smem(kIndex) bytes in all
+    // broadcast bodies: the block is staged once per CTA into the region after the stages when it fits kSharedStage
+    // (a run-time choice, uniform across the launch), else run() reads it from global memory
+    using Bc = record::BroadcastOf<B>;
+    uint64_t* bcast_full = nullptr;
+    uint8_t* const bcast_stage = out_stage + (size_t)kOut * L::kOutBytes;   // L::stages(kIndex) bytes in
+    bool staged = false;
+    uint32_t bcast_bulk = 0;                           // bytes of the block the bulk load brings (the rest: consumers)
+    if constexpr (Bc::kOn && Bc::kStage > 0) {
+        __shared__ uint64_t s_bcast_full;
+        bcast_full = &s_bcast_full;
+        staged = wp.shared_bytes <= Bc::kStage;
+        if ((reinterpret_cast<uintptr_t>(wp.shared) & 15) == 0) bcast_bulk = (uint32_t)wp.shared_bytes & ~15u;
+    }
     if (threadIdx.x == 0) {
         for (int s = 0; s < kIn; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], C); }
+        if constexpr (Bc::kOn && Bc::kStage > 0) mbar_init(bcast_full, 1);
         s_fault[0] = 0; s_fault[1] = 0;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -1007,6 +1051,18 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
     if (threadIdx.x < 32) {
         if (threadIdx.x != 0) return;
         // ---------------- producer ----------------
+        if constexpr (Bc::kOn && Bc::kStage > 0) {
+            // before the first claim: every consumer waits for the block once (also in a CTA that gets no unit, so no
+            // bulk load is still in flight when the CTA exits)
+            if (staged) {
+                if (bcast_bulk) {
+                    mbar_expect_tx(bcast_full, bcast_bulk);
+                    bulk_load(bcast_stage, wp.shared, bcast_bulk, bcast_full);
+                } else {
+                    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bcast_full)) : "memory");
+                }
+            }
+        }
         for (uint32_t seq = 0;; ++seq) {
             const int sg = seq % kIn;
             mbar_wait(&empty[sg], ((seq / kIn) & 1) ^ 1);      // fresh barrier: passes immediately
@@ -1037,6 +1093,14 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
 
     // ---------------- consumers (threads 32..287) ----------------
     const uint32_t ct = threadIdx.x - 32;
+    if constexpr (Bc::kOn && Bc::kStage > 0) {
+        if (staged) {
+            // the bytes the bulk load could not take (an unaligned base, a tail under 16 B) are copied by hand, never
+            // reading past shared_bytes; the named barrier before the first run() publishes them to every consumer
+            mbar_wait(bcast_full, 0);
+            record::coop_copy(bcast_stage + bcast_bulk, wp.shared + bcast_bulk, (uint32_t)wp.shared_bytes - bcast_bulk, ct, C);
+        }
+    }
     for (uint32_t seq = 0;; ++seq) {
         const int sg = seq % kIn, og = seq % kOut;
         mbar_wait(&full[sg], (seq / kIn) & 1);
@@ -1063,14 +1127,33 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
         int* const unit_fault = &s_fault[seq & 1];
         const ErrSink es{wp.err_word, unit_fault};
         const uint64_t g0 = wp.index_base + rec.first;
-        for (uint32_t i = ct; i < rec.count; i += C) {
-            Res& r = *reinterpret_cast<Res*>(out + (size_t)i * L::R);
-            if constexpr (kIndex) {
-                const Arg a = (Arg)(wp.index_start + (int64_t)(rec.first + i) * wp.index_step);
-                B::run(a, r, g0 + i, es, rec.attempt);
-            } else {
-                B::run(*reinterpret_cast<const Arg*>(in + (size_t)i * L::A), r, g0 + i, es, rec.attempt);
+        if constexpr (!Bc::kOn) {
+            for (uint32_t i = ct; i < rec.count; i += C) {
+                Res& r = *reinterpret_cast<Res*>(out + (size_t)i * L::R);
+                if constexpr (kIndex) {
+                    const Arg a = (Arg)(wp.index_start + (int64_t)(rec.first + i) * wp.index_step);
+                    B::run(a, r, g0 + i, es, rec.attempt);
+                } else {
+                    B::run(*reinterpret_cast<const Arg*>(in + (size_t)i * L::A), r, g0 + i, es, rec.attempt);
+                }
             }
+        } else {
+            using T = typename Bc::T;
+            // one loop per placement of the block, so each sees its pointer's address space (shared or global loads)
+            auto run_unit = [&](const Broadcast<T>& sh) {
+                for (uint32_t i = ct; i < rec.count; i += C) {
+                    Res& r = *reinterpret_cast<Res*>(out + (size_t)i * L::R);
+                    if constexpr (kIndex) {
+                        const Arg a = (Arg)(wp.index_start + (int64_t)(rec.first + i) * wp.index_step);
+                        B::run(a, r, sh, g0 + i, es, rec.attempt);
+                    } else {
+                        B::run(*reinterpret_cast<const Arg*>(in + (size_t)i * L::A), r, sh, g0 + i, es, rec.attempt);
+                    }
+                }
+            };
+            const uint64_t n_elems = wp.shared_bytes / Bc::kElem;
+            if (staged) run_unit(Broadcast<T>{reinterpret_cast<const T*>(bcast_stage), n_elems});
+            else run_unit(Broadcast<T>{reinterpret_cast<const T*>(wp.shared), n_elems});
         }
         // generic-proxy writes of this unit's stages become visible to the async proxy (the bulk store below, the
         // next bulk load into the IN stage); then the IN stage goes back to the producer

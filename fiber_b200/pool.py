@@ -479,6 +479,13 @@ class Pool:
         if self._isolation == "process":
             if self._proc is None:
                 from .procpool import ProcessPool
+                init = None
+                if self._initializer is not None:
+                    # every worker process runs the initializer (fiber/pool.py:858-859): it uploads initargs itself.
+                    # Bad initargs raise here, as with thread isolation, instead of killing every worker process at start
+                    body = self._initializer.__fbr_init_body__
+                    registry.spec(body).shared_block(*self._initargs)
+                    init = (body, tuple(self._initargs), registry.module_of(body))
                 lib = _abi.load()
                 n = ctypes.c_int(0)
                 _abi.check(lib.fbr_device_count(ctypes.byref(n)))            # counts devices, creates no context
@@ -486,7 +493,7 @@ class Pool:
                     raise _abi.EngineError(_abi.FBR_ENODEV, "no CUDA device visible; fiber_b200 has no CPU fallback")
                 devs = self._devices if self._devices is not None else list(range(n.value))
                 self._proc = ProcessPool(self._processes, devs, results="bytes" if not self._results_bits else "host",
-                                         redispatch=self._error_handling)
+                                         redispatch=self._error_handling, init=init)
             self._proc.start()
             self._worker_handler_started = True
             return

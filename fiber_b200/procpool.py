@@ -82,14 +82,31 @@ def _proxy_for(body):
     return proxy
 
 
-def gpu_worker_main(device, conn, results, sys_path):
-    """Worker process: one engine on one GPU, blocks in, ordered result bytes out (into shared memory)."""
+def _initializer_for(body):
+    """A pool initializer bound to the broadcast block of device body ``body`` (the worker runs the master's initializer,
+    like every worker of the reference runs ``initializer(*initargs)``)."""
+    from . import registry
+
+    def initializer(*a):
+        raise RuntimeError("bound to the broadcast block of device body %s" % body)
+    return registry.device_initializer(body)(initializer)
+
+
+def gpu_worker_main(device, conn, results, sys_path, init=None):
+    """Worker process: one engine on one GPU, blocks in, ordered result bytes out (into shared memory).  ``init``:
+    (body, initargs, module) of the pool's initializer, or None."""
     for p in sys_path:
         if p not in sys.path:
             sys.path.insert(0, p)
     import fiber_b200
     from fiber_b200 import _abi, registry
-    pool = fiber_b200.Pool(1, devices=[device], express=False, results=results)
+    kw = {}
+    if init is not None:
+        body, initargs, module = init
+        if module is not None and body not in registry.body_names():
+            registry.register_module(body, *module)
+        kw = {"initializer": _initializer_for(body), "initargs": initargs}
+    pool = fiber_b200.Pool(1, devices=[device], express=False, results=results, **kw)
     pool.start_workers()
     proxies, segments = {}, {}
     conn.send(("ready", os.getpid()))
@@ -199,8 +216,10 @@ class ProcessResult:
 class ProcessPool:
     """One worker process per GPU slot; pull dispatch of blocks; dead workers are replaced and their blocks re-queued."""
 
-    def __init__(self, processes, devices, results="host", redispatch=True, worker_main=gpu_worker_main, block_tasks=None):
+    def __init__(self, processes, devices, results="host", redispatch=True, worker_main=gpu_worker_main, block_tasks=None,
+                 init=None):
         self._n = processes
+        self._init = init            # (initializer body, initargs, module) every worker process starts with, or None
         self._devices = list(devices)
         self._results = results
         self._redispatch = redispatch
@@ -218,7 +237,8 @@ class ProcessPool:
     # -- workers -----------------------------------------------------------------------------------------
     def _spawn(self, w):
         parent, child = self._ctx.Pipe()
-        w.proc = self._ctx.Process(target=self._worker_main, args=(w.device, child, self._results, [ROOT]), daemon=True)
+        kw = {"init": self._init} if self._init is not None else {}
+        w.proc = self._ctx.Process(target=self._worker_main, args=(w.device, child, self._results, [ROOT]), kwargs=kw, daemon=True)
         w.proc.start()
         child.close()
         w.conn, w.block, w.ready = parent, None, False

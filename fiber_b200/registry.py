@@ -21,7 +21,7 @@ from . import _abi
 _BOUND = {}  # callables that cannot carry attributes (builtins) -> body name
 
 
-def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entry=None, result=None, **meta):
+def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entry=None, result=None, shared=None, **meta):
     """Decorator: ``@device_body("pi_inside_det")`` binds ``func`` to the device body ``name`` and sets
     ``func.__fiber_meta__`` (``gpu=1`` unless overridden), like ``fiber.meta``.
 
@@ -38,7 +38,12 @@ def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entr
     A RECORD body (``FBR_EXPORT_RECORD_BODY``: any fixed-size argument and result structs) describes both records
     with NumPy dtypes: ``args`` and ``result`` take anything ``np.dtype()`` accepts, e.g. ``"<f8"`` or
     ``[("x", "<f8"), ("y", "<f8")]``, sub-array fields included.  The field names are the function's parameter
-    names; a one-field (or plain scalar) result is returned as that value, several fields as a tuple."""
+    names; a one-field (or plain scalar) result is returned as that value, several fields as a tuple.
+
+    A record body with a broadcast element (``using Shared = ...`` in its struct) also reads one array every task of a
+    map shares: ``shared=("centroids", <element dtype>)`` names the function's FIRST parameter and describes one
+    element of that array; the ``args`` fields are the parameters after it.  Tasks pass the array as that parameter, or
+    leave it out and read the block of the pool's initializer (``device_initializer``)."""
     from .meta import VALID_META_KEYS
     for k in meta:
         assert k in VALID_META_KEYS, "Invalid meta argument \"{}\"".format(k)
@@ -46,7 +51,7 @@ def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entr
     md.update(meta)
     if source is not None:
         from . import bodies
-        register_module(name, bodies.compile_module(name, source), entry, args, bits_entry, result)
+        register_module(name, bodies.compile_module(name, source), entry, args, bits_entry, result, shared)
 
     def decorator(func):
         bind(func, name, **md)
@@ -54,7 +59,8 @@ def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entr
     return decorator
 
 
-_MODULES = {}   # body name -> (module path, entry, argument layout, bits entry, result layout) of bodies registered from their own module
+_MODULES = {}   # body name -> (module path, entry, argument layout, bits entry, result layout, broadcast parameter) of bodies
+                # registered from their own module
 
 
 def module_of(name):
@@ -62,10 +68,12 @@ def module_of(name):
     return _MODULES.get(name)
 
 
-def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_entry=None, result=None):
+def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_entry=None, result=None, shared=None):
     """``fbr_register_body`` + the host-side encoder for the body's argument records (and, with ``bits_entry``, the
     body's bit-packed twin ``<name>_bits8``).  Record bodies (``FBR_BODY_RECORD``) take NumPy dtypes for ``args`` and
-    ``result``; their sizes must be the module's ``arg_bytes`` / ``result_bytes`` (``ValueError`` otherwise)."""
+    ``result``; their sizes must be the module's ``arg_bytes`` / ``result_bytes`` (``ValueError`` otherwise).
+    Broadcast bodies (``FBR_BODY_BROADCAST``) also take ``shared=(parameter name, element dtype)``, whose size must be
+    the module's element size; ``shared`` is refused for every other body (``ValueError``)."""
     import ctypes
     specs = _load_specs()           # the table as it was: the body registered below gets the encoder its layout asks for
     if bits_entry is not None:
@@ -79,7 +87,17 @@ def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_
     info = _abi.BodyInfo()
     _abi.check(L.fbr_body_info(fid.value, ctypes.byref(info)))
     record = None
-    if info.flags & _abi.FBR_BODY_RECORD:
+    if info.flags & _abi.FBR_BODY_BROADCAST:
+        if result is None or shared is None:
+            raise ValueError("broadcast body %s: pass result=<dtype> and shared=(<parameter name>, <element dtype>)" % name)
+        elem, stage = ctypes.c_uint32(0), ctypes.c_uint32(0)
+        _abi.check(L.fbr_body_shared_info(fid.value, ctypes.byref(elem), ctypes.byref(stage)))
+        record = _Broadcast(info, args, result, shared, elem.value, stage.value)   # validates all three layouts
+        args, result, shared = record.arg_dtype, record.res_dtype, (record.shared_name, record.shared_dtype)
+    elif shared is not None:
+        raise ValueError("body %s reads no broadcast block (its record struct has no Shared element type): shared= is "
+                         "for broadcast bodies only" % name)
+    elif info.flags & _abi.FBR_BODY_RECORD:
         if result is None:
             raise ValueError("record body %s: pass result=<dtype> (its %d-byte result record)" % (name, info.result_bytes))
         record = _Record(info, args, result)        # validates both layouts against the module
@@ -87,11 +105,11 @@ def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_
     elif result is not None:
         raise ValueError("body %s is not a record body (FBR_EXPORT_RECORD_BODY): its result layout is fixed" % name)
     old = specs.get(name)
-    if record is not None and isinstance(old, _Record) and (old.arg_dtype, old.res_dtype) != (record.arg_dtype, record.res_dtype):
-        raise ValueError("record body %s is registered already with args=%s, result=%s; a name keeps its layouts"
-                         % (name, old.arg_dtype, old.res_dtype))
+    if record is not None and isinstance(old, _Record) and old.layouts() != record.layouts():
+        raise ValueError("record body %s is registered already with %s; a name keeps its layouts"
+                         % (name, ", ".join("%s=%s" % kv for kv in zip(("args", "result", "shared"), old.layouts()))))
     # the engine keeps the first module registered under a name (fbr_register_body is idempotent): so do worker processes
-    _MODULES.setdefault(name, (str(module_path), entry, args, bits_entry, result))
+    _MODULES.setdefault(name, (str(module_path), entry, args, bits_entry, result, shared))
     if name not in specs:
         if record is not None:
             specs[name] = record
@@ -434,6 +452,10 @@ class _Record(BodySpec):
         self._sdt = self.arg_dtype if self.params else np.dtype([("_0", self.arg_dtype)])
         self._fields = self._sdt.names
 
+    def layouts(self):
+        """What a name keeps once registered: the argument and result dtypes."""
+        return (self.arg_dtype, self.res_dtype)
+
     # ---- arguments ------------------------------------------------------------------------------------------------
     def _fast_map_ok(self, items):
         return True
@@ -523,6 +545,125 @@ class _Record(BodySpec):
         return sum(vals.tolist())                        # Python's left-to-right sum, as over the reference's list
 
 
+def _same_bytes(a, b):
+    """Whether two arrays are the same block: equal dtype and shape and the same bytes.  Comparing values would call
+    -0.0 and +0.0 (or two NaNs with different payloads) the same while their blocks differ, and never call an array
+    holding a NaN equal to its own copy."""
+    if a.dtype != b.dtype or a.shape != b.shape:
+        return False
+    return np.array_equal(np.ascontiguousarray(a).reshape(-1).view(np.uint8), np.ascontiguousarray(b).reshape(-1).view(np.uint8))
+
+
+class _LastBlock:
+    """The broadcast block built from the last arguments, reused while new arguments compare equal to them.  A map's
+    tasks usually all pass the same array (the reference pickles it into every task message), and an exact comparison
+    with a kept copy is far cheaper than building the block again.  Returning the very same bytes object also lets
+    ``Pool`` skip fingerprinting it before the upload-cache lookup."""
+
+    def __init__(self):
+        self._last = None         # (copies of the arguments, block)
+
+    def get(self, arrays, build):
+        last = self._last
+        if last is not None and all(_same_bytes(a, b) for a, b in zip(last[0], arrays)):
+            return last[1]
+        blob = build(*arrays)
+        self._last = ([a.copy() for a in arrays], blob)
+        return blob
+
+
+def _block_bytes(a):
+    return np.ascontiguousarray(a).tobytes()
+
+
+class _Broadcast(_Record):
+    """A record body whose run() also reads the map's broadcast block (``FBR_BODY_BROADCAST``): an array of
+    ``shared_dtype`` elements that every task shares, uploaded once per worker.
+
+    The function's first parameter (``shared_name``) is that array, the argument dtype's fields are the parameters
+    after it: ``starmap(f, [(C, p0), (C, p1)])``, ``apply_async(f, (C, p))`` and ``apply_async(f, (p,), {name: C})`` pass
+    it with every task (the same array each time); ``map(f, points)`` and items without it read the pool's initializer
+    block (``Pool(initializer=<@device_initializer(body)>, initargs=(C,))``)."""
+
+    def __init__(self, info, args, result, shared, elem_bytes, stage_bytes):
+        super().__init__(info, args, result)
+        if not (isinstance(shared, (tuple, list)) and len(shared) == 2 and isinstance(shared[0], str) and shared[0].isidentifier()):
+            raise ValueError("%s: shared= is (<parameter name>, <element dtype>), got %r" % (self.name, shared))
+        self.shared_name = shared[0]
+        if self.params is not None and self.shared_name in self.params:
+            raise ValueError("%s: the broadcast parameter %r is also an argument field" % (self.name, self.shared_name))
+        self.shared_dtype = _record_dtype(shared[1], "broadcast element", self.name)
+        if self.shared_dtype.itemsize != elem_bytes:
+            raise ValueError("%s: broadcast element dtype %s is %d bytes, the body's Shared element is %d"
+                             % (self.name, self.shared_dtype, self.shared_dtype.itemsize, elem_bytes))
+        self.elem_bytes, self.stage_bytes = elem_bytes, stage_bytes
+        # the element as a plain array's trailing shape and base type: (K, 16) float32 for ("c", "<f4", (16,))
+        d = self.shared_dtype
+        if d.names is not None and len(d.names) == 1:
+            d = d.fields[d.names[0]][0]
+        self._plain = (d.subdtype[0], d.subdtype[1]) if d.subdtype is not None else (d, ())
+        self._blocks = _LastBlock()
+
+    def layouts(self):
+        return (self.arg_dtype, self.res_dtype, (self.shared_name, self.shared_dtype))
+
+    def _block_array(self, x):
+        """The broadcast array as a contiguous array of elements: exactly the element dtype (1-D), or a plain array whose
+        trailing shape and base type are the element's (viewed, not converted)."""
+        a = np.asarray(x)
+        base, shape = self._plain
+        if a.dtype == self.shared_dtype and a.ndim == 1:
+            pass
+        elif a.dtype == base and a.ndim == 1 + len(shape) and a.shape[1:] == shape:
+            if self.shared_dtype.names is not None and len(a):
+                # the same elements as a 1-D array of the element dtype (a view when `a` is contiguous), so a plain array
+                # and its structured twin find the same kept block
+                a = np.ascontiguousarray(a).reshape(len(a), -1).view(self.shared_dtype).reshape(len(a))
+        else:
+            raise TypeError("%s: %s must be a 1-D array of %s or an array of shape (n,) + %s and dtype %s, got shape %s "
+                            "and dtype %s" % (self.name, self.shared_name, self.shared_dtype, shape, base, a.shape, a.dtype))
+        if len(a) == 0:
+            raise ValueError("%s: %s is empty; the broadcast block needs at least one element" % (self.name, self.shared_name))
+        return a
+
+    def shared_block(self, *initargs):
+        """The broadcast block of ``initializer(array)``: the array's bytes, kept while later arrays compare equal."""
+        if len(initargs) != 1:
+            raise TypeError("%s: the initializer takes exactly one argument (%s), got %d" % (self.name, self.shared_name, len(initargs)))
+        return self._blocks.get((self._block_array(initargs[0]),), _block_bytes)
+
+    def _encode(self, items, fast, apply=False):
+        if fast:
+            return super()._encode(items, fast)              # map(f, points): the block is the initializer's
+        n_params = len(self._fields)
+        rows, first, block, carried = [], None, None, None      # first: the first item's array; block: its element view
+        for it in items:
+            args, kwds = self._split(it, apply)
+            if self.shared_name in kwds:
+                kwds = dict(kwds)
+                b = kwds.pop(self.shared_name)
+            elif args and len(args) + len(kwds) > n_params:    # one more argument than the record has fields
+                b, args = args[0], tuple(args[1:])
+            else:
+                b = _MISSING
+            has = b is not _MISSING
+            if carried is None:
+                carried = has
+            elif carried != has:
+                raise TypeError("%s: mixed items with and without %s in one map" % (self.name, self.shared_name))
+            if has:
+                # the same object as the first item's: nothing to check; else the same elements, byte for byte, in
+                # either of the accepted forms (C and C["c"] are one block)
+                if first is None:
+                    first, block = b, self._block_array(b)
+                elif b is not first and not _same_bytes(self._block_array(b), block):
+                    raise ValueError("%s: all tasks of one map must share %s" % (self.name, self.shared_name))
+            rows.append(self._bind(args, kwds))
+        enc = self._columns([list(c) for c in zip(*rows)] if rows else [[] for _ in self._fields])
+        enc.shared = self._blocks.get((block,), _block_bytes) if block is not None else None
+        return enc
+
+
 class _SleepF64(BodySpec):
     def _fast_map_ok(self, items):
         return True
@@ -553,21 +694,14 @@ class _Parzen(BodySpec):
     def __init__(self, info, elem):
         super().__init__(info)
         self.elem = np.dtype(elem)
+        self._blocks = _LastBlock()
 
     def shared_block(self, x_samples, point_x):
         """The broadcast block for (x_samples, point_x).  The reference pickles both into every one of its task
         messages; the example submits 102 ``apply_async`` calls with the same arrays, so the last block is kept
         and reused when the arguments compare equal (an exact memcmp of 160 KB, ~10 us, instead of casting and
         serialising them again)."""
-        xs = np.asarray(x_samples)
-        px = np.asarray(point_x)
-        last = getattr(self, "_last_block", None)
-        if last is not None and last[0].shape == xs.shape and last[1].shape == px.shape and last[0].dtype == xs.dtype \
-                and np.array_equal(last[0], xs) and np.array_equal(last[1], px):
-            return last[2]
-        blob = self._build_block(xs, px)
-        self._last_block = (xs.copy(), px.copy(), blob)
-        return blob
+        return self._blocks.get((np.asarray(x_samples), np.asarray(point_x)), self._build_block)
 
     def _build_block(self, xs, px):
         if xs.ndim != 2 or px.ndim != 2 or px.shape[0] != xs.shape[1]:

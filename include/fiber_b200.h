@@ -70,7 +70,9 @@ typedef enum fbr_result_kind {
 #define FBR_BODY_RECORD 0x10u     /* argument and result records are staged through shared memory by dispatch_record_kernel
                                      (FBR_EXPORT_RECORD_BODY): arg_bytes and result_bytes are any multiples of 4 up to
                                      4096, arg_stride any multiple of 4 >= arg_bytes; result kind FBR_RES_BYTES, not
-                                     SUMMABLE, not NEEDS_SHARED, no bit-packed twin */
+                                     SUMMABLE, no bit-packed twin; NEEDS_SHARED only together with BROADCAST */
+#define FBR_BODY_BROADCAST 0x20u  /* record body whose run() receives the map's broadcast block as an array of its
+                                     Shared element type (fbr_body_shared_info); always set with NEEDS_SHARED */
 
 typedef struct fbr_body_info {
     int32_t func_id;
@@ -96,7 +98,7 @@ int fbr_body_lookup(const char* name, int* func_id);
  * (func_id >= the compiled-in count; the same name may be registered once).  The module's launch routine
  * receives the same wave parameters as the compiled-in kernels, so registered bodies run in the same
  * persistent-CTA dispatch kernels (direct placement, ring + gather_ordered, resilient re-dispatch). */
-#define FBR_BODY_MODULE_ABI 1
+#define FBR_BODY_MODULE_ABI 2
 typedef struct fbr_body_module {
     uint32_t abi;               /* FBR_BODY_MODULE_ABI */
     uint32_t wave_params_bytes; /* sizeof(fbr::WaveParams) the module was compiled against */
@@ -104,9 +106,16 @@ typedef struct fbr_body_module {
     uint32_t arg_bytes, result_bytes, result_kind, flags, unit_tasks;
     void (*launch)(const void* wave_params, int grid, void* cuda_stream);
     int (*occupancy)(int index_mode);   /* resident CTAs per SM on the current device */
+    /* FBR_BODY_BROADCAST record bodies: sizeof(Shared) (a multiple of 4 up to 4096) and the body's shared-memory
+       budget for the block (a multiple of 16; 0 = always read it from global memory).  0, 0 for every other body */
+    uint32_t shared_elem_bytes, shared_stage_bytes;
 } fbr_body_module_t;
 typedef const fbr_body_module_t* (*fbr_body_entry_fn)(void);
 int fbr_register_body(const char* name, const char* module_path, const char* entry, int* func_id);
+/* Broadcast element size and staging budget of a FBR_BODY_BROADCAST body (0, 0 for other bodies).  A map of such a body
+ * passes a block of shared_bytes > 0, a multiple of elem_bytes; blocks up to stage_bytes are staged into shared memory
+ * once per CTA, larger ones are read from global memory. */
+int fbr_body_shared_info(int func_id, uint32_t* elem_bytes, uint32_t* stage_bytes);
 
 /* ---- pool lifecycle -------------------------------------------------------------------------
  * fbr_pool_create   <- ZPool.__init__ (fiber/pool.py:888-943) + worker start
@@ -172,7 +181,9 @@ typedef struct fbr_map_desc {
     const void* args;        /* n_tasks records of arg_stride bytes (host, ideally pinned; or device) */
     int64_t index_start;     /* implicit argument of task i = index_start + i*index_step (range()) */
     int64_t index_step;
-    const void* shared;      /* broadcast argument block (e.g. parzen samples), may be NULL */
+    const void* shared;      /* broadcast argument block (e.g. parzen samples), may be NULL.  A FBR_ARGS_DEVICE block may
+                                start at any address: one that is not 16 B aligned is read in place only when a broadcast
+                                body stages it into shared memory, else from an aligned device copy made per map */
     uint64_t shared_bytes;
     void* out;               /* NULL: engine-owned pinned result segment; else n_tasks*result_bytes */
     uint64_t task_index_base;/* global index of task 0 (sharded maps: rank's block start) */

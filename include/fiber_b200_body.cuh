@@ -43,6 +43,25 @@
 // args=[("x", "<f8"), ("y", "<f8")], result=[("r2", "<f8"), ("r", "<f8")]) -- the NumPy dtypes describe the
 // two structs byte for byte (INTEGRATION.md).  Record bodies cannot fold sums on the device and have no
 // bit-packed twin.
+//
+// A record body may also read one array every task of a map shares (the pool initializer's initargs, or the same array
+// in every task tuple): it declares the array's element type and a shared-memory budget, and run() gets the block
+// after the result:
+//
+//     struct NearestCentroid {
+//         struct Arg { float p[16]; }; struct Res { uint32_t k; float d2; };
+//         struct Centroid { float c[16]; };
+//         using Shared = Centroid;                        // trivially copyable, sizeof a multiple of 4, at most 4096
+//         static constexpr uint32_t kSharedStage = 32768; // blocks up to this many bytes are staged in shared memory;
+//                                                         // with the IN / OUT stages at most 200 KB in all
+//         static constexpr bool kIndexArg = false, kCanFault = false;
+//         __device__ static void run(const Arg& a, Res& r, const fbr::Broadcast<Shared>& sh, uint64_t task_index,
+//                                    const fbr::ErrSink& es, uint32_t attempt) { ... sh.data[0 .. sh.n) ... }
+//     };
+//
+// FBR_EXPORT_RECORD_BODY then sets FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST itself.  sh.n is shared_bytes /
+// sizeof(Shared).  A block of at most kSharedStage bytes is bulk-loaded into shared memory once per CTA (sh.data points
+// there); a larger one, or any block when kSharedStage is 0, is read from global memory.
 #pragma once
 #include "fiber_b200.h"
 #include "kernels.cuh"      // fiber_b200/csrc: dispatch_thread_kernel, WaveParams, ErrSink, TaskError
@@ -157,12 +176,18 @@ constexpr bool record_body_ok() {
     static_assert(!B::kIndexArg || std::is_same<typename B::Arg, int64_t>::value, "record bodies with kIndexArg take Arg = int64_t");
     return true;
 }
+// the flags a record body's descriptor carries on top of the exported ones: broadcast bodies need a block and take it
+template <class B>
+constexpr uint32_t record_flags() {
+    return FBR_BODY_RECORD | (fbr::record::BroadcastOf<B>::kOn ? (FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST) : 0u);
+}
 }  // namespace fbr_body_export
 
 // Body: a RecordBody -- Arg and Res are trivially copyable, sizeof a multiple of 4 and at most 4096 (see the header
 // comment).  The result kind is FBR_RES_BYTES; FBR_BODY_RECORD is added to body_flags, which carry FBR_BODY_INDEX_ARG
 // exactly when Body::kIndexArg is true (a range() map of a body without the index instantiation would read no
 // arguments).  unit_tasks is the number of tasks whose records fill one shared-memory stage of dispatch_record_kernel.
+// A body with a Shared type also gets FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST and its element size and staging budget.
 #define FBR_EXPORT_RECORD_BODY(Body, body_name, entry, body_flags)                                                \
     static_assert(fbr_body_export::record_body_ok<Body>(), "record body");                                       \
     static_assert((((body_flags) & FBR_BODY_INDEX_ARG) != 0) == Body::kIndexArg,                                 \
@@ -170,9 +195,11 @@ constexpr bool record_body_ok() {
     extern "C" const fbr_body_module_t* entry(void) {                                                            \
         static const fbr_body_module_t m = {FBR_BODY_MODULE_ABI, (uint32_t)sizeof(fbr::WaveParams), body_name,   \
                                             fbr::record::Layout<Body>::A, fbr::record::Layout<Body>::R,          \
-                                            (uint32_t)FBR_RES_BYTES, (uint32_t)(body_flags) | FBR_BODY_RECORD,    \
+                                            (uint32_t)FBR_RES_BYTES,                                             \
+                                            (uint32_t)(body_flags) | fbr_body_export::record_flags<Body>(),      \
                                             fbr::record::Layout<Body>::kUnit,                                    \
-                                            fbr_body_export::launch_record<Body>, fbr_body_export::occupancy_record<Body>}; \
+                                            fbr_body_export::launch_record<Body>, fbr_body_export::occupancy_record<Body>, \
+                                            fbr::record::BroadcastOf<Body>::kElem, fbr::record::BroadcastOf<Body>::kStage}; \
         return &m;                                                                                               \
     }
 
