@@ -1481,11 +1481,28 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
         dlclose(h);
         return fail(FBR_EINVAL, "module %s: body '%s': only record bodies take a broadcast block (FBR_BODY_BROADCAST)", module_path, name);
     }
+    const uint32_t group = m->group_threads;
+    if (group > 1 && (group > 32 || (group & (group - 1)) != 0)) {
+        dlclose(h);
+        return fail(FBR_EINVAL, "module %s: body '%s': group_threads %u is not 0, 1, 2, 4, 8, 16 or 32", module_path, name, group);
+    }
+    if (group > 1 && !(m->flags & FBR_BODY_RECORD)) {
+        dlclose(h);
+        return fail(FBR_EINVAL, "module %s: body '%s': only record bodies run a task on a group of threads (group_threads %u)", module_path, name, group);
+    }
     if (m->flags & FBR_BODY_RECORD) {
-        // staged through shared memory by dispatch_record_kernel: sizes are free within its stages
+        // staged through shared memory by dispatch_record_kernel: sizes are free within its stages.  A group body's
+        // tasks must also come in 16 B-aligned groups of kAlign that fit one 32 KB stage
+        const uint32_t big = std::max(m->arg_bytes, m->result_bytes);
+        const uint32_t align = (m->arg_bytes % 16 == 0 && m->result_bytes % 16 == 0) ? 1u
+                             : (m->arg_bytes % 8 == 0 && m->result_bytes % 8 == 0) ? 2u : 4u;
         const char* why = nullptr;
         if (m->arg_bytes == 0 || m->result_bytes == 0 || m->arg_bytes % 4 || m->result_bytes % 4) why = "argument and result bytes must be non-zero multiples of 4";
-        else if (m->arg_bytes > 4096 || m->result_bytes > 4096) why = "argument and result records are at most 4096 bytes";
+        else if (group <= 1 && big > 4096) why = "argument and result records are at most 4096 bytes";
+        else if (big > 32768) why = "argument and result records of group bodies are at most 32768 bytes";
+        else if ((uint64_t)align * big > 32768)
+            why = "one 16 B-aligned group of tasks must fit a 32768-byte stage: kAlign * max(arg_bytes, result_bytes) <= 32768, "
+                  "kAlign = 1 when both sizes are multiples of 16, 2 when both are multiples of 8, else 4";
         else if (m->result_kind != FBR_RES_BYTES) why = "the result kind must be FBR_RES_BYTES (no bit-packed twin)";
         else if (m->flags & FBR_BODY_SUMMABLE) why = "results cannot be folded on the device (FBR_BODY_SUMMABLE)";
         else if ((m->flags & FBR_BODY_NEEDS_SHARED) && !bcast)

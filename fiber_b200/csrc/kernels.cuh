@@ -904,7 +904,8 @@ __global__ void __launch_bounds__(160) dispatch_payload_map_tma_kernel(const Wav
 
 // ================================================================================================
 // dispatch: record bodies (FBR_BODY_RECORD) -- any trivially copyable Arg / Res of 4..4096 bytes (multiples
-// of 4), staged through shared memory (warp-specialised, like dispatch_payload_map_tma_kernel):
+// of 4; up to 32768 for group bodies), staged through shared memory (warp-specialised, like
+// dispatch_payload_map_tma_kernel):
 //   warp 0 (one elected lane)  waits for an EMPTY IN stage, claims a unit by ticket and bulk-loads the unit's
 //                              count * A argument bytes into it (cp.async.bulk + FULL mbarrier complete_tx);
 //                              with two IN stages the next unit's load overlaps this unit's compute;
@@ -920,6 +921,8 @@ __global__ void __launch_bounds__(160) dispatch_payload_map_tma_kernel(const Wav
 // i's record starts at i * A -- a body that walks a large record word by word has every lane on the same bank
 // (A = 1024: 32-way); reading it in 16 B vectors cuts that to 8-way.  A stage holds kStageBytes of the larger
 // record, so for large records most consumers are idle during B::run (A = 1024: 32 tasks per unit).
+// Group bodies (kGroup = G) answer both: G lanes run each task (run_group_unit), reading consecutive words of one
+// record, and their records may fill a whole stage (32 KB, one task per unit).
 // Bodies with a Shared element type also receive the map's broadcast block: one within the body's kSharedStage is
 // bulk-loaded once per CTA into a region after the stages (DESIGN.md section 4 has the staged vs global measurement).
 // ================================================================================================
@@ -929,6 +932,16 @@ template <class T>
 struct Broadcast {
     const T* data;
     uint64_t n;
+};
+
+// What a group record body (kGroup = G) knows of the G threads that run each task together: G consecutive lanes of one
+// warp.  `mask` names them for __shfl_*_sync; sync() is __syncwarp over them.
+template <uint32_t G>
+struct Group {
+    uint32_t rank;                       // 0 .. G-1
+    static constexpr uint32_t size = G;
+    uint32_t mask;
+    __device__ __forceinline__ void sync() const { __syncwarp(mask); }
 };
 
 namespace record {
@@ -955,15 +968,31 @@ struct BroadcastOf<B, std::void_t<typename B::Shared>> {
     static_assert(kStage % 16 == 0, "broadcast bodies: kSharedStage is a multiple of 16 (0: never stage)");
 };
 
+// A record body opts into groups with `static constexpr uint32_t kGroup = G;` (G = 2, 4, 8, 16 or 32): G threads run
+// each task, and its run() takes a const Group<G>& after the result (after the broadcast block, if it has one).
+template <class B, class = void>
+struct GroupOf {
+    static constexpr uint32_t kG = 1;
+};
+template <class B>
+struct GroupOf<B, std::void_t<decltype(B::kGroup)>> {
+    static constexpr uint32_t kG = B::kGroup;
+    static_assert(kG == 2 || kG == 4 || kG == 8 || kG == 16 || kG == 32, "group record bodies: kGroup is 2, 4, 8, 16 or 32");
+};
+
 template <class B>
 struct Layout {
     static constexpr uint32_t A = (uint32_t)sizeof(typename B::Arg), R = (uint32_t)sizeof(typename B::Res);
-    static_assert(A % 4 == 0 && R % 4 == 0 && A >= 4 && R >= 4 && A <= 4096 && R <= 4096,
+    static_assert(GroupOf<B>::kG > 1 || (A % 4 == 0 && R % 4 == 0 && A >= 4 && R >= 4 && A <= 4096 && R <= 4096),
                   "record bodies: sizeof(Arg) and sizeof(Res) are multiples of 4 between 4 and 4096");
+    static_assert(GroupOf<B>::kG == 1 || (A % 4 == 0 && R % 4 == 0 && A >= 4 && R >= 4 && A <= kStageBytes && R <= kStageBytes),
+                  "group record bodies: sizeof(Arg) and sizeof(Res) are multiples of 4 between 4 and 32768");
     // the broadcast region after the IN / OUT stages (0 bytes for bodies without a Shared type)
     static constexpr uint32_t kShared = BroadcastOf<B>::kStage;
     // tasks per unit that make count * A and count * R multiples of 16 (A and R are multiples of 4)
     static constexpr uint32_t kAlign = ((A % 16 == 0) && (R % 16 == 0)) ? 1u : ((A % 8 == 0) && (R % 8 == 0)) ? 2u : 4u;
+    static_assert(GroupOf<B>::kG == 1 || kAlign * (A > R ? A : R) <= kStageBytes,
+                  "group record bodies: one 16 B-aligned group of tasks fits a stage (kAlign * max(sizeof(Arg), sizeof(Res)) <= 32768)");
     static constexpr uint32_t unit() {
         const uint32_t w = A > R ? A : R;
         uint32_t u = kMaxUnit;
@@ -1007,6 +1036,30 @@ __device__ __forceinline__ void gather_records(uint8_t* dst, const uint8_t* src,
     for (uint32_t w = tid; w < count * W; w += n) {
         const uint32_t i = w / W, k = w - i * W;
         reinterpret_cast<uint32_t*>(dst)[w] = *reinterpret_cast<const uint32_t*>(src + (size_t)i * stride + 4 * k);
+    }
+}
+
+// One unit of a group body (kGroup = G > 1): consumer ct is rank ct % G of group ct / G, and group g runs tasks g,
+// g + C/G, ...  All G lanes of a group see the same i, so the group stays converged through B::run.  `sh` is the
+// broadcast block of a body that has one (nothing otherwise).
+template <class B, bool kIndex, class... Sh>
+__device__ __forceinline__ void run_group_unit(const WaveParams& wp, const TaskRecord& rec, const uint8_t* in, uint8_t* out,
+                                               uint32_t ct, const ErrSink& es, const Sh&... sh) {
+    using L = Layout<B>;
+    using Arg = typename B::Arg;
+    using Res = typename B::Res;
+    constexpr uint32_t G = GroupOf<B>::kG, C = kConsumers;
+    const uint32_t lane = ct & 31u;         // consumers start at thread 32: ct % 32 is the lane
+    const Group<G> grp{ct % G, (G == 32 ? 0xffffffffu : ((1u << G) - 1u) << (lane & ~(G - 1u)))};
+    const uint64_t g0 = wp.index_base + rec.first;
+    for (uint32_t i = ct / G; i < rec.count; i += C / G) {
+        Res& r = *reinterpret_cast<Res*>(out + (size_t)i * L::R);
+        if constexpr (kIndex) {
+            const Arg a = (Arg)(wp.index_start + (int64_t)(rec.first + i) * wp.index_step);
+            B::run(a, r, sh..., grp, g0 + i, es, rec.attempt);
+        } else {
+            B::run(*reinterpret_cast<const Arg*>(in + (size_t)i * L::A), r, sh..., grp, g0 + i, es, rec.attempt);
+        }
     }
 }
 }  // namespace record
@@ -1127,7 +1180,9 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
         int* const unit_fault = &s_fault[seq & 1];
         const ErrSink es{wp.err_word, unit_fault};
         const uint64_t g0 = wp.index_base + rec.first;
-        if constexpr (!Bc::kOn) {
+        if constexpr (!Bc::kOn && record::GroupOf<B>::kG > 1) {
+            record::run_group_unit<B, kIndex>(wp, rec, in, out, ct, es);
+        } else if constexpr (!Bc::kOn) {
             for (uint32_t i = ct; i < rec.count; i += C) {
                 Res& r = *reinterpret_cast<Res*>(out + (size_t)i * L::R);
                 if constexpr (kIndex) {
@@ -1141,13 +1196,17 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
             using T = typename Bc::T;
             // one loop per placement of the block, so each sees its pointer's address space (shared or global loads)
             auto run_unit = [&](const Broadcast<T>& sh) {
-                for (uint32_t i = ct; i < rec.count; i += C) {
-                    Res& r = *reinterpret_cast<Res*>(out + (size_t)i * L::R);
-                    if constexpr (kIndex) {
-                        const Arg a = (Arg)(wp.index_start + (int64_t)(rec.first + i) * wp.index_step);
-                        B::run(a, r, sh, g0 + i, es, rec.attempt);
-                    } else {
-                        B::run(*reinterpret_cast<const Arg*>(in + (size_t)i * L::A), r, sh, g0 + i, es, rec.attempt);
+                if constexpr (record::GroupOf<B>::kG > 1) {
+                    record::run_group_unit<B, kIndex>(wp, rec, in, out, ct, es, sh);
+                } else {
+                    for (uint32_t i = ct; i < rec.count; i += C) {
+                        Res& r = *reinterpret_cast<Res*>(out + (size_t)i * L::R);
+                        if constexpr (kIndex) {
+                            const Arg a = (Arg)(wp.index_start + (int64_t)(rec.first + i) * wp.index_step);
+                            B::run(a, r, sh, g0 + i, es, rec.attempt);
+                        } else {
+                            B::run(*reinterpret_cast<const Arg*>(in + (size_t)i * L::A), r, sh, g0 + i, es, rec.attempt);
+                        }
                     }
                 }
             };

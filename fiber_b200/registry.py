@@ -43,7 +43,12 @@ def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entr
     A record body with a broadcast element (``using Shared = ...`` in its struct) also reads one array every task of a
     map shares: ``shared=("centroids", <element dtype>)`` names the function's FIRST parameter and describes one
     element of that array; the ``args`` fields are the parameters after it.  Tasks pass the array as that parameter, or
-    leave it out and read the block of the pool's initializer (``device_initializer``)."""
+    leave it out and read the block of the pool's initializer (``device_initializer``).
+
+    A GROUP record body (``static constexpr uint32_t kGroup = G;`` in its struct, G = 2, 4, 8, 16 or 32) runs each task on
+    G lanes of one warp, and its records may reach 32 KB (INTEGRATION.md has the size rules).  Nothing changes here:
+    ``kGroup`` lives in the CUDA source, and ``map(f, rows)`` over a plain ``(n, k)`` array of a one-field body with a
+    ``(k,)`` sub-array passes the rows without a copy, e.g. ``args=[("x", "<f8", (1024,))]`` for 8 KB rows."""
     from .meta import VALID_META_KEYS
     for k in meta:
         assert k in VALID_META_KEYS, "Invalid meta argument \"{}\"".format(k)
@@ -73,7 +78,9 @@ def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_
     body's bit-packed twin ``<name>_bits8``).  Record bodies (``FBR_BODY_RECORD``) take NumPy dtypes for ``args`` and
     ``result``; their sizes must be the module's ``arg_bytes`` / ``result_bytes`` (``ValueError`` otherwise).
     Broadcast bodies (``FBR_BODY_BROADCAST``) also take ``shared=(parameter name, element dtype)``, whose size must be
-    the module's element size; ``shared`` is refused for every other body (``ValueError``)."""
+    the module's element size; ``shared`` is refused for every other body (``ValueError``).  A group record body
+    (``group_threads`` > 1 in its module descriptor: several threads per task, records up to 32 KB) registers like any
+    other record body."""
     import ctypes
     specs = _load_specs()           # the table as it was: the body registered below gets the encoder its layout asks for
     if bits_entry is not None:

@@ -69,8 +69,10 @@ typedef enum fbr_result_kind {
 #define FBR_BODY_INDEX_ONLY 0x8u  /* body takes range() arguments only (arg_stride must be 0) */
 #define FBR_BODY_RECORD 0x10u     /* argument and result records are staged through shared memory by dispatch_record_kernel
                                      (FBR_EXPORT_RECORD_BODY): arg_bytes and result_bytes are any multiples of 4 up to
-                                     4096, arg_stride any multiple of 4 >= arg_bytes; result kind FBR_RES_BYTES, not
-                                     SUMMABLE, no bit-packed twin; NEEDS_SHARED only together with BROADCAST */
+                                     4096 -- up to 32768 for a group body (group_threads > 1 in its module descriptor)
+                                     whose 16 B-aligned group of tasks fits one 32 KB stage --, arg_stride any multiple
+                                     of 4 >= arg_bytes; result kind FBR_RES_BYTES, not SUMMABLE, no bit-packed twin;
+                                     NEEDS_SHARED only together with BROADCAST */
 #define FBR_BODY_BROADCAST 0x20u  /* record body whose run() receives the map's broadcast block as an array of its
                                      Shared element type (fbr_body_shared_info); always set with NEEDS_SHARED */
 
@@ -98,7 +100,7 @@ int fbr_body_lookup(const char* name, int* func_id);
  * (func_id >= the compiled-in count; the same name may be registered once).  The module's launch routine
  * receives the same wave parameters as the compiled-in kernels, so registered bodies run in the same
  * persistent-CTA dispatch kernels (direct placement, ring + gather_ordered, resilient re-dispatch). */
-#define FBR_BODY_MODULE_ABI 2
+#define FBR_BODY_MODULE_ABI 3
 typedef struct fbr_body_module {
     uint32_t abi;               /* FBR_BODY_MODULE_ABI */
     uint32_t wave_params_bytes; /* sizeof(fbr::WaveParams) the module was compiled against */
@@ -109,6 +111,10 @@ typedef struct fbr_body_module {
     /* FBR_BODY_BROADCAST record bodies: sizeof(Shared) (a multiple of 4 up to 4096) and the body's shared-memory
        budget for the block (a multiple of 16; 0 = always read it from global memory).  0, 0 for every other body */
     uint32_t shared_elem_bytes, shared_stage_bytes;
+    /* record bodies only: threads that run each task together (the body's kGroup: 2, 4, 8, 16 or 32), which lets its
+       records reach 32768 bytes (kAlign * max(arg_bytes, result_bytes) <= 32768, kAlign = 1, 2 or 4 tasks: both sizes
+       multiples of 16, of 8, or neither).  0 or 1: one thread per task */
+    uint32_t group_threads;
 } fbr_body_module_t;
 typedef const fbr_body_module_t* (*fbr_body_entry_fn)(void);
 int fbr_register_body(const char* name, const char* module_path, const char* entry, int* func_id);

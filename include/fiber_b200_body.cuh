@@ -25,7 +25,8 @@
 //
 // A ThreadBody returns a 1- or 8-byte value.  A function over other fixed-size records -- f(x: float) -> float,
 // f(x, y) -> (r, theta), a row of 256 uint32 -> a few statistics -- is a RECORD body: Arg and Res are any
-// trivially copyable structs (sizeof a multiple of 4, at most 4096 bytes), and run() writes the result in place:
+// trivially copyable structs (sizeof a multiple of 4, at most 4096 bytes; a group body below may reach 32 KB), and
+// run() writes the result in place:
 //
 //     struct Polar {
 //         struct Arg { double x, y; }; struct Res { double r2, r; };
@@ -62,6 +63,34 @@
 // FBR_EXPORT_RECORD_BODY then sets FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST itself.  sh.n is shared_bytes /
 // sizeof(Shared).  A block of at most kSharedStage bytes is bulk-loaded into shared memory once per CTA (sh.data points
 // there); a larger one, or any block when kSharedStage is 0, is read from global memory.
+//
+// A GROUP record body runs each task on G threads of one warp (G = 2, 4, 8, 16 or 32): the lanes of a group read
+// consecutive words of one record (no shared-memory bank conflicts) and reduce with shuffles, and its records may reach
+// 32 KB.  It declares kGroup, and run() gets a const fbr::Group<G>& after the result (after the broadcast block, if any):
+//
+//     struct RowSum {
+//         struct Arg { double x[1024]; }; struct Res { double s; uint32_t pad[2]; };
+//         static constexpr uint32_t kGroup = 32;
+//         static constexpr bool kIndexArg = false, kCanFault = false;
+//         __device__ static void run(const Arg& a, Res& r, const fbr::Group<32>& g, uint64_t task_index,
+//                                    const fbr::ErrSink& es, uint32_t attempt) {
+//             double s = 0.0;
+//             for (uint32_t k = g.rank; k < 1024; k += g.size) s = __dadd_rn(s, a.x[k]);
+//             for (uint32_t o = g.size / 2; o > 0; o >>= 1) s = __dadd_rn(s, __shfl_xor_sync(g.mask, s, o));
+//             if (g.rank == 0) r.s = s;
+//         }
+//     };
+//
+// g.rank is 0 .. G-1, g.size is G, g.mask is the group's lanes within its warp (for __shfl_*_sync), g.sync() is
+// __syncwarp(g.mask).  The contract:
+//   - all G threads call run() for the same task, with the same a, r, task_index and attempt;
+//   - a and r are in shared memory, and any thread may write any part of r;
+//   - every thread of the group reaches the same collective calls (shuffles, g.sync());
+//   - a fault reported through es by any thread marks the task's unit, as for a one-thread body.
+// Sizes: sizeof(Arg) and sizeof(Res) are multiples of 4 up to 32768, and kAlign * max(sizeof(Arg), sizeof(Res)) <= 32768,
+// where kAlign (fbr::record::Layout<B>::kAlign) is 1 when both sizes are multiples of 16, 2 when both are multiples of
+// 8, else 4: records that are multiples of 16 may reach 32 KB, multiples of 8 16 KB, any other pair 8 KB.  A body
+// without kGroup is a one-thread body with records up to 4096 bytes.  FBR_EXPORT_RECORD_BODY checks all of this.
 #pragma once
 #include "fiber_b200.h"
 #include "kernels.cuh"      // fiber_b200/csrc: dispatch_thread_kernel, WaveParams, ErrSink, TaskError
@@ -181,13 +210,19 @@ template <class B>
 constexpr uint32_t record_flags() {
     return FBR_BODY_RECORD | (fbr::record::BroadcastOf<B>::kOn ? (FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST) : 0u);
 }
+// the descriptor's group_threads: kGroup of a group body, 0 for a one-thread body
+template <class B>
+constexpr uint32_t record_group() {
+    return fbr::record::GroupOf<B>::kG > 1 ? fbr::record::GroupOf<B>::kG : 0u;
+}
 }  // namespace fbr_body_export
 
-// Body: a RecordBody -- Arg and Res are trivially copyable, sizeof a multiple of 4 and at most 4096 (see the header
-// comment).  The result kind is FBR_RES_BYTES; FBR_BODY_RECORD is added to body_flags, which carry FBR_BODY_INDEX_ARG
-// exactly when Body::kIndexArg is true (a range() map of a body without the index instantiation would read no
-// arguments).  unit_tasks is the number of tasks whose records fill one shared-memory stage of dispatch_record_kernel.
-// A body with a Shared type also gets FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST and its element size and staging budget.
+// Body: a RecordBody -- Arg and Res are trivially copyable, sizeof a multiple of 4 and at most 4096, or 32768 for a group
+// body within one stage (see the header comment).  The result kind is FBR_RES_BYTES; FBR_BODY_RECORD is added to
+// body_flags, which carry FBR_BODY_INDEX_ARG exactly when Body::kIndexArg is true (a range() map of a body without the
+// index instantiation would read no arguments).  unit_tasks is the number of tasks whose records fill one shared-memory
+// stage of dispatch_record_kernel.  A body with a Shared type also gets FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST and
+// its element size and staging budget; a body with kGroup gets group_threads = kGroup.
 #define FBR_EXPORT_RECORD_BODY(Body, body_name, entry, body_flags)                                                \
     static_assert(fbr_body_export::record_body_ok<Body>(), "record body");                                       \
     static_assert((((body_flags) & FBR_BODY_INDEX_ARG) != 0) == Body::kIndexArg,                                 \
@@ -199,7 +234,8 @@ constexpr uint32_t record_flags() {
                                             (uint32_t)(body_flags) | fbr_body_export::record_flags<Body>(),      \
                                             fbr::record::Layout<Body>::kUnit,                                    \
                                             fbr_body_export::launch_record<Body>, fbr_body_export::occupancy_record<Body>, \
-                                            fbr::record::BroadcastOf<Body>::kElem, fbr::record::BroadcastOf<Body>::kStage}; \
+                                            fbr::record::BroadcastOf<Body>::kElem, fbr::record::BroadcastOf<Body>::kStage, \
+                                            fbr_body_export::record_group<Body>()};                              \
         return &m;                                                                                               \
     }
 
