@@ -18,8 +18,9 @@ FBR_OK, FBR_EINVAL, FBR_ECUDA, FBR_ENOMEM, FBR_ESTATE, FBR_ETIMEOUT, FBR_ETASK, 
 # fbr_result_kind
 FBR_RES_BYTES, FBR_RES_BOOL, FBR_RES_I64, FBR_RES_U32, FBR_RES_F64X2, FBR_RES_NONE, FBR_RES_BITS8 = range(7)
 # body flags
-FBR_BODY_INDEX_ARG, FBR_BODY_NEEDS_SHARED, FBR_BODY_SUMMABLE, FBR_BODY_INDEX_ONLY, FBR_BODY_RECORD, FBR_BODY_BROADCAST = \
-    0x1, 0x2, 0x4, 0x8, 0x10, 0x20
+FBR_BODY_INDEX_ARG, FBR_BODY_NEEDS_SHARED, FBR_BODY_SUMMABLE, FBR_BODY_INDEX_ONLY, FBR_BODY_RECORD, FBR_BODY_BROADCAST, \
+    FBR_BODY_ITEMS = 0x1, 0x2, 0x4, 0x8, 0x10, 0x20, 0x40
+FBR_BODY_MODULE_ABI = 4
 # pool flags
 FBR_POOL_TIMING, FBR_POOL_OVERLAP = 0x1, 0x2
 # map flags
@@ -33,9 +34,10 @@ FBR_TASK_OK, FBR_TASK_OVERFLOW, FBR_TASK_BADARG, FBR_TASK_FAULT = range(4)
 SYMBOLS = [
     "fbr_abi_version", "fbr_last_error", "fbr_device_count",
     "fbr_body_count", "fbr_body_info", "fbr_body_lookup", "fbr_register_body", "fbr_body_shared_info",
+    "fbr_body_items_info",
     "fbr_pool_create", "fbr_pool_close", "fbr_pool_terminate", "fbr_pool_join", "fbr_pool_destroy",
     "fbr_pool_n_workers", "fbr_pool_worker_device",
-    "fbr_map_submit", "fbr_shared_put", "fbr_shared_drop", "fbr_plan_query",
+    "fbr_map_submit", "fbr_map_submit_items", "fbr_shared_put", "fbr_shared_drop", "fbr_plan_query",
     "fbr_result_wait", "fbr_result_poll", "fbr_result_data", "fbr_result_fetch", "fbr_result_release",
     "fbr_host_alloc", "fbr_host_free", "fbr_device_alloc", "fbr_device_free",
     "fbr_memcpy_h2d", "fbr_memcpy_d2h", "fbr_payload_fill_device",
@@ -74,6 +76,11 @@ class MapDesc(ctypes.Structure):
                 ("shared", ctypes.c_void_p), ("shared_bytes", ctypes.c_uint64), ("out", ctypes.c_void_p),
                 ("task_index_base", ctypes.c_uint64), ("shuffle_seed", ctypes.c_uint64), ("n_items", ctypes.c_uint64),
                 ("attempt", ctypes.c_uint32), ("pad", ctypes.c_uint32)]
+
+
+class ItemsDesc(ctypes.Structure):
+    _fields_ = [("items", ctypes.c_void_p), ("offsets", ctypes.c_void_p), ("n_items", ctypes.c_uint64),
+                ("item_bytes", ctypes.c_uint32), ("pad", ctypes.c_uint32)]
 
 
 class Plan(ctypes.Structure):
@@ -138,6 +145,7 @@ def load():
         "fbr_body_lookup": (i32, [ctypes.c_char_p, P(i32)]),
         "fbr_register_body": (i32, [ctypes.c_char_p, ctypes.c_char_p, ctypes.c_char_p, P(i32)]),
         "fbr_body_shared_info": (i32, [i32, P(u32), P(u32)]),
+        "fbr_body_items_info": (i32, [i32, P(u32)]),
         "fbr_pool_create": (i32, [i32, P(i32), u64, u32, P(vp)]),
         "fbr_pool_close": (i32, [vp]),
         "fbr_pool_terminate": (i32, [vp]),
@@ -146,6 +154,7 @@ def load():
         "fbr_pool_n_workers": (i32, [vp, P(i32)]),
         "fbr_pool_worker_device": (i32, [vp, i32, P(i32)]),
         "fbr_map_submit": (i32, [vp, P(MapDesc), P(u64)]),
+        "fbr_map_submit_items": (i32, [vp, P(MapDesc), P(ItemsDesc), P(u64)]),
         "fbr_shared_put": (i32, [vp, vp, u64, P(u64)]),
         "fbr_shared_drop": (i32, [vp, u64]),
         "fbr_plan_query": (i32, [i32, u64, u32, u64, i32, i32, i32, P(Plan)]),

@@ -182,6 +182,7 @@ struct BodyEntry {
     int max_ctas_per_sm = 0;   // 0 = as many as fit; streaming read+write bodies run best with few, fat streams
     void* module = nullptr;    // dlopen handle of a registered body (never closed: kernels may be in flight)
     uint32_t shared_elem_bytes = 0, shared_stage_bytes = 0;   // FBR_BODY_BROADCAST record bodies
+    uint32_t item_bytes = 0;                                  // FBR_BODY_ITEMS record bodies
 };
 
 static std::mutex g_body_mu;
@@ -265,6 +266,7 @@ struct Worker {
     SlotHeader* d_headers = nullptr;   // kRecCapacity
     uint8_t* d_ring = nullptr;         // result ring arena (ring_bytes)
     uint8_t* d_args[2] = {nullptr, nullptr};
+    uint8_t* d_items[2] = {nullptr, nullptr};   // items bodies, host-resident items: a wave's offsets slice, then its item span
     uint8_t* d_out[2] = {nullptr, nullptr};
     uint32_t* d_tickets = nullptr;
     SeqCtrl* d_ctrl = nullptr;
@@ -299,6 +301,8 @@ struct PartCtx {                          // constants of one worker's block of 
                                           // out-staging halves and PUSHED there by this worker's copy engine (the D2H machinery)
     bool peer_push = false;               // arguments live on worker 0 (another GPU): worker 0's copy engine PUSHES each wave's
                                           // records into this worker's staging halves over NVLink (host_args machinery)
+    bool host_items = false;              // items bodies, host-resident items, not resilient: each wave copies its offsets slice
+                                          // and item span into the worker's d_items staging half
     bool direct = false;                  // contiguous, unshuffled, non-resilient block: the dispatch kernel stores every
                                           // unit at its final index (no ring, no task records, no gather launch)
     const uint8_t* d_shared = nullptr;
@@ -306,6 +310,10 @@ struct PartCtx {                          // constants of one worker's block of 
     const uint8_t* args_full = nullptr;   // device-resident arguments of the whole map (args_dev / resilient)
     uint64_t wave_tasks_cap = 0;
     uint64_t args_limit_bytes = 0;        // host arguments end here (n_items records); 0 = n_tasks * arg_stride
+    // items bodies: where the kernel finds the part's items and offsets for the whole map (WaveParams::items ...)
+    const uint8_t* items = nullptr;
+    const uint64_t* item_offs = nullptr;
+    uint64_t item_first = 0, item_base = 0, item_count = 0;
 };
 
 struct SeqPart {
@@ -319,6 +327,8 @@ struct SeqPart {
     void* d_shared_tmp = nullptr;         // per-seq device copy of a host shared block
     void* d_window = nullptr;             // FULL_WINDOW device output
     void* d_args_full = nullptr;          // resilient: device copy of all argument records
+    void* d_items = nullptr;              // items bodies with host-resident items: the part's item span ...
+    void* d_item_offs = nullptr;          // ... and its count + 1 offsets, on the device for the part's whole life
     LostUnit* d_lost = nullptr;           // resilient: units whose worker "died" (filled by gather)
     LostUnit* h_lost = nullptr;           // pinned mirror
     uint32_t lost_cap = 0, attempt = 0;
@@ -343,6 +353,7 @@ struct SeqState {
     uint32_t n_waves = 0;
     uint32_t redispatched_units = 0;
     fbr_map_desc_t desc;
+    fbr_items_desc_t items;                // items bodies (fbr_map_submit_items); zero otherwise
     std::vector<SeqPart> parts;
     std::vector<SeqPart> graveyard;        // parts that were running on a worker when it died (their blocks were re-dispatched)
     int waiters = 0;                       // threads inside fbr_result_wait for this seq (they hold event handles outside the lock)
@@ -602,6 +613,7 @@ static void worker_destroy(Worker& w) {
     cudaFree(w.d_ring);
     for (int i = 0; i < 2; ++i) {
         cudaFree(w.d_args[i]);
+        cudaFree(w.d_items[i]);
         cudaFree(w.d_out[i]);
     }
     cudaFree(w.d_tickets);
@@ -634,7 +646,7 @@ static uint32_t pick_unit_record(const BodyEntry& b, uint32_t chunksize, uint64_
     const uint64_t per_task = std::max(b.result_bytes, b.arg_bytes);
     while (pref > 1 && (uint64_t)pref * per_task > ring_bytes / 2) pref >>= 1;
     while (pref > 256 && (uint64_t)pref * (uint64_t)sm_count > n_tasks) pref >>= 1;
-    const uint32_t ar = 16u / gcd_u32(16u, b.result_bytes), aa = 16u / gcd_u32(16u, b.arg_bytes);
+    const uint32_t ar = 16u / gcd_u32(16u, b.result_bytes), aa = b.arg_bytes ? 16u / gcd_u32(16u, b.arg_bytes) : 1u;
     const uint32_t align = ar / gcd_u32(ar, aa) * aa;                       // lcm of two powers of two
     uint32_t unit = pref;
     if (chunksize <= pref) {
@@ -699,7 +711,7 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
     // nothing in (computed records, range() or device-resident arguments) skips the hop through s_in -- every
     // cross-stream event costs the GPU a few microseconds per wave -- except the first wave of a block, which
     // has to see the control block (and shared block) its submit_part put on s_in.
-    const bool in_copies = have_records || cx.host_args || part.first_wave_pending;
+    const bool in_copies = have_records || cx.host_args || cx.host_items || part.first_wave_pending;
     part.first_wave_pending = false;
     if (in_copies) {
         CK(cudaStreamWaitEvent(w.s_in, w.ev_comp[rw], 0));  // wave wno-4 kernels done (device window free)
@@ -742,6 +754,22 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
             STAT_ADD(p, h2d_bytes, bytes);
         }
         wave_args = w.d_args[half];
+    }
+    // items of a streaming wave: its wt + 1 offsets at the start of the staging half, its item span 256 B further on
+    const uint8_t* wave_items = cx.items;
+    const uint64_t* wave_offs = cx.item_offs;
+    uint64_t item_first = cx.item_first, item_base = cx.item_base, item_count = cx.item_count;
+    if (cx.host_items) {
+        const fbr_items_desc_t& it = st.items;
+        const uint64_t lo = it.offsets[wave_first], hi = it.offsets[wave_first + wt];
+        const uint64_t obytes = (wt + 1) * sizeof(uint64_t), ioff = round_up(obytes, 256), ibytes = (hi - lo) * it.item_bytes;
+        CK(cudaMemcpyAsync(w.d_items[half], it.offsets + wave_first, obytes, cudaMemcpyHostToDevice, w.s_in));
+        if (ibytes)
+            CK(cudaMemcpyAsync(w.d_items[half] + ioff, (const uint8_t*)it.items + lo * it.item_bytes, ibytes, cudaMemcpyHostToDevice, w.s_in));
+        STAT_ADD(p, h2d_bytes, obytes + ibytes);
+        wave_offs = (const uint64_t*)w.d_items[half];
+        wave_items = w.d_items[half] + ioff;
+        item_first = wave_first; item_base = lo; item_count = hi;
     }
     if (in_copies) CK(cudaEventRecord(w.ev_rec_h2d[rw], w.s_in));
 
@@ -792,6 +820,11 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
     wp.syn_func = (uint32_t)st.func_id;
     wp.syn_attempt = part.attempt;
     wp.n_items = d.n_items ? d.n_items : ~0ull;
+    wp.items = wave_items;
+    wp.item_offs = wave_offs;
+    wp.item_first = item_first;
+    wp.item_base = item_base;
+    wp.item_count = item_count;
     int occ_d = worker_occ(w, st.func_id, body, d.arg_stride == 0);
     if (body.max_ctas_per_sm) occ_d = std::min(occ_d, body.max_ctas_per_sm);
     if (ov && occ_d > 1) occ_d -= 1;     // leave SM slots for the concurrently running gather CTAs
@@ -1061,6 +1094,33 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
         cx.args_full = (const uint8_t*)part.d_args_full;
     }
 
+    // items: device-resident ones are read in place.  Host-resident ones (offsets checked by fbr_map_submit_items) stream
+    // wave by wave through the worker's d_items staging halves (run_wave); a resilient map may re-dispatch any unit at
+    // any time, so it copies its part's whole item span and count + 1 offsets to the device once, like d_args_full
+    if (body.flags & FBR_BODY_ITEMS) {
+        const fbr_items_desc_t& it = st.items;
+        if (cx.args_dev) {
+            cx.items = (const uint8_t*)it.items;
+            cx.item_offs = it.offsets;
+            cx.item_first = 0; cx.item_base = 0; cx.item_count = it.n_items;
+        } else if (!cx.resilient) {
+            cx.host_items = true;
+            for (int i = 0; i < 2; ++i)
+                if (!w.d_items[i]) CK(cudaMalloc((void**)&w.d_items[i], p->ring_bytes));
+        } else {
+            const uint64_t lo = it.offsets[part.first], hi = it.offsets[part.first + part.count];
+            const uint64_t ibytes = (hi - lo) * it.item_bytes, obytes = (part.count + 1) * sizeof(uint64_t);
+            CK(cudaMallocAsync(&part.d_items, std::max<uint64_t>(16, ibytes), w.s_in));
+            CK(cudaMallocAsync(&part.d_item_offs, obytes, w.s_in));
+            if (ibytes) CK(cudaMemcpyAsync(part.d_items, (const uint8_t*)it.items + lo * it.item_bytes, ibytes, cudaMemcpyHostToDevice, w.s_in));
+            CK(cudaMemcpyAsync(part.d_item_offs, it.offsets + part.first, obytes, cudaMemcpyHostToDevice, w.s_in));
+            STAT_ADD(p, h2d_bytes, ibytes + obytes);
+            cx.items = (const uint8_t*)part.d_items;
+            cx.item_offs = (const uint64_t*)part.d_item_offs;
+            cx.item_first = part.first; cx.item_base = lo; cx.item_count = hi;
+        }
+    }
+
     // Opt-in (FBR_POOL_OVERLAP): gather(w) runs on a second, higher-priority stream while the next
     // wave's / next map's dispatch kernel computes; the ring is then used in alternating halves.
     // On the pi map (ALU-bound dispatch + HBM-bound gather) the gather is a small share of the step and the
@@ -1085,8 +1145,12 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
     cx.wave_tasks_cap = units_cap * unit;
     // Host-resident output: cut large maps into ~8 waves (>= 8 MiB of results each) so the D2H of
     // wave w overlaps the kernels of wave w+1 instead of trailing one monolithic launch.
-    if (!cx.full_window || cx.host_args) {
-        const uint64_t bytes_per_task = std::max<uint64_t>(R, cx.host_args ? d.arg_stride : 0);
+    if (!cx.full_window || cx.host_args || cx.host_items) {
+        uint64_t bytes_per_task = std::max<uint64_t>(R, cx.host_args ? d.arg_stride : 0);
+        if (cx.host_items && part.count) {
+            const uint64_t mean = (st.items.offsets[part.first + part.count] - st.items.offsets[part.first]) * st.items.item_bytes / part.count;
+            bytes_per_task = std::max<uint64_t>(bytes_per_task, mean + sizeof(uint64_t));
+        }
         // a wave must carry enough kernel time to hide its launches: 8 MiB of byte results is tens of us of
         // pi dispatch; a byte of bit-packed results stands for 8 tasks, so 1 MiB is the same work
         uint64_t min_wave_bytes = body.result_kind == FBR_RES_BITS8 ? (1ull << 20) : (8ull << 20);
@@ -1151,6 +1215,18 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
     static const bool pyramid_on = getenv("FBR_PYRAMID") && atoi(getenv("FBR_PYRAMID")) != 0;
     const bool pyramid = pyramid_on && (cx.peer_push || cx.peer_out);
     const uint64_t pyr_base = round_up(std::max<uint64_t>(unit, cx.wave_tasks_cap / 16), unit);
+    if (cx.host_items) {
+        // before any wave launches: every claim unit's offsets and items must fit one staging half
+        const uint64_t* o = st.items.offsets;
+        for (uint64_t t0 = part.first; t0 < part.first + part.count; t0 += unit) {
+            const uint64_t t1 = std::min<uint64_t>(t0 + unit, part.first + part.count);
+            const uint64_t ib = (o[t1] - o[t0]) * st.items.item_bytes;
+            if (round_up((t1 - t0 + 1) * sizeof(uint64_t), 256) + ib > p->ring_bytes)
+                return fail(FBR_EINVAL, "the claim unit of tasks [%llu, %llu) carries %llu item bytes, more than a staging half of "
+                            "ring_bytes %llu holds with its offsets: raise ring_bytes or split the items",
+                            (unsigned long long)t0, (unsigned long long)t1, (unsigned long long)ib, (unsigned long long)p->ring_bytes);
+        }
+    }
     uint64_t done_tasks = 0;
     uint32_t wave_idx = 0;
     while (done_tasks < part.count) {
@@ -1165,6 +1241,21 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
         ++wave_idx;
         if (taper && left <= 2 * cx.wave_tasks_cap && left > min_tail_tasks)
             wt = std::min(left, std::max(min_tail_tasks, round_up(left / 2, unit)));
+        if (cx.host_items) {
+            // the wave's offsets and item span must fit one staging half: the most whole units (or the rest of the block)
+            // that do, found by binary search over the host offsets
+            const uint64_t* o = st.items.offsets;
+            const uint64_t f = part.first + done_tasks;
+            auto fits = [&](uint64_t tasks) {
+                return round_up((tasks + 1) * sizeof(uint64_t), 256) + (o[f + tasks] - o[f]) * st.items.item_bytes <= p->ring_bytes;
+            };
+            uint64_t lo_u = 0, hi_u = (wt + unit - 1) / unit;               // fits(lo_u units) holds (0 tasks always fit)
+            while (lo_u < hi_u) {
+                const uint64_t mid = (lo_u + hi_u + 1) / 2;
+                if (fits(std::min<uint64_t>(mid * unit, wt))) lo_u = mid; else hi_u = mid - 1;
+            }
+            wt = std::min<uint64_t>(std::max<uint64_t>(lo_u, 1) * unit, wt);     // every unit fits (checked above)
+        }
         const uint32_t n_units = (uint32_t)((wt + unit - 1) / unit);
         const uint64_t wno = w.wave_no++;
         const int rw = (int)(wno % kRecWindows);
@@ -1366,6 +1457,8 @@ static void free_seq(fbr_pool* p, SeqState& st) {
         if (part.d_shared_tmp) cudaFreeAsync(part.d_shared_tmp, w.s_in);
         if (part.d_window) cudaFreeAsync(part.d_window, w.s_in);
         if (part.d_args_full) cudaFreeAsync(part.d_args_full, w.s_in);
+        if (part.d_items) cudaFreeAsync(part.d_items, w.s_in);
+        if (part.d_item_offs) cudaFreeAsync(part.d_item_offs, w.s_in);
         if (part.d_lost) cudaFreeAsync(part.d_lost, w.s_in);
         if (part.h_lost) cudaFreeHost(part.h_lost);
         if (part.ctrl_slot >= 0) w.ctrl_free.push_back(part.ctrl_slot);
@@ -1444,6 +1537,13 @@ int fbr_body_shared_info(int func_id, uint32_t* elem_bytes, uint32_t* stage_byte
     return FBR_OK;
 }
 
+int fbr_body_items_info(int func_id, uint32_t* item_bytes) {
+    const BodyEntry* bp = body_of(func_id);
+    if (!item_bytes || !bp) return fail(FBR_EINVAL, "bad func_id %d", func_id);
+    *item_bytes = bp->item_bytes;
+    return FBR_OK;
+}
+
 int fbr_body_lookup(const char* name, int* func_id) {
     if (!name || !func_id) return fail(FBR_EINVAL, "NULL argument");
     for (int f = 0, n = body_count(); f < n; ++f)
@@ -1481,6 +1581,20 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
         dlclose(h);
         return fail(FBR_EINVAL, "module %s: body '%s': only record bodies take a broadcast block (FBR_BODY_BROADCAST)", module_path, name);
     }
+    const bool items = (m->flags & FBR_BODY_ITEMS) != 0;
+    {
+        const char* why = nullptr;
+        const uint32_t e = m->item_bytes;
+        if (!items && m->item_bytes) why = "describes an item element but lacks FBR_BODY_ITEMS";
+        else if (items && !(m->flags & FBR_BODY_RECORD)) why = "only record bodies take items (FBR_BODY_ITEMS)";
+        else if (items && !(e == 1 || e == 2 || (e % 4 == 0 && e >= 4 && e <= 4096)))
+            why = "the item size must be 1, 2 or a multiple of 4 up to 4096 bytes";
+        else if (items && (m->flags & FBR_BODY_INDEX_ARG)) why = "an items body cannot take range() indices (FBR_BODY_INDEX_ARG)";
+        if (why) {
+            dlclose(h);
+            return fail(FBR_EINVAL, "module %s: body '%s' %s", module_path, name, why);
+        }
+    }
     const uint32_t group = m->group_threads;
     if (group > 1 && (group > 32 || (group & (group - 1)) != 0)) {
         dlclose(h);
@@ -1497,7 +1611,8 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
         const uint32_t align = (m->arg_bytes % 16 == 0 && m->result_bytes % 16 == 0) ? 1u
                              : (m->arg_bytes % 8 == 0 && m->result_bytes % 8 == 0) ? 2u : 4u;
         const char* why = nullptr;
-        if (m->arg_bytes == 0 || m->result_bytes == 0 || m->arg_bytes % 4 || m->result_bytes % 4) why = "argument and result bytes must be non-zero multiples of 4";
+        if (m->arg_bytes == 0 && !items) why = "argument bytes may be 0 (no head record, fbr::NoArg) only for an items body (FBR_BODY_ITEMS)";
+        else if (m->result_bytes == 0 || m->arg_bytes % 4 || m->result_bytes % 4) why = "argument and result bytes must be non-zero multiples of 4";
         else if (group <= 1 && big > 4096) why = "argument and result records are at most 4096 bytes";
         else if (big > 32768) why = "argument and result records of group bodies are at most 32768 bytes";
         else if ((uint64_t)align * big > 32768)
@@ -1537,6 +1652,7 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
     b.arg_bytes = m->arg_bytes; b.result_bytes = m->result_bytes; b.result_kind = m->result_kind;
     b.flags = m->flags; b.unit_tasks = m->unit_tasks;
     b.shared_elem_bytes = m->shared_elem_bytes; b.shared_stage_bytes = m->shared_stage_bytes;
+    b.item_bytes = m->item_bytes;
     b.launch = m->launch; b.occupancy = m->occupancy;
     b.module = h;
     g_bodies.push_back(b);
@@ -1715,8 +1831,55 @@ int fbr_shared_drop(fbr_pool_t* p, uint64_t handle) {
     return FBR_OK;
 }
 
+static int map_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out);
+
 int fbr_map_submit(fbr_pool_t* p, const fbr_map_desc_t* d, uint64_t* seq_out) {
     if (!p || !d || !seq_out) return fail(FBR_EINVAL, "NULL argument");
+    const BodyEntry* b = body_of(d->func_id);
+    if (b && (b->flags & FBR_BODY_ITEMS))
+        return fail(FBR_EINVAL, "body %s takes items: submit its maps with fbr_map_submit_items", b->name.c_str());
+    return map_submit(p, d, nullptr, seq_out);
+}
+
+int fbr_map_submit_items(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* it, uint64_t* seq_out) {
+    if (!p || !d || !it || !seq_out) return fail(FBR_EINVAL, "NULL argument");
+    const BodyEntry* b = body_of(d->func_id);
+    if (!b) return fail(FBR_EINVAL, "bad func_id %d", d->func_id);
+    if (!(b->flags & FBR_BODY_ITEMS))
+        return fail(FBR_EINVAL, "body %s takes no items: submit its maps with fbr_map_submit", b->name.c_str());
+    if (it->item_bytes != b->item_bytes)
+        return fail(FBR_EINVAL, "item_bytes %u does not match body %s (%u)", it->item_bytes, b->name.c_str(), b->item_bytes);
+    if (d->n_tasks && !it->offsets) return fail(FBR_EINVAL, "offsets is NULL");
+    if (it->n_items && !it->items) return fail(FBR_EINVAL, "items is NULL");
+    if (d->flags & FBR_ARGS_DEVICE) {
+        // a body may load its items as vectors as wide as the largest power of two dividing item_bytes, up to 16 B (a double,
+        // a 16 B struct); this is the alignment required, which can be stricter than alignof(Item) (four floats: 16, not 4)
+        const uint32_t e = it->item_bytes, align = std::min<uint32_t>(16u, e & (~e + 1u));
+        if ((uintptr_t)it->items % align)
+            return fail(FBR_EINVAL, "device-resident items of body %s must be %u-byte aligned", b->name.c_str(), align);
+        if ((uintptr_t)it->offsets % 8) return fail(FBR_EINVAL, "device-resident offsets must be 8-byte aligned");
+        int nw = 0;
+        {
+            std::lock_guard<std::mutex> g(p->mu);
+            nw = (int)p->workers.size();
+        }
+        if (nw != 1)
+            return fail(FBR_EINVAL, "device-resident items (FBR_ARGS_DEVICE) need a one-worker pool; this pool has %d workers", nw);
+    } else if (d->n_tasks) {
+        // the kernel trusts host-resident offsets: check them before anything launches
+        const uint64_t* o = it->offsets;
+        for (uint64_t j = 0; j < d->n_tasks; ++j)
+            if (o[j] > o[j + 1])
+                return fail(FBR_EINVAL, "offsets decrease at task %llu (%llu > %llu)", (unsigned long long)j,
+                            (unsigned long long)o[j], (unsigned long long)o[j + 1]);
+        if (o[d->n_tasks] > it->n_items)
+            return fail(FBR_EINVAL, "offsets[%llu] = %llu is past n_items %llu", (unsigned long long)d->n_tasks,
+                        (unsigned long long)o[d->n_tasks], (unsigned long long)it->n_items);
+    }
+    return map_submit(p, d, it, seq_out);
+}
+
+static int map_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out) {
     std::lock_guard<std::mutex> g(p->mu);
     if (p->state != ST_RUN) return fail(FBR_ESTATE, "Pool is not running");
     if (!body_of(d->func_id)) return fail(FBR_EINVAL, "bad func_id %d", d->func_id);
@@ -1724,7 +1887,9 @@ int fbr_map_submit(fbr_pool_t* p, const fbr_map_desc_t* d, uint64_t* seq_out) {
     const bool dev_mode = (d->flags & (FBR_ARGS_DEVICE | FBR_OUT_DEVICE)) != 0;
     if (dev_mode && p->workers.size() != 1 && !ensure_peer_access(p))
         return fail(FBR_EINVAL, "device-resident args/out on a multi-worker pool need peer access between all its GPUs");
-    if (d->arg_stride == 0) {
+    if ((body.flags & FBR_BODY_ITEMS) && body.arg_bytes == 0) {
+        if (d->arg_stride != 0) return fail(FBR_EINVAL, "body %s has no head record (arg_stride must be 0)", body.name.c_str());
+    } else if (d->arg_stride == 0) {
         if (!(body.flags & FBR_BODY_INDEX_ARG))
             return fail(FBR_EINVAL, "body %s needs explicit argument records (arg_stride=0)", body.name.c_str());
     } else if (body.flags & FBR_BODY_INDEX_ONLY) {
@@ -1787,6 +1952,8 @@ int fbr_map_submit(fbr_pool_t* p, const fbr_map_desc_t* d, uint64_t* seq_out) {
         st->result_kind = body.result_kind;
         st->out = d->out;
         st->desc = *d;
+        if (items) st->items = *items;
+        else memset(&st->items, 0, sizeof st->items);
         const bool need_segment = !st->out && d->n_tasks && !(d->flags & FBR_RESULTS_ON_DEVICE);
         // host allocations fail with the sticky error too once a context of this process has died: tell the two apart
         auto died_meanwhile = [&]() {

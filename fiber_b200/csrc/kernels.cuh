@@ -81,6 +81,13 @@ struct WaveParams {
     uint32_t syn_attempt;       // re-dispatch count of the whole wave (a dead worker's block re-run elsewhere)
     uint64_t n_items;           // bodies whose task consumes several argument items (bit-packed bool twins: 8 per
                                 // task): number of items of the whole map, items at or past it are not read
+    // items record bodies (FBR_BODY_ITEMS): map task j reads items [o[j], o[j+1]) with o = item_offs - item_first, and
+    // item k lies at items + (k - item_base) * item_bytes.  Offsets outside [item_base, item_count] are bad arguments
+    const uint8_t* items;
+    const uint64_t* item_offs;
+    uint64_t item_first;        // map index of item_offs[0]
+    uint64_t item_base;         // item index of items[0]
+    uint64_t item_count;        // offsets end here (the map's n_items)
 };
 
 // Task record of ticket t: from the device task ring, or computed (contiguous wave).
@@ -944,6 +951,17 @@ struct Group {
     __device__ __forceinline__ void sync() const { __syncwarp(mask); }
 };
 
+// The variable-length items of one task of an items record body (`using Item = ...`): n elements, read-only, in global
+// memory (through L1 / L2; DESIGN.md section 4 has the staged vs global measurement that chose this).
+template <class T>
+struct Items {
+    const T* data;
+    uint64_t n;
+};
+
+// The Arg of an items record body without a fixed head record: run() then takes no argument record.
+struct NoArg {};
+
 namespace record {
 constexpr int kConsumers = 256;
 constexpr int kThreads = 32 + kConsumers;
@@ -980,12 +998,31 @@ struct GroupOf<B, std::void_t<decltype(B::kGroup)>> {
     static_assert(kG == 2 || kG == 4 || kG == 8 || kG == 16 || kG == 32, "group record bodies: kGroup is 2, 4, 8, 16 or 32");
 };
 
+// A record body opts into variable-length items with `using Item = <element>;`: run() then takes a const Items<Item>&
+// after the argument record (or first, when Arg is NoArg).
+template <class B, class = void>
+struct ItemsOf {
+    static constexpr bool kOn = false;
+    static constexpr uint32_t kElem = 0;
+};
+template <class B>
+struct ItemsOf<B, std::void_t<typename B::Item>> {
+    using T = typename B::Item;
+    static constexpr bool kOn = true;
+    static constexpr uint32_t kElem = (uint32_t)sizeof(T);
+    static_assert(std::is_trivially_copyable<T>::value, "items bodies: Item is trivially copyable");
+    static_assert(kElem == 1 || kElem == 2 || (kElem % 4 == 0 && kElem <= 4096), "items bodies: sizeof(Item) is 1, 2 or a multiple of 4 up to 4096");
+    static_assert(!B::kIndexArg, "items bodies cannot take range() indices (kIndexArg)");
+};
+
 template <class B>
 struct Layout {
-    static constexpr uint32_t A = (uint32_t)sizeof(typename B::Arg), R = (uint32_t)sizeof(typename B::Res);
-    static_assert(GroupOf<B>::kG > 1 || (A % 4 == 0 && R % 4 == 0 && A >= 4 && R >= 4 && A <= 4096 && R <= 4096),
+    static constexpr bool kNoArg = std::is_same<typename B::Arg, NoArg>::value;
+    static constexpr uint32_t A = kNoArg ? 0u : (uint32_t)sizeof(typename B::Arg), R = (uint32_t)sizeof(typename B::Res);
+    static_assert(!kNoArg || ItemsOf<B>::kOn, "record bodies: only an items body may have no argument record (NoArg)");
+    static_assert(GroupOf<B>::kG > 1 || (A % 4 == 0 && R % 4 == 0 && (A >= 4 || kNoArg) && R >= 4 && A <= 4096 && R <= 4096),
                   "record bodies: sizeof(Arg) and sizeof(Res) are multiples of 4 between 4 and 4096");
-    static_assert(GroupOf<B>::kG == 1 || (A % 4 == 0 && R % 4 == 0 && A >= 4 && R >= 4 && A <= kStageBytes && R <= kStageBytes),
+    static_assert(GroupOf<B>::kG == 1 || (A % 4 == 0 && R % 4 == 0 && (A >= 4 || kNoArg) && R >= 4 && A <= kStageBytes && R <= kStageBytes),
                   "group record bodies: sizeof(Arg) and sizeof(Res) are multiples of 4 between 4 and 32768");
     // the broadcast region after the IN / OUT stages (0 bytes for bodies without a Shared type)
     static constexpr uint32_t kShared = BroadcastOf<B>::kStage;
@@ -1062,6 +1099,39 @@ __device__ __forceinline__ void run_group_unit(const WaveParams& wp, const TaskR
         }
     }
 }
+
+// One unit of an items body (one thread or a group per task, like the loops above): task i reads offsets o[i], o[i+1]
+// and its items from global memory; a task whose offsets decrease or leave [item_base, item_count] reports TASK_BADARG
+// and its body is not called.  `sh` is the broadcast block of a body that has one.
+template <class B, class... Sh>
+__device__ __forceinline__ void run_items_unit(const WaveParams& wp, const TaskRecord& rec, const uint8_t* in, uint8_t* out,
+                                               uint32_t ct, const ErrSink& es, const Sh&... sh) {
+    using L = Layout<B>;
+    using T = typename ItemsOf<B>::T;
+    using Res = typename B::Res;
+    constexpr uint32_t G = GroupOf<B>::kG, C = kConsumers;
+    const uint64_t* o = wp.item_offs + (rec.first - wp.item_first);
+    const uint64_t g0 = wp.index_base + rec.first;
+    for (uint32_t i = ct / G; i < rec.count; i += C / G) {
+        const uint64_t a = o[i], b = o[i + 1];
+        if (a > b || a < wp.item_base || b > wp.item_count) {
+            if (ct % G == 0) es.report(TASK_BADARG, g0 + i);
+            continue;
+        }
+        const Items<T> x{reinterpret_cast<const T*>(wp.items + (a - wp.item_base) * sizeof(T)), b - a};
+        Res& r = *reinterpret_cast<Res*>(out + (size_t)i * L::R);
+        auto call = [&](const auto&... grp) {
+            if constexpr (L::kNoArg) B::run(x, r, sh..., grp..., g0 + i, es, rec.attempt);
+            else B::run(*reinterpret_cast<const typename B::Arg*>(in + (size_t)i * L::A), x, r, sh..., grp..., g0 + i, es, rec.attempt);
+        };
+        if constexpr (G > 1) {
+            const uint32_t lane = ct & 31u;
+            call(Group<G>{ct % G, (G == 32 ? 0xffffffffu : ((1u << G) - 1u) << (lane & ~(G - 1u)))});
+        } else {
+            call();
+        }
+    }
+}
 }  // namespace record
 
 template <class B, bool kIndex>
@@ -1093,6 +1163,9 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
         staged = wp.shared_bytes <= Bc::kStage;
         if ((reinterpret_cast<uintptr_t>(wp.shared) & 15) == 0) bcast_bulk = (uint32_t)wp.shared_bytes & ~15u;
     }
+    // items bodies read each task's items from global memory (run_items_unit)
+    using It = record::ItemsOf<B>;
+    constexpr bool kArgs = !kIndex && L::A > 0;          // NoArg items bodies have no argument records
     if (threadIdx.x == 0) {
         for (int s = 0; s < kIn; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], C); }
         if constexpr (Bc::kOn && Bc::kStage > 0) mbar_init(bcast_full, 1);
@@ -1131,7 +1204,7 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
             s_rec[sg] = rec;
             s_ticket[sg] = t;
             uint32_t nb = 0;
-            if constexpr (!kIndex) {
+            if constexpr (kArgs) {
                 const uint8_t* src = wp.args + rec.arg_off;
                 if (wp.arg_stride == L::A && (reinterpret_cast<uintptr_t>(src) & 15) == 0) nb = (rec.count * L::A) & ~15u;
                 s_bulk[sg] = nb;
@@ -1162,7 +1235,7 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
         const uint32_t t = s_ticket[sg];
         const uint8_t* in = in_stage + (size_t)sg * L::kInBytes;
         uint8_t* out = out_stage + (size_t)og * L::kOutBytes;
-        if constexpr (!kIndex) {
+        if constexpr (kArgs) {
             const uint8_t* src = wp.args + rec.arg_off;
             uint8_t* stage = in_stage + (size_t)sg * L::kInBytes;
             if (wp.arg_stride == L::A) {
@@ -1180,7 +1253,17 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
         int* const unit_fault = &s_fault[seq & 1];
         const ErrSink es{wp.err_word, unit_fault};
         const uint64_t g0 = wp.index_base + rec.first;
-        if constexpr (!Bc::kOn && record::GroupOf<B>::kG > 1) {
+        if constexpr (It::kOn) {
+            // one loop per placement of the broadcast block, so each sees its pointer's address space
+            if constexpr (Bc::kOn) {
+                using T = typename Bc::T;
+                const uint64_t n_elems = wp.shared_bytes / Bc::kElem;
+                const uint8_t* blk = staged ? bcast_stage : wp.shared;
+                record::run_items_unit<B>(wp, rec, in, out, ct, es, Broadcast<T>{reinterpret_cast<const T*>(blk), n_elems});
+            } else {
+                record::run_items_unit<B>(wp, rec, in, out, ct, es);
+            }
+        } else if constexpr (!Bc::kOn && record::GroupOf<B>::kG > 1) {
             record::run_group_unit<B, kIndex>(wp, rec, in, out, ct, es);
         } else if constexpr (!Bc::kOn) {
             for (uint32_t i = ct; i < rec.count; i += C) {

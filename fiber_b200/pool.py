@@ -609,7 +609,14 @@ class Pool:
         d.attempt = self._attempt
         d.flags = flags
         seq = ctypes.c_uint64(0)
-        if enc.n:
+        if enc.n and enc.items is not None:
+            values, offsets = enc.items
+            keep += [values, offsets]
+            it = _abi.ItemsDesc()
+            it.items, it.offsets = values.ctypes.data, offsets.ctypes.data
+            it.n_items, it.item_bytes = len(values), values.dtype.itemsize
+            _abi.check(eng.lib.fbr_map_submit_items(eng.handle, ctypes.byref(d), ctypes.byref(it), ctypes.byref(seq)))
+        elif enc.n:
             _abi.check(eng.lib.fbr_map_submit(eng.handle, ctypes.byref(d), ctypes.byref(seq)))
         self.sent_tasks += enc.n
         r = cls(self, eng, spec, seq.value, enc.n, keep)
@@ -649,8 +656,8 @@ class Pool:
 
     def _submit_proc(self, spec, kind, items, chunksize, single=False):
         """Process-isolated workers: the map is cut into blocks that worker processes pull (procpool.py)."""
-        if not isinstance(items, (range, list, np.ndarray)):
-            items = list(items)
+        if not isinstance(items, (range, list, np.ndarray, registry.Ragged)):
+            items = list(items)         # a Ragged stays one: its blocks are slices with rebased offsets
         if kind == "map" and len(items):
             spec.encode_map(items[:1] if not isinstance(items, range) else items)      # argument validation up front
         twin = registry.BITS_TWIN.get(spec.name) if (self._results_bits and kind != "apply") else None

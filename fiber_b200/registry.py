@@ -12,6 +12,7 @@ Encoders turn the Python-level task arguments (what the reference would pickle,
 fiber/pool.py:1181,1297-1301,1112-1113) into fixed-layout argument records.
 """
 import hashlib
+import operator
 import struct
 
 import numpy as np
@@ -21,7 +22,8 @@ from . import _abi
 _BOUND = {}  # callables that cannot carry attributes (builtins) -> body name
 
 
-def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entry=None, result=None, shared=None, **meta):
+def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entry=None, result=None, shared=None, items=None,
+                **meta):
     """Decorator: ``@device_body("pi_inside_det")`` binds ``func`` to the device body ``name`` and sets
     ``func.__fiber_meta__`` (``gpu=1`` unless overridden), like ``fiber.meta``.
 
@@ -48,7 +50,15 @@ def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entr
     A GROUP record body (``static constexpr uint32_t kGroup = G;`` in its struct, G = 2, 4, 8, 16 or 32) runs each task on
     G lanes of one warp, and its records may reach 32 KB (INTEGRATION.md has the size rules).  Nothing changes here:
     ``kGroup`` lives in the CUDA source, and ``map(f, rows)`` over a plain ``(n, k)`` array of a one-field body with a
-    ``(k,)`` sub-array passes the rows without a copy, e.g. ``args=[("x", "<f8", (1024,))]`` for 8 KB rows."""
+    ``(k,)`` sub-array passes the rows without a copy, e.g. ``args=[("x", "<f8", (1024,))]`` for 8 KB rows.
+
+    An ITEMS record body (``using Item = ...`` in its struct) also takes one variable-length array per task:
+    ``items=("doc", "u1")`` names that parameter and describes one element.  The parameters are the broadcast parameter
+    (if any), then the items parameter, then the ``args`` fields; ``args=None`` means no head record (``fbr::NoArg``).
+    A task's items are a 1-D array of the element dtype (or a 1-D array / list whose values the dtype holds exactly: floats
+    into an integer dtype or integers out of its range raise ``TypeError``), or, for a 1-byte
+    element, ``bytes`` / ``bytearray`` / ``memoryview`` / ``str`` (sent as UTF-8).  ``map(f, Ragged(values, offsets))``
+    passes a whole ragged array without a copy."""
     from .meta import VALID_META_KEYS
     for k in meta:
         assert k in VALID_META_KEYS, "Invalid meta argument \"{}\"".format(k)
@@ -56,7 +66,7 @@ def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entr
     md.update(meta)
     if source is not None:
         from . import bodies
-        register_module(name, bodies.compile_module(name, source), entry, args, bits_entry, result, shared)
+        register_module(name, bodies.compile_module(name, source), entry, args, bits_entry, result, shared, items)
 
     def decorator(func):
         bind(func, name, **md)
@@ -64,8 +74,8 @@ def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entr
     return decorator
 
 
-_MODULES = {}   # body name -> (module path, entry, argument layout, bits entry, result layout, broadcast parameter) of bodies
-                # registered from their own module
+_MODULES = {}   # body name -> (module path, entry, argument layout, bits entry, result layout, broadcast parameter, items
+                # parameter) of bodies registered from their own module
 
 
 def module_of(name):
@@ -73,14 +83,16 @@ def module_of(name):
     return _MODULES.get(name)
 
 
-def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_entry=None, result=None, shared=None):
+def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_entry=None, result=None, shared=None, items=None):
     """``fbr_register_body`` + the host-side encoder for the body's argument records (and, with ``bits_entry``, the
     body's bit-packed twin ``<name>_bits8``).  Record bodies (``FBR_BODY_RECORD``) take NumPy dtypes for ``args`` and
     ``result``; their sizes must be the module's ``arg_bytes`` / ``result_bytes`` (``ValueError`` otherwise).
     Broadcast bodies (``FBR_BODY_BROADCAST``) also take ``shared=(parameter name, element dtype)``, whose size must be
     the module's element size; ``shared`` is refused for every other body (``ValueError``).  A group record body
     (``group_threads`` > 1 in its module descriptor: several threads per task, records up to 32 KB) registers like any
-    other record body."""
+    other record body.  Items bodies (``FBR_BODY_ITEMS``) take ``items=(parameter name, element dtype)``, whose size must
+    be the module's item size, and ``args=None`` when they have no head record; ``items`` is refused for every other
+    body (``ValueError``)."""
     import ctypes
     specs = _load_specs()           # the table as it was: the body registered below gets the encoder its layout asks for
     if bits_entry is not None:
@@ -94,7 +106,28 @@ def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_
     info = _abi.BodyInfo()
     _abi.check(L.fbr_body_info(fid.value, ctypes.byref(info)))
     record = None
-    if info.flags & _abi.FBR_BODY_BROADCAST:
+    if info.flags & _abi.FBR_BODY_ITEMS:
+        if result is None or items is None:
+            raise ValueError("items body %s: pass result=<dtype> and items=(<parameter name>, <element dtype>)" % name)
+        ib = ctypes.c_uint32(0)
+        _abi.check(L.fbr_body_items_info(fid.value, ctypes.byref(ib)))
+        elem, stage = ctypes.c_uint32(0), ctypes.c_uint32(0)
+        if info.flags & _abi.FBR_BODY_BROADCAST:
+            if shared is None:
+                raise ValueError("items body %s reads a broadcast block: pass shared=(<parameter name>, <element dtype>)" % name)
+            _abi.check(L.fbr_body_shared_info(fid.value, ctypes.byref(elem), ctypes.byref(stage)))
+        elif shared is not None:
+            raise ValueError("body %s reads no broadcast block (its record struct has no Shared element type): shared= is "
+                             "for broadcast bodies only" % name)
+        # args left at its default means no head record for a body that has none
+        head = None if (isinstance(args, str) and args == "i64" and info.arg_bytes == 0) else args
+        record = _Items(info, items, head, result, shared, ib.value, elem.value, stage.value)
+        args, result, items = record.arg_dtype, record.res_dtype, (record.item_name, record.item_dtype)
+        shared = (record.shared_name, record.shared_dtype) if record.shared_name is not None else None
+    elif items is not None:
+        raise ValueError("body %s takes no items (its record struct has no Item element type): items= is for items bodies "
+                         "only" % name)
+    elif info.flags & _abi.FBR_BODY_BROADCAST:
         if result is None or shared is None:
             raise ValueError("broadcast body %s: pass result=<dtype> and shared=(<parameter name>, <element dtype>)" % name)
         elem, stage = ctypes.c_uint32(0), ctypes.c_uint32(0)
@@ -114,9 +147,9 @@ def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_
     old = specs.get(name)
     if record is not None and isinstance(old, _Record) and old.layouts() != record.layouts():
         raise ValueError("record body %s is registered already with %s; a name keeps its layouts"
-                         % (name, ", ".join("%s=%s" % kv for kv in zip(("args", "result", "shared"), old.layouts()))))
+                         % (name, ", ".join("%s=%s" % kv for kv in zip(("args", "result", "shared", "items"), old.layouts()))))
     # the engine keeps the first module registered under a name (fbr_register_body is idempotent): so do worker processes
-    _MODULES.setdefault(name, (str(module_path), entry, args, bits_entry, result, shared))
+    _MODULES.setdefault(name, (str(module_path), entry, args, bits_entry, result, shared, items))
     if name not in specs:
         if record is not None:
             specs[name] = record
@@ -178,13 +211,15 @@ def body_name_of(func):
 # ------------------------------------------------------------------------------------------------
 class Encoded:
     """Fixed-layout form of one map's arguments."""
-    __slots__ = ("n", "args", "arg_stride", "index_start", "index_step", "shared", "task_index_base", "keepalive", "n_items")
+    __slots__ = ("n", "args", "arg_stride", "index_start", "index_step", "shared", "task_index_base", "keepalive", "n_items",
+                 "items")
 
     def __init__(self, n, args=None, arg_stride=0, index_start=0, index_step=1, shared=None, task_index_base=0, n_items=0):
         self.n, self.args, self.arg_stride = n, args, arg_stride
         self.index_start, self.index_step = index_start, index_step
         self.shared, self.task_index_base = shared, task_index_base
         self.n_items = n_items     # bit-packed twins: argument items of the whole map (8 per task, the last may be short)
+        self.items = None          # items bodies: (values, uint64 offsets) -- task j reads values[offsets[j]:offsets[j+1]]
 
 
 def _as_i64(values, what):
@@ -594,6 +629,9 @@ class _Broadcast(_Record):
 
     def __init__(self, info, args, result, shared, elem_bytes, stage_bytes):
         super().__init__(info, args, result)
+        self._init_shared(shared, elem_bytes, stage_bytes)
+
+    def _init_shared(self, shared, elem_bytes, stage_bytes):
         if not (isinstance(shared, (tuple, list)) and len(shared) == 2 and isinstance(shared[0], str) and shared[0].isidentifier()):
             raise ValueError("%s: shared= is (<parameter name>, <element dtype>), got %r" % (self.name, shared))
         self.shared_name = shared[0]
@@ -669,6 +707,187 @@ class _Broadcast(_Record):
         enc = self._columns([list(c) for c in zip(*rows)] if rows else [[] for _ in self._fields])
         enc.shared = self._blocks.get((block,), _block_bytes) if block is not None else None
         return enc
+
+
+class Ragged:
+    """A sequence of variable-length 1-D arrays in two arrays: ``r[i]`` is ``values[offsets[i]:offsets[i+1]]``.
+
+    ``map(f, Ragged(values, offsets))`` over an items body passes both arrays to the engine without a copy (when
+    ``values`` is contiguous with the body's element dtype and ``offsets`` contiguous 64-bit integers).  ``offsets`` are
+    n + 1 non-decreasing indices, all within ``values``; ``offsets[0]`` need not be 0.  Slicing gives a Ragged over the
+    slice's values with rebased offsets."""
+
+    def __init__(self, values, offsets):
+        values, offsets = np.asarray(values), np.asarray(offsets)
+        if values.ndim != 1:
+            raise ValueError("Ragged: values must be 1-D, got shape %s" % (values.shape,))
+        if offsets.ndim != 1 or len(offsets) == 0 or offsets.dtype.kind not in "iu":
+            raise ValueError("Ragged: offsets must be a non-empty 1-D integer array (n + 1 entries)")
+        if len(offsets) > 1 and bool(np.any(offsets[1:] < offsets[:-1])):
+            raise ValueError("Ragged: offsets must not decrease")
+        if (offsets.dtype.kind == "i" and int(offsets[0]) < 0) or int(offsets[-1]) > len(values):
+            raise ValueError("Ragged: offsets must lie in [0, len(values)] (last offset %d, %d values)" % (int(offsets[-1]), len(values)))
+        self.values, self.offsets = values, offsets
+
+    def __len__(self):
+        return len(self.offsets) - 1
+
+    def __getitem__(self, i):
+        if isinstance(i, slice):
+            start, stop, step = i.indices(len(self))
+            if step != 1:
+                raise ValueError("Ragged: only contiguous slices")
+            o = self.offsets[start:max(start, stop) + 1]
+            return Ragged(self.values[int(o[0]):int(o[-1])], o.astype(np.int64) - int(o[0]))
+        i = operator.index(i)
+        n = len(self)
+        if i < 0:
+            i += n
+        if not 0 <= i < n:
+            raise IndexError("Ragged index out of range")
+        return self.values[int(self.offsets[i]):int(self.offsets[i + 1])]
+
+    def __reduce__(self):
+        return (Ragged, (self.values, self.offsets))
+
+
+def _item_array(name, dtype, x):
+    """One task's items as a 1-D array of `dtype`.  Values the dtype cannot hold exactly -- floats into an integer dtype,
+    integers out of its range, text or objects -- are refused (TypeError) rather than truncated or wrapped."""
+    try:
+        a = np.asarray(x)
+    except (ValueError, TypeError, OverflowError) as e:
+        raise TypeError("%s: an item is not convertible to a 1-D array of %s (%s)" % (name, dtype, e)) from None
+    if a.ndim != 1:
+        raise TypeError("%s: every item must be 1-D, got shape %s" % (name, a.shape))
+    if a.dtype == dtype:
+        return a
+    kind = dtype.kind
+    if a.dtype.kind in "OUSV" or (a.dtype.kind in "fc" and kind in "iub") or (a.dtype.kind == "c" and kind == "f"):
+        raise TypeError("%s: an item of %s is not convertible to a 1-D array of %s without loss" % (name, a.dtype, dtype))
+    out = a.astype(dtype)
+    if a.dtype.kind in "iub" and kind in "iu" and not np.array_equal(out, a):
+        raise TypeError("%s: an item holds integers outside the range of %s" % (name, dtype))
+    return out
+
+
+def _encode_items(name, dtype, xs):
+    """One map's items as (values, uint64 offsets): a Ragged as it is, else the concatenation of every task's items.  Byte
+    strings are joined in one call (no NumPy call per item)."""
+    if isinstance(xs, Ragged):
+        v, o = xs.values, xs.offsets
+        if v.dtype != dtype:
+            raise TypeError("%s: Ragged values are %s, the body's items are %s" % (name, v.dtype, dtype))
+        if o.dtype == np.int64:
+            o = o.view(np.uint64)                 # validated non-negative by Ragged
+        return np.ascontiguousarray(v), np.ascontiguousarray(o, dtype=np.uint64)
+    xs = list(xs)
+    byteish = [isinstance(x, (bytes, bytearray, memoryview, str)) for x in xs]
+    if any(byteish):
+        if dtype.itemsize != 1:
+            raise TypeError("%s: bytes and str items need a 1-byte item dtype, the body's is %s" % (name, dtype))
+        if not all(byteish):
+            raise TypeError("%s: mixed byte strings and arrays in one map" % name)
+        parts = [x.encode("utf-8") if isinstance(x, str) else bytes(x) for x in xs]
+        lens = np.fromiter(map(len, parts), dtype=np.uint64, count=len(parts))
+        values = np.frombuffer(b"".join(parts), dtype=dtype)
+    else:
+        arrays = [_item_array(name, dtype, x) for x in xs]
+        lens = np.fromiter(map(len, arrays), dtype=np.uint64, count=len(arrays))
+        values = np.concatenate(arrays) if arrays else np.empty(0, dtype)
+    offsets = np.zeros(len(lens) + 1, np.uint64)
+    np.cumsum(lens, out=offsets[1:])
+    return values, offsets
+
+
+class _Items(_Broadcast):
+    """A record body whose task also takes one variable-length array (``FBR_BODY_ITEMS``): ``item_name`` is its
+    parameter, ``item_dtype`` one element.  The parameters are the broadcast parameter (bodies with a Shared type), the
+    items, then the argument dtype's fields (none when ``args`` is None: the body has no head record).  ``map(f, xs)``
+    passes one items array per task (bodies without a head record); ``starmap`` / ``apply_async`` bind the items like any
+    other parameter."""
+
+    def __init__(self, info, items, args, result, shared, item_bytes, shared_elem=0, shared_stage=0):
+        if args is None:
+            if info.arg_bytes:
+                raise ValueError("%s: args=None, but the body's head record is %d bytes" % (info.name.decode(), info.arg_bytes))
+            BodySpec.__init__(self, info)
+            self.arg_dtype, self.params, self._sdt, self._fields = None, None, None, ()
+            self.res_dtype = _record_dtype(result, "result", self.name)
+            if self.res_dtype.itemsize != self.result_bytes:
+                raise ValueError("%s: result dtype %s is %d bytes, the body's result record is %d"
+                                 % (self.name, self.res_dtype, self.res_dtype.itemsize, self.result_bytes))
+        else:
+            _Record.__init__(self, info, args, result)
+        self.shared_name = self.shared_dtype = None
+        if shared is not None:
+            self._init_shared(shared, shared_elem, shared_stage)
+        if not (isinstance(items, (tuple, list)) and len(items) == 2 and isinstance(items[0], str) and items[0].isidentifier()):
+            raise ValueError("%s: items= is (<parameter name>, <element dtype>), got %r" % (self.name, items))
+        self.item_name = items[0]
+        if self.item_name == self.shared_name or (self.params is not None and self.item_name in self.params):
+            raise ValueError("%s: the items parameter %r is also another parameter" % (self.name, self.item_name))
+        self.item_dtype = _record_dtype(items[1], "item", self.name)
+        if self.item_dtype.itemsize != item_bytes:
+            raise ValueError("%s: item dtype %s is %d bytes, the body's Item is %d"
+                             % (self.name, self.item_dtype, self.item_dtype.itemsize, item_bytes))
+
+    def layouts(self):
+        shared = (self.shared_name, self.shared_dtype) if self.shared_name is not None else None
+        return (self.arg_dtype, self.res_dtype, shared, (self.item_name, self.item_dtype))
+
+    def _with_items(self, enc, xs):
+        enc.items = _encode_items(self.name, self.item_dtype, xs)
+        enc.n = len(enc.items[1]) - 1
+        return enc
+
+    def _encode(self, items, fast, apply=False):
+        if fast:
+            if self.arg_dtype is None:      # map(f, xs): each item is one task's items; a broadcast block is the initializer's
+                return self._with_items(Encoded(0), items)
+            items = [(it,) for it in items]
+        n_fields = len(self._fields)
+        xs, rows, first, block, carried = [], [], None, None, None
+        for it in items:
+            args, kwds = self._split(it, apply)
+            kwds = dict(kwds)
+            if self.shared_name is not None:
+                if self.shared_name in kwds:
+                    b = kwds.pop(self.shared_name)
+                elif args and len(args) + len(kwds) > 1 + n_fields:    # one more argument than the items and the record
+                    b, args = args[0], tuple(args[1:])
+                else:
+                    b = _MISSING
+                has = b is not _MISSING
+                if carried is None:
+                    carried = has
+                elif carried != has:
+                    raise TypeError("%s: mixed items with and without %s in one map" % (self.name, self.shared_name))
+                if has:
+                    if first is None:
+                        first, block = b, self._block_array(b)
+                    elif b is not first and not _same_bytes(self._block_array(b), block):
+                        raise ValueError("%s: all tasks of one map must share %s" % (self.name, self.shared_name))
+            if self.item_name in kwds:
+                x = kwds.pop(self.item_name)
+            elif args:
+                x, args = args[0], tuple(args[1:])
+            else:
+                raise TypeError("%s() missing 1 required positional argument: %r" % (self.name, self.item_name))
+            xs.append(x)
+            if self.arg_dtype is None:
+                if args or kwds:
+                    raise TypeError("%s() takes %d positional argument%s but more were given (unexpected %s)"
+                                    % (self.name, 1 + (self.shared_name is not None), "" if self.shared_name is None else "s",
+                                       ", ".join([repr(a) for a in args] + list(map(repr, kwds)))))
+            else:
+                rows.append(self._bind(args, kwds))
+        if self.arg_dtype is None:
+            enc = Encoded(0)
+        else:
+            enc = self._columns([list(c) for c in zip(*rows)] if rows else [[] for _ in self._fields])
+        enc.shared = self._blocks.get((block,), _block_bytes) if block is not None else None
+        return self._with_items(enc, xs)
 
 
 class _SleepF64(BodySpec):

@@ -75,6 +75,9 @@ typedef enum fbr_result_kind {
                                      NEEDS_SHARED only together with BROADCAST */
 #define FBR_BODY_BROADCAST 0x20u  /* record body whose run() receives the map's broadcast block as an array of its
                                      Shared element type (fbr_body_shared_info); always set with NEEDS_SHARED */
+#define FBR_BODY_ITEMS 0x40u      /* record body whose task also takes a variable-length array of its Item element type
+                                     (fbr_body_items_info); its maps go through fbr_map_submit_items.  arg_bytes may be 0
+                                     (no head record, Arg = fbr::NoArg); never with FBR_BODY_INDEX_ARG */
 
 typedef struct fbr_body_info {
     int32_t func_id;
@@ -100,7 +103,7 @@ int fbr_body_lookup(const char* name, int* func_id);
  * (func_id >= the compiled-in count; the same name may be registered once).  The module's launch routine
  * receives the same wave parameters as the compiled-in kernels, so registered bodies run in the same
  * persistent-CTA dispatch kernels (direct placement, ring + gather_ordered, resilient re-dispatch). */
-#define FBR_BODY_MODULE_ABI 3
+#define FBR_BODY_MODULE_ABI 4
 typedef struct fbr_body_module {
     uint32_t abi;               /* FBR_BODY_MODULE_ABI */
     uint32_t wave_params_bytes; /* sizeof(fbr::WaveParams) the module was compiled against */
@@ -115,6 +118,9 @@ typedef struct fbr_body_module {
        records reach 32768 bytes (kAlign * max(arg_bytes, result_bytes) <= 32768, kAlign = 1, 2 or 4 tasks: both sizes
        multiples of 16, of 8, or neither).  0 or 1: one thread per task */
     uint32_t group_threads;
+    /* FBR_BODY_ITEMS record bodies: sizeof(Item) (1, 2 or a multiple of 4 up to 4096).  0 (or left out of a hand-written
+       descriptor) for every other body */
+    uint32_t item_bytes;
 } fbr_body_module_t;
 typedef const fbr_body_module_t* (*fbr_body_entry_fn)(void);
 int fbr_register_body(const char* name, const char* module_path, const char* entry, int* func_id);
@@ -122,6 +128,8 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
  * passes a block of shared_bytes > 0, a multiple of elem_bytes; blocks up to stage_bytes are staged into shared memory
  * once per CTA, larger ones are read from global memory. */
 int fbr_body_shared_info(int func_id, uint32_t* elem_bytes, uint32_t* stage_bytes);
+/* Item size of a FBR_BODY_ITEMS body (0 for other bodies).  The dispatch kernel reads each task's items from global memory. */
+int fbr_body_items_info(int func_id, uint32_t* item_bytes);
 
 /* ---- pool lifecycle -------------------------------------------------------------------------
  * fbr_pool_create   <- ZPool.__init__ (fiber/pool.py:888-943) + worker start
@@ -203,6 +211,25 @@ typedef struct fbr_map_desc {
 } fbr_map_desc_t;
 
 int fbr_map_submit(fbr_pool_t* pool, const fbr_map_desc_t* desc, uint64_t* seq);
+
+/* Maps of FBR_BODY_ITEMS bodies: besides its head record (args / arg_stride, if the body has one; arg_stride 0 when
+ * arg_bytes is 0), task j reads items [offsets[j], offsets[j+1]) of `items`.  offsets[0] may be non-zero (a slice of a
+ * larger array).  Host-resident offsets are checked before anything launches; device-resident ones (FBR_ARGS_DEVICE:
+ * items and offsets are device pointers on worker 0, one-worker pools only, offsets 8-byte aligned, items aligned to the
+ * largest power of two that divides item_bytes, at most 16: 1, 2, 4, 8 or 16 bytes, so a body may load its items as
+ * vectors that wide) are checked by the kernel, and a task whose offsets decrease or pass n_items fails with
+ * FBR_TASK_BADARG.  Host-resident items and offsets stream to the device wave by wave through two staging halves of
+ * ring_bytes each (a resilient map copies its whole block once); a claim unit whose offsets and items do not fit one
+ * half is refused with FBR_EINVAL before anything launches.
+ * fbr_map_submit refuses items bodies and fbr_map_submit_items every other body (FBR_EINVAL). */
+typedef struct fbr_items_desc {
+    const void* items;        /* item array: host, or device on worker 0 with FBR_ARGS_DEVICE */
+    const uint64_t* offsets;  /* n_tasks + 1 non-decreasing item indices: task j reads items [offsets[j], offsets[j+1]) */
+    uint64_t n_items;         /* items in `items`; every offset is <= n_items */
+    uint32_t item_bytes;      /* must equal the body's */
+    uint32_t pad;
+} fbr_items_desc_t;
+int fbr_map_submit_items(fbr_pool_t* pool, const fbr_map_desc_t* desc, const fbr_items_desc_t* items, uint64_t* seq);
 
 /* Broadcast argument blocks (initargs / arguments every task shares, e.g. the parzen sample array
  * the reference pickles into each of its 102 task messages, SURVEY.md 3.2): uploaded once to every

@@ -91,6 +91,24 @@
 // where kAlign (fbr::record::Layout<B>::kAlign) is 1 when both sizes are multiples of 16, 2 when both are multiples of
 // 8, else 4: records that are multiples of 16 may reach 32 KB, multiples of 8 16 KB, any other pair 8 KB.  A body
 // without kGroup is a one-thread body with records up to 4096 bytes.  FBR_EXPORT_RECORD_BODY checks all of this.
+//
+// An ITEMS record body's task also takes one variable-length array (a string, a document's tokens, a user's session):
+// it declares the element type, and run() gets the task's items after its head record.  Arg = fbr::NoArg means no head record (run() then starts with the items):
+//
+//     struct Fnv1a {
+//         using Item = uint8_t;                           // sizeof 1, 2, or a multiple of 4 up to 4096
+//         using Arg = fbr::NoArg;
+//         struct Res { uint64_t h; uint32_t n, pad; };
+//         static constexpr bool kIndexArg = false, kCanFault = false;
+//         __device__ static void run(const fbr::Items<Item>& x, Res& r, uint64_t task_index, const fbr::ErrSink& es,
+//                                    uint32_t attempt) { ... x.data[0 .. x.n) ... }
+//     };
+//     FBR_EXPORT_RECORD_BODY(Fnv1a, "fnv1a_bytes", fnv1a_entry, 0)
+//
+// The full signature is run([const Arg& a,] const fbr::Items<Item>& x, Res& r, [Broadcast], [Group], task_index, es,
+// attempt).  x.data is read-only and points into the map's item array in global memory, so vector loads legal on the
+// array are legal on x.data.  All G lanes of a group body get the same x.  Items bodies cannot have kIndexArg.
+// FBR_EXPORT_RECORD_BODY sets FBR_BODY_ITEMS and writes item_bytes.
 #pragma once
 #include "fiber_b200.h"
 #include "kernels.cuh"      // fiber_b200/csrc: dispatch_thread_kernel, WaveParams, ErrSink, TaskError
@@ -208,7 +226,8 @@ constexpr bool record_body_ok() {
 // the flags a record body's descriptor carries on top of the exported ones: broadcast bodies need a block and take it
 template <class B>
 constexpr uint32_t record_flags() {
-    return FBR_BODY_RECORD | (fbr::record::BroadcastOf<B>::kOn ? (FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST) : 0u);
+    return FBR_BODY_RECORD | (fbr::record::BroadcastOf<B>::kOn ? (FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST) : 0u) |
+           (fbr::record::ItemsOf<B>::kOn ? FBR_BODY_ITEMS : 0u);
 }
 // the descriptor's group_threads: kGroup of a group body, 0 for a one-thread body
 template <class B>
@@ -222,7 +241,8 @@ constexpr uint32_t record_group() {
 // body_flags, which carry FBR_BODY_INDEX_ARG exactly when Body::kIndexArg is true (a range() map of a body without the
 // index instantiation would read no arguments).  unit_tasks is the number of tasks whose records fill one shared-memory
 // stage of dispatch_record_kernel.  A body with a Shared type also gets FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST and
-// its element size and staging budget; a body with kGroup gets group_threads = kGroup.
+// its element size and staging budget; a body with kGroup gets group_threads = kGroup; a body with an Item type gets
+// FBR_BODY_ITEMS and its item size.
 #define FBR_EXPORT_RECORD_BODY(Body, body_name, entry, body_flags)                                                \
     static_assert(fbr_body_export::record_body_ok<Body>(), "record body");                                       \
     static_assert((((body_flags) & FBR_BODY_INDEX_ARG) != 0) == Body::kIndexArg,                                 \
@@ -235,7 +255,8 @@ constexpr uint32_t record_group() {
                                             fbr::record::Layout<Body>::kUnit,                                    \
                                             fbr_body_export::launch_record<Body>, fbr_body_export::occupancy_record<Body>, \
                                             fbr::record::BroadcastOf<Body>::kElem, fbr::record::BroadcastOf<Body>::kStage, \
-                                            fbr_body_export::record_group<Body>()};                              \
+                                            fbr_body_export::record_group<Body>(),                               \
+                                            fbr::record::ItemsOf<Body>::kElem};                                  \
         return &m;                                                                                               \
     }
 
