@@ -14,7 +14,8 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "_lib")
 SO = os.path.join(LIBDIR, "libfiber_b200.so")
 SOURCES = ["engine.cu", "queues.cu", "express.cu", "comm.cu"]
-HEADERS = ["kernels.cuh", "bodies.cuh", os.path.join("..", "..", "include", "fiber_b200.h")]
+HEADERS = ["kernels.cuh", "bodies.cuh", os.path.join("..", "..", "include", "fiber_b200.h"),
+           os.path.join("..", "..", "include", "fiber_b200_body.cuh")]
 
 # every device object of the project (library, body modules, microbenchmarks) is built for this one target:
 # the kernels use sm_90a's bulk async copies and mbarriers, and the library refuses any other device
@@ -24,6 +25,7 @@ NVCC_FLAGS = ARCH_FLAGS + [
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function",
     "-shared",
+    "-I" + CSRC,            # engine.cu includes fiber_b200_body.cuh, which includes kernels.cuh
 ]
 LINK_FLAGS = ["-ldl"]   # body modules (fbr_register_body) and NCCL (fbr_comm_*) are bound at run time
 

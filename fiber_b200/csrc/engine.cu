@@ -33,9 +33,11 @@
 #include <vector>
 
 #include "../../include/fiber_b200.h"
+#include "../../include/fiber_b200_body.cuh"
 #include "kernels.cuh"
 
 using namespace fbr;
+using fbr_body_export::occupancy_of;
 
 // ------------------------------------------------------------------------------------------------
 // errors
@@ -44,13 +46,23 @@ static thread_local std::string g_err;
 
 static int fail(int code, const char* fmt, ...);
 const std::string& last_error_of_this_thread();
-static int fail(int code, const char* fmt, ...) {
+static std::string vstrf(const char* fmt, va_list ap) {
     char buf[512];
+    vsnprintf(buf, sizeof buf, fmt, ap);
+    return buf;
+}
+static std::string strf(const char* fmt, ...) {
     va_list ap;
     va_start(ap, fmt);
-    vsnprintf(buf, sizeof buf, fmt, ap);
+    std::string s = vstrf(fmt, ap);
     va_end(ap);
-    g_err = buf;
+    return s;
+}
+static int fail(int code, const char* fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    g_err = vstrf(fmt, ap);
+    va_end(ap);
     return code;
 }
 const std::string& last_error_of_this_thread() { return g_err; }
@@ -101,30 +113,6 @@ struct SubmitThread {
 typedef void (*launch_fn)(const void* wave_params, int grid, void* stream);
 typedef int (*occupancy_fn)(int index_mode);
 
-template <class B>
-static void launch_thread(const void* wpv, int grid, void* sv) {
-    const WaveParams& wp = *(const WaveParams*)wpv;
-    cudaStream_t s = (cudaStream_t)sv;
-    if constexpr (B::kIndexArg) {
-        if (wp.arg_stride == 0) {
-            dispatch_thread_kernel<B, true><<<grid, kThreads, 0, s>>>(wp);
-            return;
-        }
-    }
-    dispatch_thread_kernel<B, false><<<grid, kThreads, 0, s>>>(wp);
-}
-static int occ_of(const void* kernel) {
-    int occ = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, kThreads, 0) != cudaSuccess) { cudaGetLastError(); return 1; }
-    return occ > 0 ? occ : 1;
-}
-template <class B>
-static int occ_thread(int index_mode) {
-    if constexpr (B::kIndexArg) {
-        if (index_mode) return occ_of((const void*)dispatch_thread_kernel<B, true>);
-    }
-    return occ_of((const void*)dispatch_thread_kernel<B, false>);
-}
 static void launch_payload_map(const void* wpv, int grid, void* sv) {
     const WaveParams& wp = *(const WaveParams*)wpv;
     cudaStream_t s = (cudaStream_t)sv;
@@ -151,12 +139,12 @@ static int occ_payload_map(int) {
     cudaFuncAttributes at;
     cudaFuncGetAttributes(&at, (const void*)dispatch_payload_map_tma_kernel<3, 2>);   // force-load
     cudaFuncGetAttributes(&at, (const void*)dispatch_payload_map_tma_kernel<6, 3>);
-    return occ_of((const void*)dispatch_payload_map_kernel);
+    return occupancy_of((const void*)dispatch_payload_map_kernel, kThreads, 0);
 }
 static void launch_payload_checksum(const void* wpv, int grid, void* sv) {
     dispatch_payload_checksum_kernel<<<grid, kThreads, 0, (cudaStream_t)sv>>>(*(const WaveParams*)wpv);
 }
-static int occ_payload_checksum(int) { return occ_of((const void*)dispatch_payload_checksum_kernel); }
+static int occ_payload_checksum(int) { return occupancy_of((const void*)dispatch_payload_checksum_kernel, kThreads, 0); }
 // bit-packed twin of a bool body: range() indices through the body's own 16-index vector routine,
 // explicit argument items through the generic ballot kernel
 static void launch_pi_bits(const void* wpv, int grid, void* sv) {
@@ -165,14 +153,14 @@ static void launch_pi_bits(const void* wpv, int grid, void* sv) {
     else dispatch_bits_items_kernel<PiInsideDet><<<grid, kThreads, 0, (cudaStream_t)sv>>>(wp);
 }
 static int occ_pi_bits(int index_mode) {
-    return index_mode ? occ_of((const void*)dispatch_pi_bits_kernel) : occ_of((const void*)dispatch_bits_items_kernel<PiInsideDet>);
+    return index_mode ? occupancy_of((const void*)dispatch_pi_bits_kernel, kThreads, 0) : occupancy_of((const void*)dispatch_bits_items_kernel<PiInsideDet>, kThreads, 0);
 }
 template <typename T>
 static void launch_parzen(const void* wpv, int grid, void* sv) {
     dispatch_parzen_kernel<T><<<grid, kThreads, 0, (cudaStream_t)sv>>>(*(const WaveParams*)wpv);
 }
 template <typename T>
-static int occ_parzen(int) { return occ_of((const void*)dispatch_parzen_kernel<T>); }
+static int occ_parzen(int) { return occupancy_of((const void*)dispatch_parzen_kernel<T>, kThreads, 0); }
 
 struct BodyEntry {
     std::string name;
@@ -199,21 +187,21 @@ static void builtin_bodies_once() {
         g_bodies.push_back(b);
     };
     // order == enum FuncId (bodies.cuh)
-    add("square_i64", 8, 8, FBR_RES_I64, FBR_BODY_INDEX_ARG | FBR_BODY_SUMMABLE, 4096, launch_thread<SquareI64>, occ_thread<SquareI64>, 0);
-    add("mul2_i64", 16, 8, FBR_RES_I64, FBR_BODY_SUMMABLE, 4096, launch_thread<Mul2I64>, occ_thread<Mul2I64>, 0);
-    add("square_scale_i64", 16, 8, FBR_RES_I64, FBR_BODY_SUMMABLE, 4096, launch_thread<SquareScaleI64>, occ_thread<SquareScaleI64>, 0);
-    add("identity_i64", 8, 8, FBR_RES_I64, FBR_BODY_INDEX_ARG | FBR_BODY_SUMMABLE, 4096, launch_thread<IdentityI64>, occ_thread<IdentityI64>, 0);
-    add("pi_inside_det", 8, 1, FBR_RES_BOOL, FBR_BODY_INDEX_ARG | FBR_BODY_SUMMABLE, 4096, launch_thread<PiInsideDet>, occ_thread<PiInsideDet>, 0);
+    add("square_i64", 8, 8, FBR_RES_I64, FBR_BODY_INDEX_ARG | FBR_BODY_SUMMABLE, 4096, fbr_body_export::launch<SquareI64>, fbr_body_export::occupancy<SquareI64>, 0);
+    add("mul2_i64", 16, 8, FBR_RES_I64, FBR_BODY_SUMMABLE, 4096, fbr_body_export::launch<Mul2I64>, fbr_body_export::occupancy<Mul2I64>, 0);
+    add("square_scale_i64", 16, 8, FBR_RES_I64, FBR_BODY_SUMMABLE, 4096, fbr_body_export::launch<SquareScaleI64>, fbr_body_export::occupancy<SquareScaleI64>, 0);
+    add("identity_i64", 8, 8, FBR_RES_I64, FBR_BODY_INDEX_ARG | FBR_BODY_SUMMABLE, 4096, fbr_body_export::launch<IdentityI64>, fbr_body_export::occupancy<IdentityI64>, 0);
+    add("pi_inside_det", 8, 1, FBR_RES_BOOL, FBR_BODY_INDEX_ARG | FBR_BODY_SUMMABLE, 4096, fbr_body_export::launch<PiInsideDet>, fbr_body_export::occupancy<PiInsideDet>, 0);
     add("parzen_f32", 8, 16, FBR_RES_F64X2, FBR_BODY_NEEDS_SHARED, 1, launch_parzen<float>, occ_parzen<float>, 0);
     add("parzen_f64", 8, 16, FBR_RES_F64X2, FBR_BODY_NEEDS_SHARED, 1, launch_parzen<double>, occ_parzen<double>, 0);
     add("payload_map_4k", 4096, 4096, FBR_RES_BYTES, 0, 32, launch_payload_map, occ_payload_map,
         3 /* few fat CTAs per SM stream read+write waves better than many thin ones */);
     add("payload_checksum_4k", 4096, 4, FBR_RES_U32, FBR_BODY_SUMMABLE, 256, launch_payload_checksum, occ_payload_checksum, 0);
-    add("sleep_f64", 8, 1, FBR_RES_NONE, 0, 1, launch_thread<SleepF64>, occ_thread<SleepF64>, 0);
-    add("fault_identity_i64", 8, 8, FBR_RES_I64, FBR_BODY_INDEX_ARG | FBR_BODY_SUMMABLE, 2, launch_thread<FaultIdentityI64>, occ_thread<FaultIdentityI64>, 0);
+    add("sleep_f64", 8, 1, FBR_RES_NONE, 0, 1, fbr_body_export::launch<SleepF64>, fbr_body_export::occupancy<SleepF64>, 0);
+    add("fault_identity_i64", 8, 8, FBR_RES_I64, FBR_BODY_INDEX_ARG | FBR_BODY_SUMMABLE, 2, fbr_body_export::launch<FaultIdentityI64>, fbr_body_export::occupancy<FaultIdentityI64>, 0);
     // a byte-task = 8 items: 8 range() indices (arg_stride 0) or 8 int64 argument items (arg_stride 64)
     add("pi_inside_bits8", 64, 1, FBR_RES_BITS8, FBR_BODY_INDEX_ARG | FBR_BODY_SUMMABLE, 512, launch_pi_bits, occ_pi_bits, 0);
-    add("trap_identity_i64", 8, 8, FBR_RES_I64, FBR_BODY_INDEX_ARG | FBR_BODY_SUMMABLE, 4096, launch_thread<TrapIdentityI64>, occ_thread<TrapIdentityI64>, 0);
+    add("trap_identity_i64", 8, 8, FBR_RES_I64, FBR_BODY_INDEX_ARG | FBR_BODY_SUMMABLE, 4096, fbr_body_export::launch<TrapIdentityI64>, fbr_body_export::occupancy<TrapIdentityI64>, 0);
 }
 static int body_count() {
     std::lock_guard<std::mutex> g(g_body_mu);
@@ -633,9 +621,9 @@ static void worker_destroy(Worker& w) {
 // every full slot is 16 B aligned on both sides of the gather.
 //
 // Record bodies (FBR_BODY_RECORD): unit_tasks is what one shared-memory stage of dispatch_record_kernel holds, so the
-// unit never exceeds it (rounded DOWN to the chunk and alignment multiples), and the alignment is
-// lcm(16/gcd(16,R), 16/gcd(16,A)) tasks: every full slot AND every unit's argument offset is 16 B aligned, which
-// keeps both sides of the unit on the bulk-copy path (R = 12, 24, 40 need 4, 2, 2 tasks; 16/R would not do).
+// unit never exceeds it (rounded DOWN to the chunk and alignment multiples), and the alignment is the kernel's
+// record::align_tasks(A, R): every full slot AND every unit's argument offset is 16 B aligned, which keeps both sides of
+// the unit on the bulk-copy path (R = 12, 24, 40 need 4, 2, 2 tasks; 16/R would not do).
 // Chunk boundaries coincide with unit boundaries only while lcm(chunksize, align) fits the stage: pick_unit may grow a
 // unit to 2*pref for that, a record unit cannot, so with e.g. chunksize 1023 and align 4 the unit is the stage-sized
 // pref and a chunk may straddle two units (which only changes how tasks are grouped, never a result).
@@ -646,8 +634,7 @@ static uint32_t pick_unit_record(const BodyEntry& b, uint32_t chunksize, uint64_
     const uint64_t per_task = std::max(b.result_bytes, b.arg_bytes);
     while (pref > 1 && (uint64_t)pref * per_task > ring_bytes / 2) pref >>= 1;
     while (pref > 256 && (uint64_t)pref * (uint64_t)sm_count > n_tasks) pref >>= 1;
-    const uint32_t ar = 16u / gcd_u32(16u, b.result_bytes), aa = b.arg_bytes ? 16u / gcd_u32(16u, b.arg_bytes) : 1u;
-    const uint32_t align = ar / gcd_u32(ar, aa) * aa;                       // lcm of two powers of two
+    const uint32_t align = record::align_tasks(b.arg_bytes, b.result_bytes);
     uint32_t unit = pref;
     if (chunksize <= pref) {
         const uint32_t m = chunksize / gcd_u32(chunksize, align) * align;   // lcm(chunksize, align)
@@ -1551,6 +1538,58 @@ int fbr_body_lookup(const char* name, int* func_id) {
     return fail(FBR_ENOENT, "no device body named '%s' is compiled into libfiber_b200 or registered with fbr_register_body", name);
 }
 
+// Why the descriptor `m` of body `name` from `module_path` cannot be registered, or "" when it can.  The rules are checked
+// in a fixed order, so a descriptor that breaks several always gets the same message.
+static std::string descriptor_error(const fbr_body_module_t* m, const char* module_path, const char* name) {
+    if (!m || m->abi != FBR_BODY_MODULE_ABI || m->wave_params_bytes != sizeof(WaveParams) || !m->launch || !m->occupancy || !m->name)
+        return strf("module %s: descriptor ABI %u / wave-parameter size %u do not match this library (%u / %u); rebuild it against include/fiber_b200_body.cuh",
+                    module_path, m ? m->abi : 0u, m ? m->wave_params_bytes : 0u, (unsigned)FBR_BODY_MODULE_ABI, (unsigned)sizeof(WaveParams));
+    if (strcmp(m->name, name) != 0) return strf("module %s exports body '%s', not '%s'", module_path, m->name, name);
+    const bool is_record = (m->flags & FBR_BODY_RECORD) != 0, bcast = (m->flags & FBR_BODY_BROADCAST) != 0;
+    if (!bcast && (m->shared_elem_bytes || m->shared_stage_bytes))
+        return strf("module %s: body '%s' describes a broadcast element but lacks FBR_BODY_BROADCAST", module_path, name);
+    if (bcast && !is_record)
+        return strf("module %s: body '%s': only record bodies take a broadcast block (FBR_BODY_BROADCAST)", module_path, name);
+    const bool items = (m->flags & FBR_BODY_ITEMS) != 0;
+    const char* why = nullptr;
+    if (!items && m->item_bytes) why = "describes an item element but lacks FBR_BODY_ITEMS";
+    else if (items && !is_record) why = "only record bodies take items (FBR_BODY_ITEMS)";
+    else if (items && !record::item_elem_ok(m->item_bytes)) why = "the item size must be 1, 2 or a multiple of 4 up to 4096 bytes";
+    else if (items && (m->flags & FBR_BODY_INDEX_ARG)) why = "an items body cannot take range() indices (FBR_BODY_INDEX_ARG)";
+    if (why) return strf("module %s: body '%s' %s", module_path, name, why);
+    const uint32_t group = m->group_threads;
+    if (group > 1 && (group > 32 || (group & (group - 1)) != 0))
+        return strf("module %s: body '%s': group_threads %u is not 0, 1, 2, 4, 8, 16 or 32", module_path, name, group);
+    if (group > 1 && !is_record)
+        return strf("module %s: body '%s': only record bodies run a task on a group of threads (group_threads %u)", module_path, name, group);
+    if (!is_record) {
+        if (m->result_bytes == 0 || m->unit_tasks == 0 || (m->arg_bytes % 8) != 0 || m->result_kind > FBR_RES_BITS8)
+            return strf("module %s: body '%s' has an invalid record layout", module_path, name);
+        return "";
+    }
+    // staged through shared memory by dispatch_record_kernel: sizes are free within its stages.  A group body's tasks must
+    // also come in 16 B-aligned groups of kAlign that fit one 32 KB stage
+    const uint32_t big = std::max(m->arg_bytes, m->result_bytes);
+    if (m->arg_bytes == 0 && !items) why = "argument bytes may be 0 (no head record, fbr::NoArg) only for an items body (FBR_BODY_ITEMS)";
+    else if (m->result_bytes == 0 || m->arg_bytes % 4 || m->result_bytes % 4) why = "argument and result bytes must be non-zero multiples of 4";
+    else if (group <= 1 && big > record::kThreadRecordBytes) why = "argument and result records are at most 4096 bytes";
+    else if (big > record::kStageBytes) why = "argument and result records of group bodies are at most 32768 bytes";
+    else if ((uint64_t)record::align_tasks(m->arg_bytes, m->result_bytes) * big > record::kStageBytes)
+        why = "one 16 B-aligned group of tasks must fit a 32768-byte stage: kAlign * max(arg_bytes, result_bytes) <= 32768, "
+              "kAlign = 1 when both sizes are multiples of 16, 2 when both are multiples of 8, else 4";
+    else if (m->result_kind != FBR_RES_BYTES) why = "the result kind must be FBR_RES_BYTES (no bit-packed twin)";
+    else if (m->flags & FBR_BODY_SUMMABLE) why = "results cannot be folded on the device (FBR_BODY_SUMMABLE)";
+    else if ((m->flags & FBR_BODY_NEEDS_SHARED) && !bcast)
+        why = "a body without a Shared element type receives no broadcast block (FBR_BODY_NEEDS_SHARED without FBR_BODY_BROADCAST)";
+    else if (bcast && !(m->flags & FBR_BODY_NEEDS_SHARED)) why = "FBR_BODY_BROADCAST needs FBR_BODY_NEEDS_SHARED (its maps must pass a block)";
+    else if (bcast && !record::shared_elem_ok(m->shared_elem_bytes)) why = "the broadcast element must be a non-zero multiple of 4 bytes up to 4096";
+    else if (bcast && m->shared_stage_bytes % 16) why = "the broadcast staging budget must be a multiple of 16 bytes";
+    else if (m->unit_tasks == 0) why = "unit_tasks is 0";
+    else if (record::smem_bytes(m->unit_tasks, m->arg_bytes, m->result_bytes, m->shared_stage_bytes) > record::kSmemBudget)
+        why = "the stages and the broadcast staging budget exceed 200 KB of shared memory";
+    return why ? strf("module %s: record body '%s': %s", module_path, name, why) : "";
+}
+
 int fbr_register_body(const char* name, const char* module_path, const char* entry, int* func_id) {
     if (!name || !module_path || !entry || !func_id) return fail(FBR_EINVAL, "NULL argument");
     // RTLD_LOCAL: several body modules may define the same helper symbols
@@ -1562,81 +1601,10 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
         return fail(FBR_ENOENT, "module %s has no entry point '%s'", module_path, entry);
     }
     const fbr_body_module_t* m = fn();
-    if (!m || m->abi != FBR_BODY_MODULE_ABI || m->wave_params_bytes != sizeof(WaveParams) || !m->launch || !m->occupancy || !m->name) {
-        const unsigned abi = m ? m->abi : 0u, wpb = m ? m->wave_params_bytes : 0u;
+    const std::string err = descriptor_error(m, module_path, name);
+    if (!err.empty()) {
         dlclose(h);
-        return fail(FBR_EINVAL, "module %s: descriptor ABI %u / wave-parameter size %u do not match this library (%u / %u); rebuild it against include/fiber_b200_body.cuh",
-                    module_path, abi, wpb, (unsigned)FBR_BODY_MODULE_ABI, (unsigned)sizeof(WaveParams));
-    }
-    if (strcmp(m->name, name) != 0) {
-        dlclose(h);
-        return fail(FBR_EINVAL, "module %s exports body '%s', not '%s'", module_path, m->name, name);
-    }
-    const bool bcast = (m->flags & FBR_BODY_BROADCAST) != 0;
-    if (!bcast && (m->shared_elem_bytes || m->shared_stage_bytes)) {
-        dlclose(h);
-        return fail(FBR_EINVAL, "module %s: body '%s' describes a broadcast element but lacks FBR_BODY_BROADCAST", module_path, name);
-    }
-    if (bcast && !(m->flags & FBR_BODY_RECORD)) {
-        dlclose(h);
-        return fail(FBR_EINVAL, "module %s: body '%s': only record bodies take a broadcast block (FBR_BODY_BROADCAST)", module_path, name);
-    }
-    const bool items = (m->flags & FBR_BODY_ITEMS) != 0;
-    {
-        const char* why = nullptr;
-        const uint32_t e = m->item_bytes;
-        if (!items && m->item_bytes) why = "describes an item element but lacks FBR_BODY_ITEMS";
-        else if (items && !(m->flags & FBR_BODY_RECORD)) why = "only record bodies take items (FBR_BODY_ITEMS)";
-        else if (items && !(e == 1 || e == 2 || (e % 4 == 0 && e >= 4 && e <= 4096)))
-            why = "the item size must be 1, 2 or a multiple of 4 up to 4096 bytes";
-        else if (items && (m->flags & FBR_BODY_INDEX_ARG)) why = "an items body cannot take range() indices (FBR_BODY_INDEX_ARG)";
-        if (why) {
-            dlclose(h);
-            return fail(FBR_EINVAL, "module %s: body '%s' %s", module_path, name, why);
-        }
-    }
-    const uint32_t group = m->group_threads;
-    if (group > 1 && (group > 32 || (group & (group - 1)) != 0)) {
-        dlclose(h);
-        return fail(FBR_EINVAL, "module %s: body '%s': group_threads %u is not 0, 1, 2, 4, 8, 16 or 32", module_path, name, group);
-    }
-    if (group > 1 && !(m->flags & FBR_BODY_RECORD)) {
-        dlclose(h);
-        return fail(FBR_EINVAL, "module %s: body '%s': only record bodies run a task on a group of threads (group_threads %u)", module_path, name, group);
-    }
-    if (m->flags & FBR_BODY_RECORD) {
-        // staged through shared memory by dispatch_record_kernel: sizes are free within its stages.  A group body's
-        // tasks must also come in 16 B-aligned groups of kAlign that fit one 32 KB stage
-        const uint32_t big = std::max(m->arg_bytes, m->result_bytes);
-        const uint32_t align = (m->arg_bytes % 16 == 0 && m->result_bytes % 16 == 0) ? 1u
-                             : (m->arg_bytes % 8 == 0 && m->result_bytes % 8 == 0) ? 2u : 4u;
-        const char* why = nullptr;
-        if (m->arg_bytes == 0 && !items) why = "argument bytes may be 0 (no head record, fbr::NoArg) only for an items body (FBR_BODY_ITEMS)";
-        else if (m->result_bytes == 0 || m->arg_bytes % 4 || m->result_bytes % 4) why = "argument and result bytes must be non-zero multiples of 4";
-        else if (group <= 1 && big > 4096) why = "argument and result records are at most 4096 bytes";
-        else if (big > 32768) why = "argument and result records of group bodies are at most 32768 bytes";
-        else if ((uint64_t)align * big > 32768)
-            why = "one 16 B-aligned group of tasks must fit a 32768-byte stage: kAlign * max(arg_bytes, result_bytes) <= 32768, "
-                  "kAlign = 1 when both sizes are multiples of 16, 2 when both are multiples of 8, else 4";
-        else if (m->result_kind != FBR_RES_BYTES) why = "the result kind must be FBR_RES_BYTES (no bit-packed twin)";
-        else if (m->flags & FBR_BODY_SUMMABLE) why = "results cannot be folded on the device (FBR_BODY_SUMMABLE)";
-        else if ((m->flags & FBR_BODY_NEEDS_SHARED) && !bcast)
-            why = "a body without a Shared element type receives no broadcast block (FBR_BODY_NEEDS_SHARED without FBR_BODY_BROADCAST)";
-        else if (bcast && !(m->flags & FBR_BODY_NEEDS_SHARED)) why = "FBR_BODY_BROADCAST needs FBR_BODY_NEEDS_SHARED (its maps must pass a block)";
-        else if (bcast && (m->shared_elem_bytes == 0 || m->shared_elem_bytes % 4 || m->shared_elem_bytes > 4096))
-            why = "the broadcast element must be a non-zero multiple of 4 bytes up to 4096";
-        else if (bcast && m->shared_stage_bytes % 16) why = "the broadcast staging budget must be a multiple of 16 bytes";
-        else if (m->unit_tasks == 0) why = "unit_tasks is 0";
-        // dispatch_record_kernel's shared memory: two IN and two OUT stages of one unit each, then the broadcast region
-        else if (2ull * m->unit_tasks * (m->arg_bytes + m->result_bytes) + m->shared_stage_bytes > (200ull << 10))
-            why = "the stages and the broadcast staging budget exceed 200 KB of shared memory";
-        if (why) {
-            dlclose(h);
-            return fail(FBR_EINVAL, "module %s: record body '%s': %s", module_path, name, why);
-        }
-    } else if (m->result_bytes == 0 || m->unit_tasks == 0 || (m->arg_bytes % 8) != 0 || m->result_kind > FBR_RES_BITS8) {
-        dlclose(h);
-        return fail(FBR_EINVAL, "module %s: body '%s' has an invalid record layout", module_path, name);
+        return fail(FBR_EINVAL, "%s", err.c_str());
     }
     std::lock_guard<std::mutex> g(g_body_mu);
     builtin_bodies_once();

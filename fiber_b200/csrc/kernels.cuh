@@ -928,7 +928,7 @@ __global__ void __launch_bounds__(160) dispatch_payload_map_tma_kernel(const Wav
 // i's record starts at i * A -- a body that walks a large record word by word has every lane on the same bank
 // (A = 1024: 32-way); reading it in 16 B vectors cuts that to 8-way.  A stage holds kStageBytes of the larger
 // record, so for large records most consumers are idle during B::run (A = 1024: 32 tasks per unit).
-// Group bodies (kGroup = G) answer both: G lanes run each task (run_group_unit), reading consecutive words of one
+// Group bodies (kGroup = G) answer both: G lanes run each task (run_unit), reading consecutive words of one
 // record, and their records may fill a whole stage (32 KB, one task per unit).
 // Bodies with a Shared element type also receive the map's broadcast block: one within the body's kSharedStage is
 // bulk-loaded once per CTA into a region after the stages (DESIGN.md section 4 has the staged vs global measurement).
@@ -968,6 +968,20 @@ constexpr int kThreads = 32 + kConsumers;
 constexpr int kInStages = 2, kOutStages = 2;
 constexpr uint32_t kStageBytes = 32768;   // per stage, for the larger of A and R
 constexpr uint32_t kMaxUnit = 1024;       // tasks per unit: 4 per consumer thread
+constexpr uint32_t kThreadRecordBytes = 4096;   // the largest record of a one-thread body (group bodies: kStageBytes)
+constexpr uint64_t kSmemBudget = 200u << 10;    // dynamic shared memory: the stages plus the broadcast region
+
+// tasks per unit that make count * A and count * R multiples of 16 (A and R are multiples of 4)
+constexpr uint32_t align_tasks(uint32_t A, uint32_t R) {
+    return (A % 16 == 0 && R % 16 == 0) ? 1u : (A % 8 == 0 && R % 8 == 0) ? 2u : 4u;
+}
+// dynamic shared memory of dispatch_record_kernel: the IN and OUT stages of `unit` tasks, then the broadcast region
+// (A = 0: range() maps and NoArg bodies read no argument bytes)
+constexpr uint64_t smem_bytes(uint32_t unit, uint32_t A, uint32_t R, uint32_t stage) {
+    return (uint64_t)kInStages * unit * A + (uint64_t)kOutStages * unit * R + stage;
+}
+constexpr bool item_elem_ok(uint32_t e) { return e == 1 || e == 2 || (e % 4 == 0 && e >= 4 && e <= 4096); }
+constexpr bool shared_elem_ok(uint32_t e) { return e != 0 && e % 4 == 0 && e <= 4096; }
 
 // A record body opts into the broadcast block with `using Shared = <element>;` and `static constexpr uint32_t
 // kSharedStage = <bytes>;`; its run() then takes a const Broadcast<Shared>& after the result.
@@ -982,7 +996,7 @@ struct BroadcastOf<B, std::void_t<typename B::Shared>> {
     static constexpr bool kOn = true;
     static constexpr uint32_t kElem = (uint32_t)sizeof(T), kStage = B::kSharedStage;
     static_assert(std::is_trivially_copyable<T>::value, "broadcast bodies: Shared is trivially copyable");
-    static_assert(kElem % 4 == 0 && kElem <= 4096, "broadcast bodies: sizeof(Shared) is a multiple of 4 up to 4096");
+    static_assert(shared_elem_ok(kElem), "broadcast bodies: sizeof(Shared) is a multiple of 4 up to 4096");
     static_assert(kStage % 16 == 0, "broadcast bodies: kSharedStage is a multiple of 16 (0: never stage)");
 };
 
@@ -1011,7 +1025,7 @@ struct ItemsOf<B, std::void_t<typename B::Item>> {
     static constexpr bool kOn = true;
     static constexpr uint32_t kElem = (uint32_t)sizeof(T);
     static_assert(std::is_trivially_copyable<T>::value, "items bodies: Item is trivially copyable");
-    static_assert(kElem == 1 || kElem == 2 || (kElem % 4 == 0 && kElem <= 4096), "items bodies: sizeof(Item) is 1, 2 or a multiple of 4 up to 4096");
+    static_assert(item_elem_ok(kElem), "items bodies: sizeof(Item) is 1, 2 or a multiple of 4 up to 4096");
     static_assert(!B::kIndexArg, "items bodies cannot take range() indices (kIndexArg)");
 };
 
@@ -1020,14 +1034,13 @@ struct Layout {
     static constexpr bool kNoArg = std::is_same<typename B::Arg, NoArg>::value;
     static constexpr uint32_t A = kNoArg ? 0u : (uint32_t)sizeof(typename B::Arg), R = (uint32_t)sizeof(typename B::Res);
     static_assert(!kNoArg || ItemsOf<B>::kOn, "record bodies: only an items body may have no argument record (NoArg)");
-    static_assert(GroupOf<B>::kG > 1 || (A % 4 == 0 && R % 4 == 0 && (A >= 4 || kNoArg) && R >= 4 && A <= 4096 && R <= 4096),
+    static_assert(GroupOf<B>::kG > 1 || (A % 4 == 0 && R % 4 == 0 && (A >= 4 || kNoArg) && R >= 4 && A <= kThreadRecordBytes && R <= kThreadRecordBytes),
                   "record bodies: sizeof(Arg) and sizeof(Res) are multiples of 4 between 4 and 4096");
     static_assert(GroupOf<B>::kG == 1 || (A % 4 == 0 && R % 4 == 0 && (A >= 4 || kNoArg) && R >= 4 && A <= kStageBytes && R <= kStageBytes),
                   "group record bodies: sizeof(Arg) and sizeof(Res) are multiples of 4 between 4 and 32768");
     // the broadcast region after the IN / OUT stages (0 bytes for bodies without a Shared type)
     static constexpr uint32_t kShared = BroadcastOf<B>::kStage;
-    // tasks per unit that make count * A and count * R multiples of 16 (A and R are multiples of 4)
-    static constexpr uint32_t kAlign = ((A % 16 == 0) && (R % 16 == 0)) ? 1u : ((A % 8 == 0) && (R % 8 == 0)) ? 2u : 4u;
+    static constexpr uint32_t kAlign = align_tasks(A, R);
     static_assert(GroupOf<B>::kG == 1 || kAlign * (A > R ? A : R) <= kStageBytes,
                   "group record bodies: one 16 B-aligned group of tasks fits a stage (kAlign * max(sizeof(Arg), sizeof(Res)) <= 32768)");
     static constexpr uint32_t unit() {
@@ -1039,11 +1052,8 @@ struct Layout {
     static constexpr uint32_t kUnit = unit();
     static constexpr uint32_t kInBytes = kUnit * A, kOutBytes = kUnit * R;   // multiples of 16
     // dynamic shared memory of an instantiation: range() maps (index) read no argument bytes and have no IN stages
-    static constexpr size_t stages(bool index) {
-        return (index ? 0 : (size_t)kInStages * kInBytes) + (size_t)kOutStages * kOutBytes;
-    }
-    static constexpr size_t smem(bool index) { return stages(index) + kShared; }
-    static_assert(kInBytes % 16 == 0 && kOutBytes % 16 == 0 && smem(false) <= (200u << 10), "record stage layout");
+    static constexpr size_t smem(bool index) { return smem_bytes(kUnit, index ? 0u : A, R, kShared); }
+    static_assert(kInBytes % 16 == 0 && kOutBytes % 16 == 0 && smem(false) <= kSmemBudget, "record stage layout");
 };
 
 // contiguous copy by `n` threads; 16 B vectors while both sides are 16 B aligned, then 4 B words, then bytes
@@ -1076,59 +1086,47 @@ __device__ __forceinline__ void gather_records(uint8_t* dst, const uint8_t* src,
     }
 }
 
-// One unit of a group body (kGroup = G > 1): consumer ct is rank ct % G of group ct / G, and group g runs tasks g,
-// g + C/G, ...  All G lanes of a group see the same i, so the group stays converged through B::run.  `sh` is the
-// broadcast block of a body that has one (nothing otherwise).
+// The G lanes that run consumer ct's task in a group body: ct is rank ct % G of group ct / G (consumers start at thread
+// 32, so ct % 32 is the lane)
+template <uint32_t G>
+__device__ __forceinline__ Group<G> group_of(uint32_t ct) {
+    return Group<G>{ct % G, (G == 32 ? 0xffffffffu : ((1u << G) - 1u) << ((ct & 31u) & ~(G - 1u)))};
+}
+
+// One unit of a record body: group g = ct / G runs tasks g, g + C/G, ... (G = 1: one thread per task).  All G lanes of a
+// group see the same i, so the group stays converged through B::run.  run() gets, in order: the head argument (a range()
+// index, a record from `in`, or none for NoArg), the task's items, the result, the broadcast block `sh` (bodies that have
+// one), the group (G > 1), then task_index, es and attempt.  An items task reads offsets o[i], o[i+1] and its items from
+// global memory; one whose offsets decrease or leave [item_base, item_count] reports TASK_BADARG and its body is not called.
 template <class B, bool kIndex, class... Sh>
-__device__ __forceinline__ void run_group_unit(const WaveParams& wp, const TaskRecord& rec, const uint8_t* in, uint8_t* out,
-                                               uint32_t ct, const ErrSink& es, const Sh&... sh) {
+__device__ __forceinline__ void run_unit(const WaveParams& wp, const TaskRecord& rec, const uint8_t* in, uint8_t* out,
+                                         uint32_t ct, const ErrSink& es, const Sh&... sh) {
     using L = Layout<B>;
     using Arg = typename B::Arg;
     using Res = typename B::Res;
     constexpr uint32_t G = GroupOf<B>::kG, C = kConsumers;
-    const uint32_t lane = ct & 31u;         // consumers start at thread 32: ct % 32 is the lane
-    const Group<G> grp{ct % G, (G == 32 ? 0xffffffffu : ((1u << G) - 1u) << (lane & ~(G - 1u)))};
     const uint64_t g0 = wp.index_base + rec.first;
+    const uint64_t* const o = wp.item_offs + (rec.first - wp.item_first);   // items bodies: the unit's offsets
     for (uint32_t i = ct / G; i < rec.count; i += C / G) {
-        Res& r = *reinterpret_cast<Res*>(out + (size_t)i * L::R);
-        if constexpr (kIndex) {
-            const Arg a = (Arg)(wp.index_start + (int64_t)(rec.first + i) * wp.index_step);
-            B::run(a, r, sh..., grp, g0 + i, es, rec.attempt);
-        } else {
-            B::run(*reinterpret_cast<const Arg*>(in + (size_t)i * L::A), r, sh..., grp, g0 + i, es, rec.attempt);
-        }
-    }
-}
-
-// One unit of an items body (one thread or a group per task, like the loops above): task i reads offsets o[i], o[i+1]
-// and its items from global memory; a task whose offsets decrease or leave [item_base, item_count] reports TASK_BADARG
-// and its body is not called.  `sh` is the broadcast block of a body that has one.
-template <class B, class... Sh>
-__device__ __forceinline__ void run_items_unit(const WaveParams& wp, const TaskRecord& rec, const uint8_t* in, uint8_t* out,
-                                               uint32_t ct, const ErrSink& es, const Sh&... sh) {
-    using L = Layout<B>;
-    using T = typename ItemsOf<B>::T;
-    using Res = typename B::Res;
-    constexpr uint32_t G = GroupOf<B>::kG, C = kConsumers;
-    const uint64_t* o = wp.item_offs + (rec.first - wp.item_first);
-    const uint64_t g0 = wp.index_base + rec.first;
-    for (uint32_t i = ct / G; i < rec.count; i += C / G) {
-        const uint64_t a = o[i], b = o[i + 1];
-        if (a > b || a < wp.item_base || b > wp.item_count) {
-            if (ct % G == 0) es.report(TASK_BADARG, g0 + i);
-            continue;
-        }
-        const Items<T> x{reinterpret_cast<const T*>(wp.items + (a - wp.item_base) * sizeof(T)), b - a};
-        Res& r = *reinterpret_cast<Res*>(out + (size_t)i * L::R);
-        auto call = [&](const auto&... grp) {
-            if constexpr (L::kNoArg) B::run(x, r, sh..., grp..., g0 + i, es, rec.attempt);
-            else B::run(*reinterpret_cast<const typename B::Arg*>(in + (size_t)i * L::A), x, r, sh..., grp..., g0 + i, es, rec.attempt);
+        auto res = [&]() -> Res& { return *reinterpret_cast<Res*>(out + (size_t)i * L::R); };
+        auto call = [&](Res& r, const auto&... head) {  // head: the head argument, then the items
+            if constexpr (G > 1) B::run(head..., r, sh..., group_of<G>(ct), g0 + i, es, rec.attempt);
+            else B::run(head..., r, sh..., g0 + i, es, rec.attempt);
         };
-        if constexpr (G > 1) {
-            const uint32_t lane = ct & 31u;
-            call(Group<G>{ct % G, (G == 32 ? 0xffffffffu : ((1u << G) - 1u) << (lane & ~(G - 1u)))});
+        if constexpr (kIndex) {
+            call(res(), (Arg)(wp.index_start + (int64_t)(rec.first + i) * wp.index_step));
+        } else if constexpr (ItemsOf<B>::kOn) {
+            using T = typename ItemsOf<B>::T;
+            const uint64_t a = o[i], b = o[i + 1];
+            if (a > b || a < wp.item_base || b > wp.item_count) {
+                if (ct % G == 0) es.report(TASK_BADARG, g0 + i);
+                continue;
+            }
+            const Items<T> x{reinterpret_cast<const T*>(wp.items + (a - wp.item_base) * sizeof(T)), b - a};
+            if constexpr (L::kNoArg) call(res(), x);
+            else call(res(), *reinterpret_cast<const Arg*>(in + (size_t)i * L::A), x);
         } else {
-            call();
+            call(res(), *reinterpret_cast<const Arg*>(in + (size_t)i * L::A));
         }
     }
 }
@@ -1138,8 +1136,6 @@ template <class B, bool kIndex>
 __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const WaveParams wp) {
     using namespace bulk;
     using L = record::Layout<B>;
-    using Arg = typename B::Arg;
-    using Res = typename B::Res;
     constexpr int kIn = record::kInStages, kOut = record::kOutStages;
     constexpr uint32_t C = record::kConsumers;
     extern __shared__ __align__(128) uint8_t smem[];
@@ -1154,7 +1150,7 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
     // (a run-time choice, uniform across the launch), else run() reads it from global memory
     using Bc = record::BroadcastOf<B>;
     uint64_t* bcast_full = nullptr;
-    uint8_t* const bcast_stage = out_stage + (size_t)kOut * L::kOutBytes;   // L::stages(kIndex) bytes in
+    uint8_t* const bcast_stage = out_stage + (size_t)kOut * L::kOutBytes;   // after the IN and OUT stages
     bool staged = false;
     uint32_t bcast_bulk = 0;                           // bytes of the block the bulk load brings (the rest: consumers)
     if constexpr (Bc::kOn && Bc::kStage > 0) {
@@ -1163,8 +1159,6 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
         staged = wp.shared_bytes <= Bc::kStage;
         if ((reinterpret_cast<uintptr_t>(wp.shared) & 15) == 0) bcast_bulk = (uint32_t)wp.shared_bytes & ~15u;
     }
-    // items bodies read each task's items from global memory (run_items_unit)
-    using It = record::ItemsOf<B>;
     constexpr bool kArgs = !kIndex && L::A > 0;          // NoArg items bodies have no argument records
     if (threadIdx.x == 0) {
         for (int s = 0; s < kIn; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], C); }
@@ -1252,50 +1246,21 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
 
         int* const unit_fault = &s_fault[seq & 1];
         const ErrSink es{wp.err_word, unit_fault};
-        const uint64_t g0 = wp.index_base + rec.first;
-        if constexpr (It::kOn) {
-            // one loop per placement of the broadcast block, so each sees its pointer's address space
-            if constexpr (Bc::kOn) {
-                using T = typename Bc::T;
-                const uint64_t n_elems = wp.shared_bytes / Bc::kElem;
-                const uint8_t* blk = staged ? bcast_stage : wp.shared;
-                record::run_items_unit<B>(wp, rec, in, out, ct, es, Broadcast<T>{reinterpret_cast<const T*>(blk), n_elems});
-            } else {
-                record::run_items_unit<B>(wp, rec, in, out, ct, es);
-            }
-        } else if constexpr (!Bc::kOn && record::GroupOf<B>::kG > 1) {
-            record::run_group_unit<B, kIndex>(wp, rec, in, out, ct, es);
-        } else if constexpr (!Bc::kOn) {
-            for (uint32_t i = ct; i < rec.count; i += C) {
-                Res& r = *reinterpret_cast<Res*>(out + (size_t)i * L::R);
-                if constexpr (kIndex) {
-                    const Arg a = (Arg)(wp.index_start + (int64_t)(rec.first + i) * wp.index_step);
-                    B::run(a, r, g0 + i, es, rec.attempt);
-                } else {
-                    B::run(*reinterpret_cast<const Arg*>(in + (size_t)i * L::A), r, g0 + i, es, rec.attempt);
-                }
-            }
+        if constexpr (!Bc::kOn) {
+            record::run_unit<B, kIndex>(wp, rec, in, out, ct, es);
         } else {
             using T = typename Bc::T;
-            // one loop per placement of the block, so each sees its pointer's address space (shared or global loads)
-            auto run_unit = [&](const Broadcast<T>& sh) {
-                if constexpr (record::GroupOf<B>::kG > 1) {
-                    record::run_group_unit<B, kIndex>(wp, rec, in, out, ct, es, sh);
-                } else {
-                    for (uint32_t i = ct; i < rec.count; i += C) {
-                        Res& r = *reinterpret_cast<Res*>(out + (size_t)i * L::R);
-                        if constexpr (kIndex) {
-                            const Arg a = (Arg)(wp.index_start + (int64_t)(rec.first + i) * wp.index_step);
-                            B::run(a, r, sh, g0 + i, es, rec.attempt);
-                        } else {
-                            B::run(*reinterpret_cast<const Arg*>(in + (size_t)i * L::A), r, sh, g0 + i, es, rec.attempt);
-                        }
-                    }
-                }
-            };
             const uint64_t n_elems = wp.shared_bytes / Bc::kElem;
-            if (staged) run_unit(Broadcast<T>{reinterpret_cast<const T*>(bcast_stage), n_elems});
-            else run_unit(Broadcast<T>{reinterpret_cast<const T*>(wp.shared), n_elems});
+            // one loop per placement of the block, so each sees its pointer's address space (shared or global loads);
+            // an items body keeps one loop over a generic pointer, because two such loops made ptxas spill
+            if constexpr (record::ItemsOf<B>::kOn) {
+                const uint8_t* blk = staged ? bcast_stage : wp.shared;
+                record::run_unit<B, kIndex>(wp, rec, in, out, ct, es, Broadcast<T>{reinterpret_cast<const T*>(blk), n_elems});
+            } else {
+                auto run = [&](const Broadcast<T>& sh) { record::run_unit<B, kIndex>(wp, rec, in, out, ct, es, sh); };
+                if (staged) run(Broadcast<T>{reinterpret_cast<const T*>(bcast_stage), n_elems});
+                else run(Broadcast<T>{reinterpret_cast<const T*>(wp.shared), n_elems});
+            }
         }
         // generic-proxy writes of this unit's stages become visible to the async proxy (the bulk store below, the
         // next bulk load into the IN stage); then the IN stage goes back to the producer

@@ -105,43 +105,38 @@ def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_
     _abi.check(L.fbr_register_body(name.encode(), str(module_path).encode(), entry.encode(), ctypes.byref(fid)))
     info = _abi.BodyInfo()
     _abi.check(L.fbr_body_info(fid.value, ctypes.byref(info)))
-    record = None
-    if info.flags & _abi.FBR_BODY_ITEMS:
-        if result is None or items is None:
-            raise ValueError("items body %s: pass result=<dtype> and items=(<parameter name>, <element dtype>)" % name)
-        ib = ctypes.c_uint32(0)
-        _abi.check(L.fbr_body_items_info(fid.value, ctypes.byref(ib)))
-        elem, stage = ctypes.c_uint32(0), ctypes.c_uint32(0)
-        if info.flags & _abi.FBR_BODY_BROADCAST:
-            if shared is None:
-                raise ValueError("items body %s reads a broadcast block: pass shared=(<parameter name>, <element dtype>)" % name)
-            _abi.check(L.fbr_body_shared_info(fid.value, ctypes.byref(elem), ctypes.byref(stage)))
-        elif shared is not None:
-            raise ValueError("body %s reads no broadcast block (its record struct has no Shared element type): shared= is "
-                             "for broadcast bodies only" % name)
-        # args left at its default means no head record for a body that has none
-        head = None if (isinstance(args, str) and args == "i64" and info.arg_bytes == 0) else args
-        record = _Items(info, items, head, result, shared, ib.value, elem.value, stage.value)
-        args, result, items = record.arg_dtype, record.res_dtype, (record.item_name, record.item_dtype)
-        shared = (record.shared_name, record.shared_dtype) if record.shared_name is not None else None
-    elif items is not None:
+    has_items, has_shared = info.flags & _abi.FBR_BODY_ITEMS, info.flags & _abi.FBR_BODY_BROADCAST
+    if items is not None and not has_items:
         raise ValueError("body %s takes no items (its record struct has no Item element type): items= is for items bodies "
                          "only" % name)
-    elif info.flags & _abi.FBR_BODY_BROADCAST:
-        if result is None or shared is None:
-            raise ValueError("broadcast body %s: pass result=<dtype> and shared=(<parameter name>, <element dtype>)" % name)
-        elem, stage = ctypes.c_uint32(0), ctypes.c_uint32(0)
-        _abi.check(L.fbr_body_shared_info(fid.value, ctypes.byref(elem), ctypes.byref(stage)))
-        record = _Broadcast(info, args, result, shared, elem.value, stage.value)   # validates all three layouts
-        args, result, shared = record.arg_dtype, record.res_dtype, (record.shared_name, record.shared_dtype)
-    elif shared is not None:
+    if has_items and (result is None or items is None):
+        raise ValueError("items body %s: pass result=<dtype> and items=(<parameter name>, <element dtype>)" % name)
+    if has_shared and (result is None or shared is None):
+        raise ValueError(("items body %s reads a broadcast block: pass shared=(<parameter name>, <element dtype>)" if has_items
+                          else "broadcast body %s: pass result=<dtype> and shared=(<parameter name>, <element dtype>)") % name)
+    if shared is not None and not has_shared:
         raise ValueError("body %s reads no broadcast block (its record struct has no Shared element type): shared= is "
                          "for broadcast bodies only" % name)
-    elif info.flags & _abi.FBR_BODY_RECORD:
+    record = None
+    if info.flags & _abi.FBR_BODY_RECORD:
         if result is None:
             raise ValueError("record body %s: pass result=<dtype> (its %d-byte result record)" % (name, info.result_bytes))
-        record = _Record(info, args, result)        # validates both layouts against the module
+        elem, stage, ib = ctypes.c_uint32(0), ctypes.c_uint32(0), ctypes.c_uint32(0)
+        if has_shared:
+            _abi.check(L.fbr_body_shared_info(fid.value, ctypes.byref(elem), ctypes.byref(stage)))
+        if has_items:
+            _abi.check(L.fbr_body_items_info(fid.value, ctypes.byref(ib)))
+            # args left at its default means no head record for a body that has none
+            head = None if (isinstance(args, str) and args == "i64" and info.arg_bytes == 0) else args
+            record = _Items(info, items, head, result, shared, ib.value, elem.value, stage.value)
+            items = (record.item_name, record.item_dtype)
+        elif has_shared:
+            record = _Broadcast(info, args, result, shared, elem.value, stage.value)
+        else:
+            record = _Record(info, args, result)        # validates the layouts against the module
         args, result = record.arg_dtype, record.res_dtype
+        if shared is not None:
+            shared = (record.shared_name, record.shared_dtype)
     elif result is not None:
         raise ValueError("body %s is not a record body (FBR_EXPORT_RECORD_BODY): its result layout is fixed" % name)
     old = specs.get(name)
@@ -481,14 +476,18 @@ class _Record(BodySpec):
 
     def __init__(self, info, args, result):
         super().__init__(info)
-        self.arg_dtype = _record_dtype(args, "argument", self.name)
+        # args=None for a body without argument bytes: an items body with no head record (fbr::NoArg), no argument fields
+        self.arg_dtype = None if args is None and not self.arg_bytes else _record_dtype(args, "argument", self.name)
         self.res_dtype = _record_dtype(result, "result", self.name)
-        if self.arg_dtype.itemsize != self.arg_bytes:
+        if self.arg_dtype is not None and self.arg_dtype.itemsize != self.arg_bytes:
             raise ValueError("%s: argument dtype %s is %d bytes, the body's argument record is %d"
                              % (self.name, self.arg_dtype, self.arg_dtype.itemsize, self.arg_bytes))
         if self.res_dtype.itemsize != self.result_bytes:
             raise ValueError("%s: result dtype %s is %d bytes, the body's result record is %d"
                              % (self.name, self.res_dtype, self.res_dtype.itemsize, self.result_bytes))
+        if self.arg_dtype is None:
+            self.params, self._sdt, self._fields = None, None, ()
+            return
         self.params = self.arg_dtype.names                 # None: one positional-only parameter
         # the argument records as a structured array with named fields (one field "_0" when the dtype has none)
         self._sdt = self.arg_dtype if self.params else np.dtype([("_0", self.arg_dtype)])
@@ -677,17 +676,20 @@ class _Broadcast(_Record):
             raise TypeError("%s: the initializer takes exactly one argument (%s), got %d" % (self.name, self.shared_name, len(initargs)))
         return self._blocks.get((self._block_array(initargs[0]),), _block_bytes)
 
-    def _encode(self, items, fast, apply=False):
-        if fast:
-            return super()._encode(items, fast)              # map(f, points): the block is the initializer's
-        n_params = len(self._fields)
-        rows, first, block, carried = [], None, None, None      # first: the first item's array; block: its element view
+    def _calls(self, items, apply, n_rest):
+        """Each item's ``(args, kwds)`` without the broadcast array, with the array's element view so far (None until an
+        item passes it).  An item passes the array by keyword, or first when it has one more argument than the ``n_rest``
+        other parameters take.  Every item of a map passes it or none does, and all pass the same elements."""
+        first = block = carried = None      # first: the first item's array; block: its element view
         for it in items:
             args, kwds = self._split(it, apply)
+            if self.shared_name is None:    # an items body without a broadcast block
+                yield args, kwds, None
+                continue
             if self.shared_name in kwds:
                 kwds = dict(kwds)
                 b = kwds.pop(self.shared_name)
-            elif args and len(args) + len(kwds) > n_params:    # one more argument than the record has fields
+            elif args and len(args) + len(kwds) > n_rest:
                 b, args = args[0], tuple(args[1:])
             else:
                 b = _MISSING
@@ -703,6 +705,13 @@ class _Broadcast(_Record):
                     first, block = b, self._block_array(b)
                 elif b is not first and not _same_bytes(self._block_array(b), block):
                     raise ValueError("%s: all tasks of one map must share %s" % (self.name, self.shared_name))
+            yield args, kwds, block
+
+    def _encode(self, items, fast, apply=False):
+        if fast:
+            return super()._encode(items, fast)              # map(f, points): the block is the initializer's
+        rows, block = [], None
+        for args, kwds, block in self._calls(items, apply, len(self._fields)):
             rows.append(self._bind(args, kwds))
         enc = self._columns([list(c) for c in zip(*rows)] if rows else [[] for _ in self._fields])
         enc.shared = self._blocks.get((block,), _block_bytes) if block is not None else None
@@ -808,17 +817,9 @@ class _Items(_Broadcast):
     other parameter."""
 
     def __init__(self, info, items, args, result, shared, item_bytes, shared_elem=0, shared_stage=0):
-        if args is None:
-            if info.arg_bytes:
-                raise ValueError("%s: args=None, but the body's head record is %d bytes" % (info.name.decode(), info.arg_bytes))
-            BodySpec.__init__(self, info)
-            self.arg_dtype, self.params, self._sdt, self._fields = None, None, None, ()
-            self.res_dtype = _record_dtype(result, "result", self.name)
-            if self.res_dtype.itemsize != self.result_bytes:
-                raise ValueError("%s: result dtype %s is %d bytes, the body's result record is %d"
-                                 % (self.name, self.res_dtype, self.res_dtype.itemsize, self.result_bytes))
-        else:
-            _Record.__init__(self, info, args, result)
+        if args is None and info.arg_bytes:
+            raise ValueError("%s: args=None, but the body's head record is %d bytes" % (info.name.decode(), info.arg_bytes))
+        _Record.__init__(self, info, args, result)
         self.shared_name = self.shared_dtype = None
         if shared is not None:
             self._init_shared(shared, shared_elem, shared_stage)
@@ -846,28 +847,9 @@ class _Items(_Broadcast):
             if self.arg_dtype is None:      # map(f, xs): each item is one task's items; a broadcast block is the initializer's
                 return self._with_items(Encoded(0), items)
             items = [(it,) for it in items]
-        n_fields = len(self._fields)
-        xs, rows, first, block, carried = [], [], None, None, None
-        for it in items:
-            args, kwds = self._split(it, apply)
+        xs, rows, block = [], [], None
+        for args, kwds, block in self._calls(items, apply, 1 + len(self._fields)):    # the items and the record's fields
             kwds = dict(kwds)
-            if self.shared_name is not None:
-                if self.shared_name in kwds:
-                    b = kwds.pop(self.shared_name)
-                elif args and len(args) + len(kwds) > 1 + n_fields:    # one more argument than the items and the record
-                    b, args = args[0], tuple(args[1:])
-                else:
-                    b = _MISSING
-                has = b is not _MISSING
-                if carried is None:
-                    carried = has
-                elif carried != has:
-                    raise TypeError("%s: mixed items with and without %s in one map" % (self.name, self.shared_name))
-                if has:
-                    if first is None:
-                        first, block = b, self._block_array(b)
-                    elif b is not first and not _same_bytes(self._block_array(b), block):
-                        raise ValueError("%s: all tasks of one map must share %s" % (self.name, self.shared_name))
             if self.item_name in kwds:
                 x = kwds.pop(self.item_name)
             elif args:

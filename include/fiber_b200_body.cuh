@@ -15,8 +15,7 @@
 //     };
 //     FBR_EXPORT_THREAD_BODY(Collatz, "collatz_steps", collatz_entry, FBR_RES_I64, FBR_BODY_INDEX_ARG | FBR_BODY_SUMMABLE)
 //
-//     nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -shared -Xcompiler -fPIC \
-//          -I<repo>/include -I<repo>/fiber_b200/csrc body.cu -o libbody.so
+//     nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -shared -Xcompiler -fPIC -I<repo>/include -I<repo>/fiber_b200/csrc body.cu -o libbody.so
 //     fbr_register_body("collatz_steps", "libbody.so", "collatz_entry", &func_id);
 //
 // (fiber_b200.device_body(name, source=...) does the last two steps from Python.)  The body is instantiated
@@ -116,6 +115,13 @@
 #include <type_traits>
 
 namespace fbr_body_export {
+// CTAs of `kernel` per SM, at least 1 (a failed query leaves no sticky error behind)
+inline int occupancy_of(const void* kernel, int threads, size_t smem) {
+    int occ = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, threads, smem) != cudaSuccess) { cudaGetLastError(); return 1; }
+    return occ > 0 ? occ : 1;
+}
+
 template <class B>
 void launch(const void* wpv, int grid, void* sv) {
     const fbr::WaveParams& wp = *(const fbr::WaveParams*)wpv;
@@ -130,22 +136,12 @@ void launch(const void* wpv, int grid, void* sv) {
 }
 template <class B>
 int occupancy(int index_mode) {
-    int occ = 0;
-    cudaError_t e;
     if constexpr (B::kIndexArg) {
-        if (index_mode) {
-            e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, (const void*)fbr::dispatch_thread_kernel<B, true>, fbr::kThreads, 0);
-            if (e != cudaSuccess) { cudaGetLastError(); return 1; }
-            return occ > 0 ? occ : 1;
-        }
+        if (index_mode) return occupancy_of((const void*)fbr::dispatch_thread_kernel<B, true>, fbr::kThreads, 0);
     }
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, (const void*)fbr::dispatch_thread_kernel<B, false>, fbr::kThreads, 0);
-    if (e != cudaSuccess) { cudaGetLastError(); return 1; }
-    return occ > 0 ? occ : 1;
+    return occupancy_of((const void*)fbr::dispatch_thread_kernel<B, false>, fbr::kThreads, 0);
 }
-}  // namespace fbr_body_export
 
-namespace fbr_body_export {
 // the bit-packed twin of a bool body: 8 items (explicit records or range() indices) per result byte
 template <class B>
 void launch_bits(const void* wpv, int grid, void* sv) {
@@ -161,13 +157,11 @@ void launch_bits(const void* wpv, int grid, void* sv) {
 }
 template <class B>
 int occupancy_bits(int index_mode) {
-    int occ = 0;
     const void* k = (const void*)fbr::dispatch_bits_items_kernel<B, false>;
     if constexpr (B::kIndexArg) {
         if (index_mode) k = (const void*)fbr::dispatch_bits_items_kernel<B, true>;
     }
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k, fbr::kThreads, 0) != cudaSuccess) { cudaGetLastError(); return 1; }
-    return occ > 0 ? occ : 1;
+    return occupancy_of(k, fbr::kThreads, 0);
 }
 }  // namespace fbr_body_export
 
@@ -212,9 +206,7 @@ int occupancy_record(int index_mode) {
             smem = L::smem(true);
         }
     }
-    int occ = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k, fbr::record::kThreads, smem) != cudaSuccess) { cudaGetLastError(); return 1; }
-    return occ > 0 ? occ : 1;
+    return occupancy_of(k, fbr::record::kThreads, smem);
 }
 template <class B>
 constexpr bool record_body_ok() {
