@@ -16,10 +16,11 @@ FBR_ABI_VERSION = 2
 FBR_OK, FBR_EINVAL, FBR_ECUDA, FBR_ENOMEM, FBR_ESTATE, FBR_ETIMEOUT, FBR_ETASK, FBR_ENODEV, FBR_ENOENT = \
     0, -1, -2, -3, -4, -5, -6, -7, -8
 # fbr_result_kind
-FBR_RES_BYTES, FBR_RES_BOOL, FBR_RES_I64, FBR_RES_U32, FBR_RES_F64X2, FBR_RES_NONE, FBR_RES_BITS8 = range(7)
+FBR_RES_BYTES, FBR_RES_BOOL, FBR_RES_I64, FBR_RES_U32, FBR_RES_F64X2, FBR_RES_NONE, FBR_RES_BITS8, FBR_RES_OFFSETS = range(8)
 # body flags
 FBR_BODY_INDEX_ARG, FBR_BODY_NEEDS_SHARED, FBR_BODY_SUMMABLE, FBR_BODY_INDEX_ONLY, FBR_BODY_RECORD, FBR_BODY_BROADCAST, \
     FBR_BODY_ITEMS = 0x1, 0x2, 0x4, 0x8, 0x10, 0x20, 0x40
+FBR_BODY_EMIT = 0x80
 FBR_BODY_MODULE_ABI = 4
 # pool flags
 FBR_POOL_TIMING, FBR_POOL_OVERLAP = 0x1, 0x2
@@ -29,16 +30,18 @@ FBR_ARGS_DEVICE, FBR_OUT_DEVICE, FBR_WANT_SUM, FBR_SHUFFLE, FBR_FULL_WINDOW, FBR
     FBR_RESULTS_ON_DEVICE, FBR_VIA_RING, FBR_NO_ZERO_COPY = 0x10, 0x20, 0x40, 0x80, 0x100, 0x200, 0x400, 0x800, 0x1000, 0x2000
 # fbr_task_error
 FBR_TASK_OK, FBR_TASK_OVERFLOW, FBR_TASK_BADARG, FBR_TASK_FAULT = range(4)
+FBR_TASK_EMIT = 4
 
 # every symbol include/fiber_b200.h declares (tests check the .so exports each of them)
 SYMBOLS = [
     "fbr_abi_version", "fbr_last_error", "fbr_device_count",
     "fbr_body_count", "fbr_body_info", "fbr_body_lookup", "fbr_register_body", "fbr_body_shared_info",
-    "fbr_body_items_info",
+    "fbr_body_items_info", "fbr_body_emit_info",
     "fbr_pool_create", "fbr_pool_close", "fbr_pool_terminate", "fbr_pool_join", "fbr_pool_destroy",
     "fbr_pool_n_workers", "fbr_pool_worker_device",
     "fbr_map_submit", "fbr_map_submit_items", "fbr_shared_put", "fbr_shared_drop", "fbr_plan_query",
     "fbr_result_wait", "fbr_result_poll", "fbr_result_data", "fbr_result_fetch", "fbr_result_release",
+    "fbr_result_values", "fbr_result_fetch_values",
     "fbr_host_alloc", "fbr_host_free", "fbr_device_alloc", "fbr_device_free",
     "fbr_memcpy_h2d", "fbr_memcpy_d2h", "fbr_payload_fill_device",
     "fbr_pool_stats", "fbr_pool_stats_reset",
@@ -146,6 +149,7 @@ def load():
         "fbr_register_body": (i32, [ctypes.c_char_p, ctypes.c_char_p, ctypes.c_char_p, P(i32)]),
         "fbr_body_shared_info": (i32, [i32, P(u32), P(u32)]),
         "fbr_body_items_info": (i32, [i32, P(u32)]),
+        "fbr_body_emit_info": (i32, [i32, P(u32)]),
         "fbr_pool_create": (i32, [i32, P(i32), u64, u32, P(vp)]),
         "fbr_pool_close": (i32, [vp]),
         "fbr_pool_terminate": (i32, [vp]),
@@ -161,6 +165,8 @@ def load():
         "fbr_result_wait": (i32, [vp, u64, i32, P(Result)]),
         "fbr_result_poll": (i32, [vp, u64, P(u64)]),
         "fbr_result_data": (i32, [vp, u64, P(vp)]),
+        "fbr_result_values": (i32, [vp, u64, P(vp), P(u64)]),
+        "fbr_result_fetch_values": (i32, [vp, u64, u64, u64, vp]),
         "fbr_result_fetch": (i32, [vp, u64, u64, u64, vp]),
         "fbr_result_release": (i32, [vp, u64]),
         "fbr_host_alloc": (i32, [vp, u64, P(vp)]),

@@ -171,6 +171,7 @@ struct BodyEntry {
     void* module = nullptr;    // dlopen handle of a registered body (never closed: kernels may be in flight)
     uint32_t shared_elem_bytes = 0, shared_stage_bytes = 0;   // FBR_BODY_BROADCAST record bodies
     uint32_t item_bytes = 0;                                  // FBR_BODY_ITEMS record bodies
+    uint32_t out_bytes = 0;                                   // FBR_BODY_EMIT record bodies
 };
 
 static std::mutex g_body_mu;
@@ -255,6 +256,7 @@ struct Worker {
     uint8_t* d_ring = nullptr;         // result ring arena (ring_bytes)
     uint8_t* d_args[2] = {nullptr, nullptr};
     uint8_t* d_items[2] = {nullptr, nullptr};   // items bodies, host-resident items: a wave's offsets slice, then its item span
+    uint8_t* d_vals[2] = {nullptr, nullptr};    // emit bodies, host-resident values: a wave's values before their D2H copy
     uint8_t* d_out[2] = {nullptr, nullptr};
     uint32_t* d_tickets = nullptr;
     SeqCtrl* d_ctrl = nullptr;
@@ -325,6 +327,30 @@ struct SeqPart {
     PartCtx cx;
 };
 
+// One worker block of an emit map: the part-local exclusive offsets its scan produced (count + 1 of them, the last is the
+// block's total) and where its values go.  Blocks are contiguous, so block k's values start at the totals of the blocks
+// before it (base).
+// Where the emit pass writes a block's values:
+//   - FBR_RESULTS_ON_DEVICE: d_values, an engine-owned device buffer of the block's exact size;
+//   - host-resident values of a block that may re-dispatch units (resilient, FBR_FULL_WINDOW): d_values too, copied to the
+//     pinned segment (host) in one piece once no unit is lost any more;
+//   - other host-resident values: wave by wave into the worker's d_vals staging half, each wave's span copied to `host`
+//     behind its kernel; h_offs (a pinned copy of the block's offsets) gives the host every wave's span before it launches.
+struct EmitPart {
+    int worker = 0;
+    uint64_t first = 0, count = 0, base = 0, total = 0;
+    uint64_t* d_offs = nullptr;
+    void* d_values = nullptr;
+    uint8_t* host = nullptr;              // the block's first value in the pinned values segment (host-resident maps)
+    uint64_t* h_offs = nullptr;           // pinned: the block's count + 1 offsets (waves staged through d_vals)
+};
+struct EmitPlan {
+    std::vector<EmitPart> parts;
+    uint32_t out_bytes = 0;
+    void* values = nullptr;               // pinned values segment (host-resident results)
+    uint64_t n_values = 0;
+};
+
 struct SeqState {
     uint64_t seq = 0, n_tasks = 0;
     int func_id = 0;
@@ -348,6 +374,7 @@ struct SeqState {
     bool release_pending = false;          // fbr_result_release arrived while they were waiting: the last one out frees the seq
     int dead_worker = -1;                  // a worker died under this map and the map could not be re-dispatched
     int dead_error = 0;
+    EmitPlan emit;                         // emit maps: per-block offsets and values (empty parts for every other map)
 };
 
 struct SharedBlock {
@@ -602,6 +629,7 @@ static void worker_destroy(Worker& w) {
     for (int i = 0; i < 2; ++i) {
         cudaFree(w.d_args[i]);
         cudaFree(w.d_items[i]);
+        cudaFree(w.d_vals[i]);
         cudaFree(w.d_out[i]);
     }
     cudaFree(w.d_tickets);
@@ -812,6 +840,22 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
     wp.item_first = item_first;
     wp.item_base = item_base;
     wp.item_count = item_count;
+    const EmitPart* emit = nullptr;
+    uint64_t v_lo = 0, v_hi = 0;            // staged emit waves: the wave's span of the block's values
+    for (const EmitPart& e : st.emit.parts)
+        if (e.worker == part.worker) emit = &e;
+    if (emit) {
+        wp.emit_offs = emit->d_offs;
+        wp.emit_first = emit->first;
+        wp.emit_base = emit->base;
+        if (emit->h_offs) {
+            v_lo = emit->h_offs[wave_first - emit->first];
+            v_hi = emit->h_offs[wave_first - emit->first + wt];
+            wp.emit_values = w.d_vals[half] - v_lo * st.emit.out_bytes;     // the wave's first value lands at d_vals[half]
+        } else {
+            wp.emit_values = (uint8_t*)emit->d_values;
+        }
+    }
     int occ_d = worker_occ(w, st.func_id, body, d.arg_stride == 0);
     if (body.max_ctas_per_sm) occ_d = std::min(occ_d, body.max_ctas_per_sm);
     if (ov && occ_d > 1) occ_d -= 1;     // leave SM slots for the concurrently running gather CTAs
@@ -930,6 +974,11 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
                 CK(cudaMemcpyAsync((uint8_t*)st.out + wave_first * cx.R, w.d_out[half], wt * cx.R, cudaMemcpyDeviceToHost, so));
                 STAT_ADD(p, d2h_bytes, wt * cx.R);
             }
+            if (emit && emit->h_offs && v_hi > v_lo) {   // the wave's values, exactly its span, into the pinned segment
+                const uint64_t ob = st.emit.out_bytes;
+                CK(cudaMemcpyAsync(emit->host + v_lo * ob, w.d_vals[half], (v_hi - v_lo) * ob, cudaMemcpyDeviceToHost, so));
+                STAT_ADD(p, d2h_bytes, (v_hi - v_lo) * ob);
+            }
             CK(cudaEventRecord(w.ev_out[half], so));
             CK(cudaEventRecord(wd, so));
         } else {
@@ -964,6 +1013,12 @@ static int finish_round(fbr_pool* p, SeqState& st, SeqPart& part, bool copy_wind
         CK(cudaMemcpyAsync((uint8_t*)st.out + part.first * cx.R, cx.window_base, part.count * cx.R, cudaMemcpyDeviceToHost, sf));
         STAT_ADD(p, d2h_bytes, part.count * cx.R);
     }
+    if (copy_window)
+        for (const EmitPart& e : st.emit.parts)
+            if (e.worker == part.worker && e.host && e.d_values && e.total) {
+                CK(cudaMemcpyAsync(e.host, e.d_values, e.total * st.emit.out_bytes, cudaMemcpyDeviceToHost, sf));
+                STAT_ADD(p, d2h_bytes, e.total * st.emit.out_bytes);
+            }
     CK(cudaMemcpyAsync(&w.h_ctrl[slot], &w.d_ctrl[slot], sizeof(SeqCtrl), cudaMemcpyDeviceToHost, sf));
     if (cx.resilient && part.lost_cap)
         CK(cudaMemcpyAsync(part.h_lost, part.d_lost, sizeof(LostUnit) * part.lost_cap, cudaMemcpyDeviceToHost, sf));
@@ -1214,6 +1269,23 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
                             (unsigned long long)t0, (unsigned long long)t1, (unsigned long long)ib, (unsigned long long)p->ring_bytes);
         }
     }
+    // emit maps whose values stream wave by wave: each wave's values must fit one staging half, so every claim unit's must
+    const EmitPart* emit = nullptr;
+    for (const EmitPart& e : st.emit.parts)
+        if (e.worker == part.worker && e.h_offs) emit = &e;
+    const uint64_t ob = st.emit.out_bytes;
+    if (emit) {
+        for (int i = 0; i < 2; ++i)
+            if (!w.d_vals[i]) CK(cudaMalloc((void**)&w.d_vals[i], p->ring_bytes));
+        const uint64_t* o = emit->h_offs;
+        for (uint64_t t0 = 0; t0 < part.count; t0 += unit) {
+            const uint64_t t1 = std::min<uint64_t>(t0 + unit, part.count);
+            if ((o[t1] - o[t0]) * ob > p->ring_bytes)
+                return fail(FBR_EINVAL, "the claim unit of tasks [%llu, %llu) emits %llu value bytes, more than a staging half of "
+                            "ring_bytes %llu holds: raise ring_bytes or use results=\"device\"", (unsigned long long)(part.first + t0),
+                            (unsigned long long)(part.first + t1), (unsigned long long)((o[t1] - o[t0]) * ob), (unsigned long long)p->ring_bytes);
+        }
+    }
     uint64_t done_tasks = 0;
     uint32_t wave_idx = 0;
     while (done_tasks < part.count) {
@@ -1240,6 +1312,17 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
             while (lo_u < hi_u) {
                 const uint64_t mid = (lo_u + hi_u + 1) / 2;
                 if (fits(std::min<uint64_t>(mid * unit, wt))) lo_u = mid; else hi_u = mid - 1;
+            }
+            wt = std::min<uint64_t>(std::max<uint64_t>(lo_u, 1) * unit, wt);     // every unit fits (checked above)
+        }
+        if (emit) {
+            // the most whole units (or the rest of the block) whose values fit one staging half, by binary search over the
+            // block's offsets
+            const uint64_t* o = emit->h_offs + done_tasks;
+            uint64_t lo_u = 0, hi_u = (wt + unit - 1) / unit;
+            while (lo_u < hi_u) {
+                const uint64_t mid = (lo_u + hi_u + 1) / 2;
+                if ((o[std::min<uint64_t>(mid * unit, wt)] - o[0]) * ob <= p->ring_bytes) lo_u = mid; else hi_u = mid - 1;
             }
             wt = std::min<uint64_t>(std::max<uint64_t>(lo_u, 1) * unit, wt);     // every unit fits (checked above)
         }
@@ -1389,7 +1472,8 @@ static void on_worker_death(fbr_pool* p, int wi, cudaError_t err) {
         if (!touched) continue;
         // device-resident arguments / outputs of a map live on worker 0
         const bool on_w0 = (st.flags & (FBR_ARGS_DEVICE | FBR_OUT_DEVICE)) != 0;
-        if (!(st.flags & FBR_RESILIENT) || live.empty() || (on_w0 && p->workers[0].dead)) {
+        // an emit map's blocks carry the offsets of the workers that counted them: it is failed, not re-cut
+        if (!(st.flags & FBR_RESILIENT) || live.empty() || (on_w0 && p->workers[0].dead) || !st.emit.parts.empty()) {
             st.dead_worker = wi;
             st.dead_error = (int)err;
             continue;
@@ -1450,6 +1534,17 @@ static void free_seq(fbr_pool* p, SeqState& st) {
         if (part.h_lost) cudaFreeHost(part.h_lost);
         if (part.ctrl_slot >= 0) w.ctrl_free.push_back(part.ctrl_slot);
     }
+    for (const EmitPart& e : st.emit.parts) {
+        Worker& w = p->workers[e.worker];
+        if (w.dead) continue;
+        cudaSetDevice(w.device);
+        if (e.d_offs) cudaFreeAsync(e.d_offs, w.s_in);
+        if (e.d_values) cudaFreeAsync(e.d_values, w.s_in);
+        if (e.h_offs) pinned_release(p, e.h_offs);
+    }
+    st.emit.parts.clear();
+    if (st.emit.values) pinned_release(p, st.emit.values);
+    st.emit.values = nullptr;
     if (st.own_out && st.out && !numa_pinned_release(p, st.out)) pinned_release(p, st.out);
 }
 
@@ -1531,6 +1626,13 @@ int fbr_body_items_info(int func_id, uint32_t* item_bytes) {
     return FBR_OK;
 }
 
+int fbr_body_emit_info(int func_id, uint32_t* out_bytes) {
+    const BodyEntry* bp = body_of(func_id);
+    if (!out_bytes || !bp) return fail(FBR_EINVAL, "bad func_id %d", func_id);
+    *out_bytes = bp->out_bytes;
+    return FBR_OK;
+}
+
 int fbr_body_lookup(const char* name, int* func_id) {
     if (!name || !func_id) return fail(FBR_EINVAL, "NULL argument");
     for (int f = 0, n = body_count(); f < n; ++f)
@@ -1556,6 +1658,19 @@ static std::string descriptor_error(const fbr_body_module_t* m, const char* modu
     else if (items && !is_record) why = "only record bodies take items (FBR_BODY_ITEMS)";
     else if (items && !record::item_elem_ok(m->item_bytes)) why = "the item size must be 1, 2 or a multiple of 4 up to 4096 bytes";
     else if (items && (m->flags & FBR_BODY_INDEX_ARG)) why = "an items body cannot take range() indices (FBR_BODY_INDEX_ARG)";
+    const bool emit = (m->flags & FBR_BODY_EMIT) != 0;
+    if (why) {
+    } else if (!emit && m->out_bytes) {
+        why = "describes an out element but lacks FBR_BODY_EMIT";
+    } else if (emit && !is_record) {
+        why = "only record bodies emit variable-length results (FBR_BODY_EMIT)";
+    } else if (emit && (m->result_bytes != 8 || m->result_kind != FBR_RES_OFFSETS)) {
+        why = "an emit body has no fixed result record (Res = fbr::NoRes): result_bytes 8 and result kind FBR_RES_OFFSETS";
+    } else if (emit && !record::item_elem_ok(m->out_bytes)) {
+        why = "the out size must be 1, 2 or a multiple of 4 up to 4096 bytes";
+    } else if (emit && (m->flags & FBR_BODY_SUMMABLE)) {
+        why = "an emit body's results cannot be folded on the device (FBR_BODY_SUMMABLE)";
+    }
     if (why) return strf("module %s: body '%s' %s", module_path, name, why);
     const uint32_t group = m->group_threads;
     if (group > 1 && (group > 32 || (group & (group - 1)) != 0))
@@ -1577,7 +1692,8 @@ static std::string descriptor_error(const fbr_body_module_t* m, const char* modu
     else if ((uint64_t)record::align_tasks(m->arg_bytes, m->result_bytes) * big > record::kStageBytes)
         why = "one 16 B-aligned group of tasks must fit a 32768-byte stage: kAlign * max(arg_bytes, result_bytes) <= 32768, "
               "kAlign = 1 when both sizes are multiples of 16, 2 when both are multiples of 8, else 4";
-    else if (m->result_kind != FBR_RES_BYTES) why = "the result kind must be FBR_RES_BYTES (no bit-packed twin)";
+    else if (m->result_kind != (emit ? (uint32_t)FBR_RES_OFFSETS : (uint32_t)FBR_RES_BYTES))
+        why = "the result kind must be FBR_RES_BYTES (no bit-packed twin)";
     else if (m->flags & FBR_BODY_SUMMABLE) why = "results cannot be folded on the device (FBR_BODY_SUMMABLE)";
     else if ((m->flags & FBR_BODY_NEEDS_SHARED) && !bcast)
         why = "a body without a Shared element type receives no broadcast block (FBR_BODY_NEEDS_SHARED without FBR_BODY_BROADCAST)";
@@ -1621,6 +1737,7 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
     b.flags = m->flags; b.unit_tasks = m->unit_tasks;
     b.shared_elem_bytes = m->shared_elem_bytes; b.shared_stage_bytes = m->shared_stage_bytes;
     b.item_bytes = m->item_bytes;
+    b.out_bytes = m->out_bytes;
     b.launch = m->launch; b.occupancy = m->occupancy;
     b.module = h;
     g_bodies.push_back(b);
@@ -1847,7 +1964,179 @@ int fbr_map_submit_items(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items
     return map_submit(p, d, it, seq_out);
 }
 
+static int map_submit_plan(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out,
+                           EmitPlan* plan);
+static int emit_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out);
+
 static int map_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out) {
+    const BodyEntry* b = body_of(d->func_id);
+    if (b && (b->flags & FBR_BODY_EMIT)) return emit_submit(p, d, items, seq_out);
+    return map_submit_plan(p, d, items, seq_out, nullptr);
+}
+
+// An emit map: the count pass is an ordinary map of the body whose records (the tasks' counts) stay on the device; once it
+// is done, scan_counts_kernel turns each block's counts into its offsets and total, the host sizes the values segment from
+// the totals, and the emit pass runs as a second ordinary map over the same blocks (`plan`).
+static int emit_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out) {
+    const BodyEntry& body = *body_of(d->func_id);
+    if (d->out || (d->flags & FBR_OUT_DEVICE))
+        return fail(FBR_EINVAL, "body %s emits variable-length results: its maps own their output (no out, no FBR_OUT_DEVICE)", body.name.c_str());
+    fbr_map_desc_t cd = *d;
+    cd.flags |= FBR_RESULTS_ON_DEVICE;
+    uint64_t cseq = 0;
+    int rc = map_submit_plan(p, &cd, items, &cseq, nullptr);
+    if (rc != FBR_OK) return rc;
+    fbr_result_t cres;
+    rc = fbr_result_wait(p, cseq, -1, &cres);
+    if (rc != FBR_OK && rc != FBR_ETASK) {
+        const std::string msg = g_err;
+        fbr_result_release(p, cseq);
+        g_err = msg;
+        return rc;
+    }
+    EmitPlan plan;
+    plan.out_bytes = body.out_bytes;
+    const bool on_device = (d->flags & FBR_RESULTS_ON_DEVICE) != 0;
+    const bool whole_block = (d->flags & (FBR_RESILIENT | FBR_FULL_WINDOW)) != 0;   // units may be re-dispatched: no waves
+    uint64_t* totals = nullptr;
+    // drop the count pass, the totals (and, on failure, what the plan holds so far) under the pool lock
+    auto drop = [&](bool with_plan) {
+        std::lock_guard<std::mutex> g(p->mu);
+        if (totals) pinned_release(p, totals);
+        auto it = p->seqs.find(cseq);
+        if (it != p->seqs.end()) {
+            free_seq(p, *it->second);
+            p->seqs.erase(it);
+        }
+        if (with_plan) {
+            SeqState tmp;
+            tmp.emit = std::move(plan);
+            free_seq(p, tmp);
+        }
+    };
+    std::vector<std::pair<int, cudaEvent_t>> scanned;   // (device, event after its block's scan)
+    {
+        std::lock_guard<std::mutex> g(p->mu);
+        auto it = p->seqs.find(cseq);
+        if (it == p->seqs.end()) return fail(FBR_ENOENT, "count pass of an emit map was released");
+        SeqState& cs = *it->second;
+        if (rc == FBR_ETASK) {
+            // the count pass failed: the map is born finished, with the count pass's error (fbr_result_wait reports it)
+            std::unique_ptr<SeqState> st(new SeqState());
+            st->seq = ++p->next_seq;
+            st->n_tasks = d->n_tasks;
+            st->func_id = d->func_id;
+            st->flags = d->flags;
+            st->result_bytes = body.result_bytes;
+            st->result_kind = body.result_kind;
+            st->desc = *d;
+            st->finished = true;
+            st->err_code = cs.err_code;
+            st->err_task = cs.err_task;
+            free_seq(p, cs);
+            p->seqs.erase(it);
+            p->stats.tasks_submitted += d->n_tasks;
+            *seq_out = st->seq;
+            p->seqs[st->seq] = std::move(st);
+            return FBR_OK;
+        }
+        std::vector<SeqPart*> parts;
+        for (auto& part : cs.parts) parts.push_back(&part);
+        std::sort(parts.begin(), parts.end(), [](const SeqPart* a, const SeqPart* b) { return a->first < b->first; });
+        // one total per block, written by its scan into pinned memory (mapped into every device's address space)
+        rc = pinned_acquire(p, sizeof(uint64_t) * std::max<size_t>(1, parts.size()), (void**)&totals);
+        auto scan_all = [&]() -> int {
+            for (size_t k = 0; k < parts.size() && rc == FBR_OK; ++k) {
+                const SeqPart& part = *parts[k];
+                Worker& w = p->workers[part.worker];
+                const uint64_t tiles = part.count / scan::kTile + 1;
+                if (tiles >= (1ull << 31)) return fail(FBR_EINVAL, "emit map block of %llu tasks is too large to scan", (unsigned long long)part.count);
+                EmitPart e;
+                e.worker = part.worker;
+                e.first = part.first;
+                e.count = part.count;
+                CK(cudaSetDevice(w.device));
+                CK(cudaMallocAsync((void**)&e.d_offs, (part.count + 1) * sizeof(uint64_t), w.s_comp));
+                plan.parts.push_back(e);
+                void* scratch = nullptr;
+                CK(cudaMallocAsync(&scratch, (tiles + 1) * sizeof(uint64_t), w.s_comp));
+                cudaMemsetAsync(scratch, 0, (tiles + 1) * sizeof(uint64_t), w.s_comp);
+                scan_counts_kernel<<<(unsigned)tiles, scan::kThreads, 0, w.s_comp>>>(
+                    (const uint64_t*)part.cx.window_base, part.count, plan.parts.back().d_offs, (unsigned long long*)scratch,
+                    (uint32_t*)((uint64_t*)scratch + tiles), totals + k);
+                const cudaError_t launched = cudaGetLastError();
+                cudaFreeAsync(scratch, w.s_comp);
+                if (launched != cudaSuccess) return fail(FBR_ECUDA, "scan_counts_kernel: %s", cudaGetErrorString(launched));
+                if (!on_device && !whole_block) {
+                    // the host cuts the emit pass's waves from the block's offsets
+                    EmitPart& ep = plan.parts.back();
+                    int r = pinned_acquire(p, (part.count + 1) * sizeof(uint64_t), (void**)&ep.h_offs);
+                    if (r != FBR_OK) return r;
+                    CK(cudaMemcpyAsync(ep.h_offs, ep.d_offs, (part.count + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, w.s_comp));
+                }
+                cudaEvent_t ev;
+                CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+                scanned.push_back({w.device, ev});
+                CK(cudaEventRecord(ev, w.s_comp));
+            }
+            return rc;
+        };
+        rc = scan_all();
+    }
+    // one wait per block, outside the pool lock: then every total is in and the blocks' bases are known
+    for (auto& s : scanned) {
+        cudaSetDevice(s.first);
+        if (rc == FBR_OK && cudaEventSynchronize(s.second) != cudaSuccess) rc = fail(FBR_ECUDA, "waiting for scan_counts_kernel failed");
+        cudaEventDestroy(s.second);
+    }
+    if (rc == FBR_OK) {
+        std::lock_guard<std::mutex> g(p->mu);
+        for (size_t k = 0; k < plan.parts.size(); ++k) {
+            EmitPart& e = plan.parts[k];
+            e.total = totals[k];
+            e.base = plan.n_values;
+            plan.n_values += e.total;
+        }
+        auto place = [&]() -> int {
+            if (plan.n_values >= (1ull << 62) / std::max<uint32_t>(1, plan.out_bytes))
+                return fail(FBR_EINVAL, "body %s: the map's count pass gave %llu values, too many to place", body.name.c_str(),
+                            (unsigned long long)plan.n_values);
+            if (!on_device) {
+                int r = pinned_acquire(p, plan.n_values * plan.out_bytes, &plan.values);
+                if (r != FBR_OK) return r;
+                for (EmitPart& e : plan.parts) e.host = (uint8_t*)plan.values + e.base * plan.out_bytes;
+            }
+            if (on_device || whole_block)
+                for (EmitPart& e : plan.parts) {
+                    Worker& w = p->workers[e.worker];
+                    CK(cudaSetDevice(w.device));
+                    CK(cudaMallocAsync(&e.d_values, std::max<uint64_t>(16, e.total * plan.out_bytes), w.s_comp));
+                }
+            return FBR_OK;
+        };
+        rc = place();
+    }
+    if (rc != FBR_OK) {
+        const std::string msg = g_err;
+        drop(true);
+        g_err = msg;
+        return rc;
+    }
+    drop(false);
+    rc = map_submit_plan(p, d, items, seq_out, &plan);
+    if (rc != FBR_OK) {
+        const std::string msg = g_err;
+        std::lock_guard<std::mutex> g(p->mu);
+        SeqState tmp;
+        tmp.emit = std::move(plan);
+        free_seq(p, tmp);
+        g_err = msg;
+    }
+    return rc;
+}
+
+static int map_submit_plan(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out,
+                           EmitPlan* plan) {
     std::lock_guard<std::mutex> g(p->mu);
     if (p->state != ST_RUN) return fail(FBR_ESTATE, "Pool is not running");
     if (!body_of(d->func_id)) return fail(FBR_EINVAL, "bad func_id %d", d->func_id);
@@ -1945,6 +2234,21 @@ static int map_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_de
         // contiguous task blocks per live worker, cut on claim-unit boundaries (block partition ==
         // PUSH round-robin with chunk = block, SURVEY.md 8(e))
         cut_blocks(p, body, *d, 0, d->n_tasks, live, d->attempt, st->parts);
+        if (plan) {
+            // the emit pass runs over the blocks the count pass counted
+            bool same = plan->parts.size() == st->parts.size();
+            for (size_t k = 0; same && k < st->parts.size(); ++k) {
+                const EmitPart& e = plan->parts[k];
+                const SeqPart& part = st->parts[k];
+                same = e.worker == part.worker && e.first == part.first && e.count == part.count;
+            }
+            if (!same) {
+                free_seq(p, *st);
+                return fail(FBR_ECUDA, "body %s: the pool's workers changed between the count and the emit pass", body.name.c_str());
+            }
+            st->emit = std::move(*plan);
+            *plan = EmitPlan();
+        }
         if (need_segment && live.size() > 1) {
             // several GPUs fill one segment: bind each worker's block to its GPU's NUMA node
             std::vector<NumaBlock> blocks;
@@ -2160,6 +2464,10 @@ int fbr_result_poll(fbr_pool_t* p, uint64_t seq, uint64_t* n_done) {
     if (it == p->seqs.end()) return fail(FBR_ENOENT, "unknown seq %llu", (unsigned long long)seq);
     SeqState& st = *it->second;
     if (st.dead_worker >= 0) return dead_map_error(p, st);
+    if (st.finished && st.parts.empty()) {   // an emit map whose count pass failed: nothing more will come, wait reports why
+        *n_done = st.n_tasks;
+        return FBR_OK;
+    }
     // ordered progress: tasks [0, n_done) are final.  Blocks are contiguous per worker, so count
     // complete waves worker by worker and stop at the first incomplete one.
     uint64_t done = 0;
@@ -2209,6 +2517,47 @@ int fbr_result_poll(fbr_pool_t* p, uint64_t seq, uint64_t* n_done) {
         if (part_done < part.count) break;
     }
     *n_done = done;
+    return FBR_OK;
+}
+
+int fbr_result_values(fbr_pool_t* p, uint64_t seq, void** values, uint64_t* n_values) {
+    if (!p || !values || !n_values) return fail(FBR_EINVAL, "NULL argument");
+    std::lock_guard<std::mutex> g(p->mu);
+    auto it = p->seqs.find(seq);
+    if (it == p->seqs.end()) return fail(FBR_ENOENT, "unknown seq %llu", (unsigned long long)seq);
+    const SeqState& st = *it->second;
+    if (!(body_of(st.func_id)->flags & FBR_BODY_EMIT)) return fail(FBR_EINVAL, "seq %llu is not a map of an emit body", (unsigned long long)seq);
+    *values = st.emit.values;
+    *n_values = st.emit.n_values;
+    return FBR_OK;
+}
+
+int fbr_result_fetch_values(fbr_pool_t* p, uint64_t seq, uint64_t first, uint64_t count, void* host_dst) {
+    if (!p || (!host_dst && count)) return fail(FBR_EINVAL, "NULL argument");
+    std::lock_guard<std::mutex> g(p->mu);
+    auto it = p->seqs.find(seq);
+    if (it == p->seqs.end()) return fail(FBR_ENOENT, "unknown seq %llu", (unsigned long long)seq);
+    SeqState& st = *it->second;
+    if (!(body_of(st.func_id)->flags & FBR_BODY_EMIT) || !(st.flags & FBR_RESULTS_ON_DEVICE))
+        return fail(FBR_EINVAL, "seq %llu is not an emit map that keeps its results on the device", (unsigned long long)seq);
+    if (first + count > st.emit.n_values || first + count < first) return fail(FBR_EINVAL, "range out of bounds");
+    const uint64_t ob = st.emit.out_bytes;
+    for (auto& part : st.parts) {
+        CK(cudaSetDevice(p->workers[part.worker].device));
+        CK(cudaEventSynchronize(part.done));
+    }
+    for (const EmitPart& e : st.emit.parts) {
+        const uint64_t lo = std::max(first, e.base), hi = std::min(first + count, e.base + e.total);
+        if (lo >= hi) continue;
+        Worker& w = p->workers[e.worker];
+        CK(cudaSetDevice(w.device));
+        CK(cudaMemcpyAsync((uint8_t*)host_dst + (lo - first) * ob, (const uint8_t*)e.d_values + (lo - e.base) * ob, (hi - lo) * ob, cudaMemcpyDeviceToHost, w.s_out));
+        p->stats.d2h_bytes += (hi - lo) * ob;
+    }
+    for (const EmitPart& e : st.emit.parts) {
+        CK(cudaSetDevice(p->workers[e.worker].device));
+        CK(cudaStreamSynchronize(p->workers[e.worker].s_out));
+    }
     return FBR_OK;
 }
 

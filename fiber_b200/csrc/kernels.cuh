@@ -88,6 +88,13 @@ struct WaveParams {
     uint64_t item_first;        // map index of item_offs[0]
     uint64_t item_base;         // item index of items[0]
     uint64_t item_count;        // offsets end here (the map's n_items)
+    // emit record bodies (FBR_BODY_EMIT): nullptr runs the count pass (each task's record is its value count).  Otherwise
+    // the emit pass: task j writes its values at emit_values + o[j] * out_bytes with o = emit_offs - emit_first (the part's
+    // exclusive offsets, o[j + 1] its end), and its record is its global end offset emit_base + o[j + 1]
+    uint8_t* emit_values;
+    const uint64_t* emit_offs;
+    uint64_t emit_first;
+    uint64_t emit_base;
 };
 
 // Task record of ticket t: from the device task ring, or computed (contiguous wave).
@@ -962,6 +969,35 @@ struct Items {
 // The Arg of an items record body without a fixed head record: run() then takes no argument record.
 struct NoArg {};
 
+// The Res of an emit record body (`using Out = ...`): its task returns a variable-length array instead of a record.
+struct NoRes {};
+
+// The result of one task of an emit body: run() appends values of type T.  The body runs twice per task: in the count pass
+// data is nullptr and only n counts; in the emit pass data points at the task's place in the map's values and cap is the
+// count the first pass gave (values past it are never written).  A one-thread body calls push(v); a group body (G > 1) calls
+// the collective push_if(g, pred, v) on every lane of the group: lanes whose pred holds append their v in rank order, and
+// every lane keeps the same n.
+template <class T, uint32_t G = 1>
+struct Emit {
+    T* data;
+    uint64_t cap;
+    uint64_t n;
+    __device__ __forceinline__ void push(const T& v) {
+        static_assert(G == 1, "a group emitter has only the collective push_if(g, pred, v)");
+        if (data != nullptr && n < cap) data[n] = v;
+        ++n;
+    }
+    __device__ __forceinline__ void push_if(const Group<G>& g, bool pred, const T& v) {
+        static_assert(G > 1, "push_if is the collective of a group emitter; a one-thread body calls push(v)");
+        const uint32_t lanes = __ballot_sync(g.mask, pred) & g.mask;
+        if (pred) {
+            const uint64_t k = n + __popc(lanes & ((1u << (threadIdx.x & 31u)) - 1u));
+            if (data != nullptr && k < cap) data[k] = v;
+        }
+        n += __popc(lanes);
+    }
+};
+
 namespace record {
 constexpr int kConsumers = 256;
 constexpr int kThreads = 32 + kConsumers;
@@ -1029,10 +1065,50 @@ struct ItemsOf<B, std::void_t<typename B::Item>> {
     static_assert(!B::kIndexArg, "items bodies cannot take range() indices (kIndexArg)");
 };
 
+// A record body opts into variable-length results with `using Out = <element>;` and `using Res = NoRes;`: run() then takes
+// an Emit<Out, G>& where other record bodies take Res&.  Its kernels are instantiated for EmitPass<B, false> (the count
+// pass) and EmitPass<B, true> (the emit pass); in both, a task's fixed result record is one uint64 (its count, or its end
+// offset), so the two passes share one claim plan.
+template <class B, class = void>
+struct EmitOf {
+    static constexpr bool kOn = false;
+    static constexpr uint32_t kElem = 0;
+};
+template <class B>
+struct EmitOf<B, std::void_t<typename B::Out>> {
+    using T = typename B::Out;
+    static constexpr bool kOn = true;
+    static constexpr uint32_t kElem = (uint32_t)sizeof(T);
+    static_assert(std::is_trivially_copyable<T>::value, "emit bodies: Out is trivially copyable");
+    static_assert(item_elem_ok(kElem), "emit bodies: sizeof(Out) is 1, 2 or a multiple of 4 up to 4096");
+    static_assert(std::is_same<typename B::Res, NoRes>::value, "emit bodies have no fixed result record (Res = fbr::NoRes)");
+};
+// an emit body's optional `static uint64_t count(...)`: run()'s parameters without the emitter, es and attempt
+template <class B, class = void>
+struct HasCount : std::false_type {};
+template <class B>
+struct HasCount<B, std::void_t<decltype(&B::count)>> : std::true_type {};
+
+template <class B, bool kValues>
+struct EmitPass : B {
+    static constexpr bool kEmitValues = kValues;
+};
+template <class B, class = void>
+struct EmitModeOf {
+    static constexpr bool kValues = false;
+};
+template <class B>
+struct EmitModeOf<B, std::void_t<decltype(B::kEmitValues)>> {
+    static constexpr bool kValues = B::kEmitValues;
+};
+// the fixed result record of one task: Res, or the uint64 count / end offset of an emit body
+template <class B>
+using ResultRecord = typename std::conditional<EmitOf<B>::kOn, uint64_t, typename B::Res>::type;
+
 template <class B>
 struct Layout {
     static constexpr bool kNoArg = std::is_same<typename B::Arg, NoArg>::value;
-    static constexpr uint32_t A = kNoArg ? 0u : (uint32_t)sizeof(typename B::Arg), R = (uint32_t)sizeof(typename B::Res);
+    static constexpr uint32_t A = kNoArg ? 0u : (uint32_t)sizeof(typename B::Arg), R = (uint32_t)sizeof(ResultRecord<B>);
     static_assert(!kNoArg || ItemsOf<B>::kOn, "record bodies: only an items body may have no argument record (NoArg)");
     static_assert(GroupOf<B>::kG > 1 || (A % 4 == 0 && R % 4 == 0 && (A >= 4 || kNoArg) && R >= 4 && A <= kThreadRecordBytes && R <= kThreadRecordBytes),
                   "record bodies: sizeof(Arg) and sizeof(Res) are multiples of 4 between 4 and 4096");
@@ -1098,20 +1174,54 @@ __device__ __forceinline__ Group<G> group_of(uint32_t ct) {
 // index, a record from `in`, or none for NoArg), the task's items, the result, the broadcast block `sh` (bodies that have
 // one), the group (G > 1), then task_index, es and attempt.  An items task reads offsets o[i], o[i+1] and its items from
 // global memory; one whose offsets decrease or leave [item_base, item_count] reports TASK_BADARG and its body is not called.
+// An emit body's task that pushed another number of values than it counted lowers *emit_err (the unit's word, in shared
+// memory) to its (task_index << 8 | TASK_EMIT): the kernel reports it only if the unit was not lost, since a faulting
+// attempt's values are discarded.
 template <class B, bool kIndex, class... Sh>
 __device__ __forceinline__ void run_unit(const WaveParams& wp, const TaskRecord& rec, const uint8_t* in, uint8_t* out,
-                                         uint32_t ct, const ErrSink& es, const Sh&... sh) {
+                                         uint32_t ct, const ErrSink& es, unsigned long long* emit_err, const Sh&... sh) {
     using L = Layout<B>;
     using Arg = typename B::Arg;
-    using Res = typename B::Res;
+    using Res = ResultRecord<B>;
     constexpr uint32_t G = GroupOf<B>::kG, C = kConsumers;
     const uint64_t g0 = wp.index_base + rec.first;
     const uint64_t* const o = wp.item_offs + (rec.first - wp.item_first);   // items bodies: the unit's offsets
     for (uint32_t i = ct / G; i < rec.count; i += C / G) {
         auto res = [&]() -> Res& { return *reinterpret_cast<Res*>(out + (size_t)i * L::R); };
         auto call = [&](Res& r, const auto&... head) {  // head: the head argument, then the items
-            if constexpr (G > 1) B::run(head..., r, sh..., group_of<G>(ct), g0 + i, es, rec.attempt);
-            else B::run(head..., r, sh..., g0 + i, es, rec.attempt);
+            if constexpr (EmitOf<B>::kOn) {
+                // emit bodies: the count pass records the task's count, the emit pass its global end offset (the span the
+                // count pass gave, so the offsets stay consistent); a task that pushed another number reports TASK_EMIT
+                using O = typename EmitOf<B>::T;
+                Emit<O, G> y{nullptr, 0, 0};
+                uint64_t lo = 0;
+                if constexpr (EmitModeOf<B>::kValues) {
+                    const uint64_t* const e = wp.emit_offs + (rec.first + i - wp.emit_first);
+                    lo = e[0];
+                    y.cap = e[1] - lo;
+                    y.data = reinterpret_cast<O*>(wp.emit_values) + lo;
+                }
+                if constexpr (!EmitModeOf<B>::kValues && HasCount<B>::value) {
+                    static_assert(G == 1, "emit bodies: the count() hook is for one-thread bodies");
+                    y.n = B::count(head..., sh..., g0 + i);
+                } else if constexpr (G > 1) {
+                    B::run(head..., y, sh..., group_of<G>(ct), g0 + i, es, rec.attempt);
+                } else {
+                    B::run(head..., y, sh..., g0 + i, es, rec.attempt);
+                }
+                if (ct % G == 0) {
+                    if constexpr (EmitModeOf<B>::kValues) {
+                        if (y.n != y.cap) atomicMin(emit_err, (unsigned long long)(((g0 + i) << 8) | TASK_EMIT));
+                        r = wp.emit_base + lo + y.cap;
+                    } else {
+                        r = y.n;
+                    }
+                }
+            } else if constexpr (G > 1) {
+                B::run(head..., r, sh..., group_of<G>(ct), g0 + i, es, rec.attempt);
+            } else {
+                B::run(head..., r, sh..., g0 + i, es, rec.attempt);
+            }
         };
         if constexpr (kIndex) {
             call(res(), (Arg)(wp.index_start + (int64_t)(rec.first + i) * wp.index_step));
@@ -1144,6 +1254,11 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
     __shared__ uint32_t s_ticket[kIn];
     __shared__ uint32_t s_bulk[kIn];      // argument bytes of the unit the bulk load brings (the rest: consumers)
     __shared__ int s_fault[2];
+    unsigned long long* s_emit_err = nullptr;   // emit bodies: per-unit count-mismatch word, by unit parity
+    if constexpr (record::EmitOf<B>::kOn) {
+        __shared__ unsigned long long s_emit_words[2];
+        s_emit_err = s_emit_words;
+    }
     uint8_t* const in_stage = smem;
     uint8_t* const out_stage = smem + (kIndex ? 0 : (size_t)kIn * L::kInBytes);   // L::smem(kIndex) bytes in all
     // broadcast bodies: the block is staged once per CTA into the region after the stages when it fits kSharedStage
@@ -1164,6 +1279,7 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
         for (int s = 0; s < kIn; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], C); }
         if constexpr (Bc::kOn && Bc::kStage > 0) mbar_init(bcast_full, 1);
         s_fault[0] = 0; s_fault[1] = 0;
+        if constexpr (record::EmitOf<B>::kOn) { s_emit_err[0] = ~0ull; s_emit_err[1] = ~0ull; }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -1246,8 +1362,9 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
 
         int* const unit_fault = &s_fault[seq & 1];
         const ErrSink es{wp.err_word, unit_fault};
+        unsigned long long* const emit_err = s_emit_err != nullptr ? &s_emit_err[seq & 1] : nullptr;
         if constexpr (!Bc::kOn) {
-            record::run_unit<B, kIndex>(wp, rec, in, out, ct, es);
+            record::run_unit<B, kIndex>(wp, rec, in, out, ct, es, emit_err);
         } else {
             using T = typename Bc::T;
             const uint64_t n_elems = wp.shared_bytes / Bc::kElem;
@@ -1255,9 +1372,9 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
             // an items body keeps one loop over a generic pointer, because two such loops made ptxas spill
             if constexpr (record::ItemsOf<B>::kOn) {
                 const uint8_t* blk = staged ? bcast_stage : wp.shared;
-                record::run_unit<B, kIndex>(wp, rec, in, out, ct, es, Broadcast<T>{reinterpret_cast<const T*>(blk), n_elems});
+                record::run_unit<B, kIndex>(wp, rec, in, out, ct, es, emit_err, Broadcast<T>{reinterpret_cast<const T*>(blk), n_elems});
             } else {
-                auto run = [&](const Broadcast<T>& sh) { record::run_unit<B, kIndex>(wp, rec, in, out, ct, es, sh); };
+                auto run = [&](const Broadcast<T>& sh) { record::run_unit<B, kIndex>(wp, rec, in, out, ct, es, emit_err, sh); };
                 if (staged) run(Broadcast<T>{reinterpret_cast<const T*>(bcast_stage), n_elems});
                 else run(Broadcast<T>{reinterpret_cast<const T*>(wp.shared), n_elems});
             }
@@ -1284,6 +1401,11 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
                 lost = *unit_fault != 0;                  // every consumer's reports for this unit are in (barrier above)
                 s_fault[(seq + 1) & 1] = 0;               // re-arm the next unit's flag: its writers start after the next barrier
             }
+            if constexpr (record::EmitOf<B>::kOn) {
+                // a count mismatch counts only in a unit that was not lost; re-arm the word like the fault flag
+                if (!lost && s_emit_err[seq & 1] != ~0ull) atomicMin(wp.err_word, s_emit_err[seq & 1]);
+                s_emit_err[seq & 1] = ~0ull;
+            }
             // the thread kernel's protocol: a lost unit is re-dispatched (resilient) or a task error
             if (lost && !wp.resilient)
                 atomicMin(wp.err_word, (unsigned long long)(((wp.index_base + rec.first) << 8) | TASK_FAULT));
@@ -1291,6 +1413,85 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
         }
     }
     if (ct == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+}
+
+// ================================================================================================
+// scan_counts_kernel: the emit pass's offsets from the count pass's counts -- offs[i] = counts[0] + ... + counts[i-1] for
+// i = 0 .. n, and *total = offs[n] (mapped pinned memory: the host reads it once the kernel is done).  A single-pass
+// exclusive scan with decoupled look-back: CTAs claim tiles of kScanTile counts by ticket, so tile t only ever waits for
+// tiles claimed before it, which are running or done.  tile_state (one word per tile, zero at launch) holds a tile's
+// aggregate (flag A) as soon as it is known, and its inclusive prefix (flag P) once the look-back has found it; counts
+// and totals are below 2^62, so flag and value fit one 64-bit word that is written and read whole.
+// ================================================================================================
+namespace scan {
+constexpr int kThreads = 256, kItems = 8;
+constexpr uint32_t kTile = kThreads * kItems;
+constexpr unsigned long long kFlagA = 1ull << 62, kFlagP = 2ull << 62, kValue = (1ull << 62) - 1;
+}  // namespace scan
+
+__global__ void __launch_bounds__(scan::kThreads) scan_counts_kernel(const uint64_t* counts, uint64_t n, uint64_t* offs,
+                                                                    unsigned long long* tile_state, uint32_t* ticket,
+                                                                    uint64_t* total) {
+    using scan::kItems; using scan::kTile; using scan::kFlagA; using scan::kFlagP; using scan::kValue;
+    constexpr int kThreads = scan::kThreads;
+    __shared__ uint32_t s_tile;
+    __shared__ uint64_t s_warp[kThreads / 32];
+    __shared__ uint64_t s_prefix;
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    if (tid == 0) s_tile = atomicAdd(ticket, 1u);
+    __syncthreads();
+    const uint32_t tile = s_tile;
+    const uint64_t base = (uint64_t)tile * kTile + (uint64_t)tid * kItems;
+    uint64_t v[kItems], mine = 0;
+#pragma unroll
+    for (int k = 0; k < kItems; ++k) {
+        v[k] = base + k < n ? counts[base + k] : 0ull;
+        mine += v[k];
+    }
+    // CTA-wide exclusive scan of the per-thread sums: warp shuffles, then the warp totals
+    uint64_t incl = mine;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint64_t u = __shfl_up_sync(0xffffffffu, incl, d);
+        if (lane >= (uint32_t)d) incl += u;
+    }
+    if (lane == 31) s_warp[warp] = incl;
+    __syncthreads();
+    uint64_t before = incl - mine, tile_total = 0;
+    for (uint32_t w = 0; w < kThreads / 32; ++w) {
+        if (w < warp) before += s_warp[w];
+        tile_total += s_warp[w];
+    }
+    if (tid == 0) {
+        volatile unsigned long long* st = tile_state;
+        uint64_t prefix = 0;
+        if (tile == 0) {
+            st[0] = kFlagP | tile_total;
+        } else {
+            st[tile] = kFlagA | tile_total;
+            for (int64_t j = (int64_t)tile - 1; j >= 0;) {
+                const unsigned long long s = st[j];
+                if ((s & ~kValue) == 0) continue;              // tile j has not published its aggregate yet
+                prefix += s & kValue;
+                if (s & kFlagP) break;
+                --j;
+            }
+            st[tile] = kFlagP | (prefix + tile_total);
+        }
+        s_prefix = prefix;
+    }
+    __syncthreads();
+    uint64_t run = s_prefix + before;
+#pragma unroll
+    for (int k = 0; k < kItems; ++k) {
+        if (base + k < n) offs[base + k] = run;
+        run += v[k];
+    }
+    if (tile == (uint32_t)(n / kTile) && tid == kThreads - 1) {   // the tile holding index n writes the end and the total
+        offs[n] = run;
+        *total = run;
+        __threadfence_system();
+    }
 }
 
 // ================================================================================================

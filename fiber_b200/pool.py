@@ -21,6 +21,7 @@ objects, and nothing on this path executes tasks on the CPU.
 import collections.abc
 import ctypes
 import math
+import operator
 import threading
 import time
 
@@ -204,6 +205,82 @@ class ResultArray(collections.abc.Sequence):
         raise TypeError("ResultArray is read-only; use sorted(result) or result.tolist()")
 
 
+class _View:
+    """A NumPy-visible block of engine memory that keeps its owner (a map's _Segment) alive."""
+
+    def __init__(self, owner, ptr, nbytes):
+        self.owner = owner
+        self.__array_interface__ = {"shape": (nbytes,), "typestr": "|u1", "data": (ptr or 0, False), "version": 3}
+
+
+def _emit_value(spec, arr):
+    """One task's values as Python sees them: a list, or bytes / str (device_body(out_as=))."""
+    if spec.out_as == "bytes":
+        return arr.tobytes()
+    if spec.out_as == "str":
+        return arr.tobytes().decode("utf-8")
+    return arr.tolist()
+
+
+class EmitResultArray(ResultArray):
+    """Ordered results of a map of an emit body: task i's value is a variable-length array, read as a list (or ``bytes`` /
+    ``str``, see ``device_body(out_as=)``).  ``ends`` are the n end offsets and ``values`` every task's values back to back,
+    both views of the map's pinned segments; ``ragged`` is the whole map as one ``Ragged``.  With ``Pool(results="device")``
+    both stay in HBM and ranges are fetched on demand."""
+
+    def __init__(self, spec, ends, values, n=None, fetch=None, fetch_values=None):
+        super().__init__(spec, ends, None, n=n, fetch=fetch)
+        self._values = values
+        self._fetch_values = fetch_values    # (lo, hi) -> ndarray of values [lo, hi), device-resident maps
+
+    def _span(self, lo, hi):
+        """End offsets of tasks [lo - 1, hi) (the first is 0 for lo = 0) and the values of tasks [lo, hi)."""
+        if self._arr is not None:
+            ends = self._arr[max(0, lo - 1):hi]
+        else:
+            ends = self._fetch(max(0, lo - 1), hi)
+        ends = np.concatenate([np.zeros(1, np.uint64), ends]) if lo == 0 else ends
+        v0, v1 = int(ends[0]), int(ends[-1])
+        vals = self._values[v0:v1] if self._values is not None else self._fetch_values(v0, v1)
+        return ends - np.uint64(v0), vals
+
+    def __getitem__(self, i):
+        if isinstance(i, slice):
+            lo, hi, step = i.indices(self._n)
+            if step != 1:
+                return [self[j] for j in range(lo, hi, step)]
+            hi = max(lo, hi)
+            o, vals = self._span(lo, hi)
+            return [_emit_value(self._spec, vals[int(o[k]):int(o[k + 1])]) for k in range(hi - lo)]
+        j = operator.index(i)
+        j = j + self._n if j < 0 else j
+        if not 0 <= j < self._n:
+            raise IndexError("ResultArray index out of range")
+        o, vals = self._span(j, j + 1)
+        return _emit_value(self._spec, vals[int(o[0]):int(o[1])])
+
+    def __eq__(self, other):
+        if isinstance(other, EmitResultArray):
+            return len(self) == len(other) and self.tolist() == other.tolist()
+        if isinstance(other, (list, tuple)):
+            return len(other) == len(self) and self.tolist() == list(other)
+        return NotImplemented
+
+    @property
+    def ragged(self):
+        """The map's values as ``Ragged(values, offsets)``: values without a copy, offsets = 0 then the end offsets."""
+        if self._values is None:
+            self._values = self._fetch_values(0, int(self._a[-1]) if self._n else 0)
+        return registry.Ragged(self._values, np.concatenate([np.zeros(1, np.uint64), self._a]))
+
+    def tolist(self):
+        return self[:]
+
+    def sum(self):
+        raise TypeError("unsupported operand type(s) for +: 'int' and 'list' (%s returns a variable-length array per task)"
+                        % self._spec.name)
+
+
 class MapResult:
     """Handle of an asynchronous map (fiber/pool.py:731-743)."""
 
@@ -225,6 +302,9 @@ class MapResult:
             raise self._exc
         if self._n == 0:
             us = self._user_spec
+            if getattr(us, "out_dtype", None) is not None:
+                self._result = EmitResultArray(us, np.empty(0, np.uint64), np.empty(0, us.out_dtype))
+                return self._result
             self._result = ResultArray(us, np.empty((0,) + us.result_dtype()[1], us.result_dtype()[0]), 0)
             return self._result
         res = _abi.Result()
@@ -246,6 +326,9 @@ class MapResult:
         # exact, unbounded sum: the device folds the two halves of int64 results separately (nothing wraps)
         dsum = (int(res.sum_hi) * (1 << 32) + int(res.sum_lo)) if (self._flags & _abi.FBR_WANT_SUM) else None
         self.n_waves = res.n_waves
+        if getattr(self._spec, "out_dtype", None) is not None:
+            self._result = self._emit_result(res)
+            return self._result
         if self._flags & _abi.FBR_RESULTS_ON_DEVICE:
             seg = self._segment                              # owns the seq (device buffer) until GC
             rb, seq = res.result_bytes, self._seq
@@ -275,9 +358,48 @@ class MapResult:
         self._result = ResultArray(self._spec, arr, dsum)
         return self._result
 
+    def _emit_result(self, res):
+        """End offsets and values of a finished emit map: views of its pinned segments, or fetched from the device."""
+        eng, seq, seg, n, od = self._engine, self._seq, self._segment, int(res.n_tasks), self._spec.out_dtype
+        if self._flags & _abi.FBR_RESULTS_ON_DEVICE:
+            def fetch(lo, hi):
+                block = _PinnedBlock(eng, max(1, (hi - lo) * 8))
+                if hi > lo:
+                    _abi.check(eng.lib.fbr_result_fetch(eng.handle, seq, lo, hi - lo, ctypes.c_void_p(block.ptr)))
+                return np.asarray(block)[: (hi - lo) * 8].view(np.uint64)
+
+            def fetch_values(lo, hi, seg=seg):
+                block = _PinnedBlock(eng, max(1, (hi - lo) * od.itemsize))
+                if hi > lo:
+                    _abi.check(eng.lib.fbr_result_fetch_values(eng.handle, seq, lo, hi - lo, ctypes.c_void_p(block.ptr)))
+                return np.asarray(block)[: (hi - lo) * od.itemsize].view(od)
+            return EmitResultArray(self._spec, None, None, n=n, fetch=fetch, fetch_values=fetch_values)
+        ends = np.asarray(seg.bind(res.data, n * 8)).view(np.uint64)
+        return EmitResultArray(self._spec, ends, self._values_view())
+
+    def _values_view(self):
+        eng, ptr, nv = self._engine, ctypes.c_void_p(), ctypes.c_uint64(0)
+        _abi.check(eng.lib.fbr_result_values(eng.handle, self._seq, ctypes.byref(ptr), ctypes.byref(nv)))
+        od = self._spec.out_dtype
+        return np.asarray(_View(self._segment, ptr.value, nv.value * od.itemsize)).view(od)
+
+    def _emit_count(self, res, task):
+        """The number of values task `task` of a failed emit map was counted to push: the difference of its end offsets."""
+        lo = max(0, task - 1)
+        ends = np.zeros(task + 1 - lo, np.uint64)
+        if self._flags & _abi.FBR_RESULTS_ON_DEVICE:
+            eng = self._engine
+            _abi.check(eng.lib.fbr_result_fetch(eng.handle, self._seq, lo, len(ends), ends.ctypes.data))
+        else:
+            ctypes.memmove(ends.ctypes.data, res.data + lo * 8, ends.nbytes)
+        return int(ends[-1]) - (int(ends[0]) if task > 0 else 0)
+
     def _raise_task_error(self, res):
         code, task = res.err_code, res.err_task
         name = getattr(self, "_user_spec", self._spec).name     # the body the caller mapped (not its bit-packed twin)
+        if code == _abi.FBR_TASK_EMIT:
+            raise RuntimeError("%s: task %d emitted another number of values than the %d its count pass gave"
+                               % (name, task, self._emit_count(res, task)))
         if code == _abi.FBR_TASK_OVERFLOW:
             raise OverflowError("%s: result of task %d does not fit int64 (Python ints are unbounded; "
                                 "the device body refuses to wrap)" % (name, task))
@@ -297,6 +419,28 @@ class MapResult:
             yield from self._wait()
             return
         eng = self._engine
+        if getattr(self._spec, "out_dtype", None) is not None:
+            # an emit map: the values of a finished wave are final in the values segment, its end offsets in the result one
+            done, emitted = ctypes.c_uint64(0), 0
+            values = None
+            while emitted < self._n:
+                _abi.check(eng.lib.fbr_result_poll(eng.handle, self._seq, ctypes.byref(done)))
+                if done.value >= self._n:
+                    break
+                if done.value > emitted:
+                    values = self._values_view() if values is None else values
+                    ends = self._peek(max(0, emitted - 1), done.value, np.dtype(np.uint64), ())
+                    if emitted == 0:
+                        ends = np.concatenate([np.zeros(1, np.uint64), ends])
+                    for k in range(len(ends) - 1):
+                        yield _emit_value(self._spec, values[int(ends[k]):int(ends[k + 1])])
+                    emitted = done.value
+                else:
+                    time.sleep(0.0002)
+            res = self._wait()
+            if emitted < self._n:
+                yield from res[emitted:]
+            return
         if self._n_items is not None:
             # bit-packed map: progress is counted in result bytes (8 tasks each); every byte of a finished
             # wave is a full byte, the (masked) last byte of the map only comes from _wait()

@@ -68,6 +68,30 @@ class SharedSegment:
             self.owner = False
 
 
+def values_name(shm_name, blk):
+    """The /dev/shm name of block ``blk``'s values in a map of an emit body (variable-length results): each block's end
+    offsets land in the map's segment like any result records (block-local: they start from 0), its values in a file of
+    their own, which the master concatenates in block order, rebasing the offsets, at get()."""
+    return "%s_v%d" % (shm_name, blk)
+
+
+def put_values(name, values):
+    """Worker side: write a block's values (a 1-D array) to /dev/shm under ``name``.  Written to a private name, then
+    renamed, so a re-dispatched block replaces an earlier attempt's file whole."""
+    path = os.path.join("/dev/shm", name)
+    tmp = "%s.%d.tmp" % (path, os.getpid())
+    np.ascontiguousarray(values).tofile(tmp)
+    os.replace(tmp, path)
+
+
+def _unlink_values(shm_name, n_blocks):
+    for b in range(n_blocks):
+        try:
+            os.unlink(os.path.join("/dev/shm", values_name(shm_name, b)))
+        except FileNotFoundError:
+            pass
+
+
 # ------------------------------------------------------------------------------------------------
 # worker side
 # ------------------------------------------------------------------------------------------------
@@ -133,6 +157,8 @@ def gpu_worker_main(device, conn, results, sys_path, init=None):
                 segments.clear()                                   # one live segment per worker is enough
                 seg = segments.setdefault(shm_name, SharedSegment(shm_name))
             seg.array[off:off + raw.nbytes] = raw                  # placement by index (fiber/pool.py:672), block-wise
+            if getattr(registry.spec(body), "out_dtype", None) is not None:
+                put_values(values_name(shm_name, blk), res.ragged.values)   # an emit body: the block's values beside it
             total = res.sum() if (registry.spec(body).flags & _abi.FBR_BODY_SUMMABLE) else None
             del res, raw
             conn.send(("done", job, blk, total))
@@ -161,9 +187,11 @@ class _Worker:
 
 
 class _Job:
-    def __init__(self, jid, body, kind, chunksize, n, result_bytes, bits, blocks, payload_of, module):
+    def __init__(self, jid, body, kind, chunksize, n, result_bytes, bits, blocks, payload_of, module, out_dtype=None):
         self.id, self.body, self.kind, self.chunksize, self.n = jid, body, kind, chunksize, n
         self.result_bytes, self.bits = result_bytes, bits
+        self.out_dtype = out_dtype                    # emit bodies: the values' dtype (blocks put them in files of their own)
+        self.ranges = [(lo, hi) for _, lo, hi, _ in blocks]
         self.blocks = collections.deque(blocks)       # (blk id, lo, hi, attempt)
         self.n_blocks, self.done_blocks = len(blocks), 0
         self.payload_of, self.module = payload_of, module
@@ -174,6 +202,8 @@ class _Job:
         self.event = threading.Event()
         if self.shm is not None:            # the /dev/shm name never outlives the job object (fire-and-forget maps, failed maps)
             weakref.finalize(self, _release_shm, self.shm)
+            if out_dtype is not None:
+                weakref.finalize(self, _unlink_values, self.shm.name, len(blocks))
 
     def offset(self, lo):
         return lo // 8 if self.bits else lo * self.result_bytes
@@ -190,6 +220,27 @@ class ProcessResult:
         self._pool, self._job, self._spec, self._single = pool, job, spec, single
         self._result = None
 
+    def _emit_result(self):
+        """An emit map: the blocks' end offsets rebased by the values of the blocks before them, and their values
+        concatenated in block order."""
+        from .pool import EmitResultArray
+        job = self._job
+        if job.n == 0:
+            return EmitResultArray(self._spec, np.empty(0, np.uint64), np.empty(0, job.out_dtype))
+        ends = job.shm.array[:job.nbytes].view(np.uint64).copy()
+        parts, base = [], 0
+        for b, (lo, hi) in enumerate(job.ranges):
+            path = os.path.join("/dev/shm", values_name(job.shm.name, b))
+            k = int(ends[hi - 1]) if hi > lo else 0
+            vals = np.fromfile(path, dtype=job.out_dtype)
+            if len(vals) != k:
+                raise RuntimeError("%s: block %d of map %d holds %d values, its offsets say %d" % (job.body, b, job.id, len(vals), k))
+            parts.append(vals)
+            ends[lo:hi] += np.uint64(base)
+            base += k
+        _unlink_values(job.shm.name, len(job.ranges))
+        return EmitResultArray(self._spec, ends, np.concatenate(parts))
+
     def get(self, timeout=None):
         from .pool import ResultArray
         if self._result is None:
@@ -200,7 +251,9 @@ class ProcessResult:
                 raise job.error
             dtype, sub = self._spec.result_dtype()
             total = job.sum if (self._spec.flags & 0x4) else None
-            if job.n == 0:
+            if job.out_dtype is not None:
+                self._result = self._emit_result()
+            elif job.n == 0:
                 self._result = ResultArray(self._spec, np.empty((0,) + sub, dtype), 0)
             elif job.bits:
                 self._result = ResultArray(self._spec, None, total, n=job.n, bits=job.shm.array[:job.nbytes])
@@ -280,7 +333,7 @@ class ProcessPool:
                 raise ValueError("Pool is not running")
             self._next_job += 1
             job = _Job(self._next_job, spec.name, kind, chunksize, n, spec.result_bytes, bits, blocks, payload_of,
-                       registry.module_of(spec.name))
+                       registry.module_of(spec.name), getattr(spec, "out_dtype", None))
             if n == 0:
                 job.event.set()
             else:

@@ -23,7 +23,7 @@ _BOUND = {}  # callables that cannot carry attributes (builtins) -> body name
 
 
 def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entry=None, result=None, shared=None, items=None,
-                **meta):
+                out=None, out_as="list", **meta):
     """Decorator: ``@device_body("pi_inside_det")`` binds ``func`` to the device body ``name`` and sets
     ``func.__fiber_meta__`` (``gpu=1`` unless overridden), like ``fiber.meta``.
 
@@ -58,7 +58,12 @@ def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entr
     A task's items are a 1-D array of the element dtype (or a 1-D array / list whose values the dtype holds exactly: floats
     into an integer dtype or integers out of its range raise ``TypeError``), or, for a 1-byte
     element, ``bytes`` / ``bytearray`` / ``memoryview`` / ``str`` (sent as UTF-8).  ``map(f, Ragged(values, offsets))``
-    passes a whole ragged array without a copy."""
+    passes a whole ragged array without a copy.
+
+    An EMIT record body (``using Out = ...;`` and ``using Res = fbr::NoRes;`` in its struct) returns a variable-length array
+    per task: ``out="<u4"`` describes one element (``result=`` is not passed).  A task's value reads as a list, or, with
+    ``out_as="bytes"`` / ``out_as="str"`` (UTF-8) and a 1-byte element, as ``bytes`` / ``str``; ``result.ragged`` is the
+    whole map as one ``Ragged(values, offsets)``, which an items body can map over directly."""
     from .meta import VALID_META_KEYS
     for k in meta:
         assert k in VALID_META_KEYS, "Invalid meta argument \"{}\"".format(k)
@@ -66,7 +71,7 @@ def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entr
     md.update(meta)
     if source is not None:
         from . import bodies
-        register_module(name, bodies.compile_module(name, source), entry, args, bits_entry, result, shared, items)
+        register_module(name, bodies.compile_module(name, source), entry, args, bits_entry, result, shared, items, out, out_as)
 
     def decorator(func):
         bind(func, name, **md)
@@ -83,7 +88,8 @@ def module_of(name):
     return _MODULES.get(name)
 
 
-def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_entry=None, result=None, shared=None, items=None):
+def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_entry=None, result=None, shared=None, items=None,
+                    out=None, out_as="list"):
     """``fbr_register_body`` + the host-side encoder for the body's argument records (and, with ``bits_entry``, the
     body's bit-packed twin ``<name>_bits8``).  Record bodies (``FBR_BODY_RECORD``) take NumPy dtypes for ``args`` and
     ``result``; their sizes must be the module's ``arg_bytes`` / ``result_bytes`` (``ValueError`` otherwise).
@@ -92,7 +98,9 @@ def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_
     (``group_threads`` > 1 in its module descriptor: several threads per task, records up to 32 KB) registers like any
     other record body.  Items bodies (``FBR_BODY_ITEMS``) take ``items=(parameter name, element dtype)``, whose size must
     be the module's item size, and ``args=None`` when they have no head record; ``items`` is refused for every other
-    body (``ValueError``)."""
+    body (``ValueError``).  Emit bodies (``FBR_BODY_EMIT``) take ``out=<element dtype>``, whose size must be the module's
+    out size, and ``out_as`` ("list", or "bytes" / "str" for 1-byte elements) instead of ``result``; ``out`` is refused for
+    every other body (``ValueError``)."""
     import ctypes
     specs = _load_specs()           # the table as it was: the body registered below gets the encoder its layout asks for
     if bits_entry is not None:
@@ -106,6 +114,25 @@ def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_
     info = _abi.BodyInfo()
     _abi.check(L.fbr_body_info(fid.value, ctypes.byref(info)))
     has_items, has_shared = info.flags & _abi.FBR_BODY_ITEMS, info.flags & _abi.FBR_BODY_BROADCAST
+    out_dtype = None
+    if out is not None and not info.flags & _abi.FBR_BODY_EMIT:
+        raise ValueError("body %s returns a fixed-size result (its record struct has no Out element type): out= is for emit "
+                         "bodies only" % name)
+    if info.flags & _abi.FBR_BODY_EMIT:
+        if out is None:
+            raise ValueError("emit body %s: pass out=<element dtype> (each task returns a variable-length array)" % name)
+        if result is not None:
+            raise ValueError("emit body %s returns a variable-length array of out=: result= is for fixed-size results" % name)
+        ob = ctypes.c_uint32(0)
+        _abi.check(L.fbr_body_emit_info(fid.value, ctypes.byref(ob)))
+        out_dtype = _record_dtype(out, "out", name)
+        if out_dtype.itemsize != ob.value:
+            raise ValueError("%s: out dtype %s is %d bytes, the body's Out is %d" % (name, out_dtype, out_dtype.itemsize, ob.value))
+        if out_as not in ("list", "bytes", "str"):
+            raise ValueError("%s: out_as is 'list', 'bytes' or 'str', got %r" % (name, out_as))
+        if out_as != "list" and out_dtype.itemsize != 1:
+            raise ValueError("%s: out_as=%r needs a 1-byte out element, the body's is %s" % (name, out_as, out_dtype))
+        result = "<u8"                  # the engine's result record of an emit body: each task's end offset
     if items is not None and not has_items:
         raise ValueError("body %s takes no items (its record struct has no Item element type): items= is for items bodies "
                          "only" % name)
@@ -143,8 +170,11 @@ def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_
     if record is not None and isinstance(old, _Record) and old.layouts() != record.layouts():
         raise ValueError("record body %s is registered already with %s; a name keeps its layouts"
                          % (name, ", ".join("%s=%s" % kv for kv in zip(("args", "result", "shared", "items"), old.layouts()))))
+    if record is not None:
+        record.out_dtype, record.out_as = out_dtype, out_as
     # the engine keeps the first module registered under a name (fbr_register_body is idempotent): so do worker processes
-    _MODULES.setdefault(name, (str(module_path), entry, args, bits_entry, result, shared, items))
+    _MODULES.setdefault(name, (str(module_path), entry, args, bits_entry, None if out_dtype is not None else result, shared,
+                               items, out_dtype, out_as))
     if name not in specs:
         if record is not None:
             specs[name] = record

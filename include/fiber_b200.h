@@ -55,12 +55,14 @@ typedef enum fbr_result_kind {
     FBR_RES_U32 = 3,     /* uint32     (Python int) */
     FBR_RES_F64X2 = 4,   /* two float64 (Python tuple of floats) */
     FBR_RES_NONE = 5,    /* body returns None; one pad byte per task */
-    FBR_RES_BITS8 = 6    /* one byte = the bool results of 8 consecutive items, bit k (LSB first) = item
+    FBR_RES_BITS8 = 6,   /* one byte = the bool results of 8 consecutive items, bit k (LSB first) = item
                             8*task + k.  A map over N items is submitted as ceil(N/8) tasks: range() indices
                             (arg_stride 0) or 8 argument items per task record (arg_stride = 8 * item size,
                             fbr_map_desc_t.n_items = N so that items past N are never read).  For range()
                             indices the bits past N in the last byte are computed like any other index and
                             are masked by the caller (fiber_b200/pool.py does) */
+    FBR_RES_OFFSETS = 7  /* emit bodies (FBR_BODY_EMIT): uint64 end offset of each task's values; task j's values are
+                            [end[j-1], end[j]) of the map's values (fbr_result_values), end[-1] = 0 */
 } fbr_result_kind;
 
 #define FBR_BODY_INDEX_ARG 0x1u   /* body can take the task index itself as its int64 argument */
@@ -78,6 +80,10 @@ typedef enum fbr_result_kind {
 #define FBR_BODY_ITEMS 0x40u      /* record body whose task also takes a variable-length array of its Item element type
                                      (fbr_body_items_info); its maps go through fbr_map_submit_items.  arg_bytes may be 0
                                      (no head record, Arg = fbr::NoArg); never with FBR_BODY_INDEX_ARG */
+#define FBR_BODY_EMIT 0x80u       /* record body whose task returns a variable-length array of its Out element type
+                                     (fbr_body_emit_info) instead of a fixed record: result_bytes 8, result kind
+                                     FBR_RES_OFFSETS.  Each map runs a count pass, a scan of the counts and an emit pass;
+                                     never SUMMABLE, no bit-packed twin */
 
 typedef struct fbr_body_info {
     int32_t func_id;
@@ -121,6 +127,9 @@ typedef struct fbr_body_module {
     /* FBR_BODY_ITEMS record bodies: sizeof(Item) (1, 2 or a multiple of 4 up to 4096).  0 (or left out of a hand-written
        descriptor) for every other body */
     uint32_t item_bytes;
+    /* FBR_BODY_EMIT record bodies: sizeof(Out) (1, 2 or a multiple of 4 up to 4096).  0 (or left out of a hand-written
+       descriptor) for every other body */
+    uint32_t out_bytes;
 } fbr_body_module_t;
 typedef const fbr_body_module_t* (*fbr_body_entry_fn)(void);
 int fbr_register_body(const char* name, const char* module_path, const char* entry, int* func_id);
@@ -130,6 +139,8 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
 int fbr_body_shared_info(int func_id, uint32_t* elem_bytes, uint32_t* stage_bytes);
 /* Item size of a FBR_BODY_ITEMS body (0 for other bodies).  The dispatch kernel reads each task's items from global memory. */
 int fbr_body_items_info(int func_id, uint32_t* item_bytes);
+/* Value size of a FBR_BODY_EMIT body (0 for other bodies). */
+int fbr_body_emit_info(int func_id, uint32_t* out_bytes);
 
 /* ---- pool lifecycle -------------------------------------------------------------------------
  * fbr_pool_create   <- ZPool.__init__ (fiber/pool.py:888-943) + worker start
@@ -275,7 +286,8 @@ typedef enum fbr_task_error {
     FBR_TASK_OK = 0,
     FBR_TASK_OVERFLOW = 1,   /* int64 result overflow (Python ints are unbounded: fail loudly) */
     FBR_TASK_BADARG = 2,
-    FBR_TASK_FAULT = 3       /* injected fault (resilient-pool tests) */
+    FBR_TASK_FAULT = 3,      /* injected fault (resilient-pool tests) */
+    FBR_TASK_EMIT = 4        /* an emit body's task pushed another number of values than its count pass gave */
 } fbr_task_error;
 
 int fbr_result_wait(fbr_pool_t* pool, uint64_t seq, int timeout_ms, fbr_result_t* res);
@@ -285,6 +297,16 @@ int fbr_result_data(fbr_pool_t* pool, uint64_t seq, void** data);
 /* Copy results [first, first+count) of a FBR_RESULTS_ON_DEVICE map to host memory (blocking). */
 int fbr_result_fetch(fbr_pool_t* pool, uint64_t seq, uint64_t first, uint64_t count, void* host_dst);
 int fbr_result_release(fbr_pool_t* pool, uint64_t seq);
+/* Maps of FBR_BODY_EMIT bodies (fbr_map_submit / fbr_map_submit_items, neither `out` nor FBR_OUT_DEVICE): the result
+ * records are the n_tasks uint64 end offsets, and the values live in a second segment of n_values elements of out_bytes
+ * each, pinned host memory (fbr_result_values: valid from submission on, final where fbr_result_poll says the tasks are;
+ * each wave's values reach it by one copy of exactly their span through a staging half of ring_bytes, so a claim unit
+ * whose values exceed ring_bytes is refused with FBR_EINVAL)
+ * or, with FBR_RESULTS_ON_DEVICE, engine-owned device memory (fbr_result_fetch_values, blocking).  Submission runs the
+ * count pass and the scan and waits for them (a count pass that fails is reported by fbr_result_wait); the emit pass
+ * then runs like any map.  A worker that dies under an emit map fails it. */
+int fbr_result_values(fbr_pool_t* pool, uint64_t seq, void** values, uint64_t* n_values);
+int fbr_result_fetch_values(fbr_pool_t* pool, uint64_t seq, uint64_t first, uint64_t count, void* host_dst);
 
 /* ---- memory helpers ------------------------------------------------------------------------
  * Pinned host segments are the endpoints that replace LazyZConnection sockets

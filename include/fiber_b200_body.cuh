@@ -108,13 +108,39 @@
 // attempt).  x.data is read-only and points into the map's item array in global memory, so vector loads legal on the
 // array are legal on x.data.  All G lanes of a group body get the same x.  Items bodies cannot have kIndexArg.
 // FBR_EXPORT_RECORD_BODY sets FBR_BODY_ITEMS and writes item_bytes.
+//
+// An EMIT record body's task returns a variable-length array (a document's tokens, an integer's prime factors): it declares
+// the element type and Res = fbr::NoRes, and run() appends to an emitter where other record bodies write Res& r:
+//
+//     struct Tokens {
+//         using Item = uint8_t;  using Arg = fbr::NoArg;
+//         using Out = uint32_t;                           // sizeof 1, 2, or a multiple of 4 up to 4096
+//         using Res = fbr::NoRes;
+//         static constexpr bool kIndexArg = false, kCanFault = false;
+//         __device__ static void run(const fbr::Items<Item>& x, fbr::Emit<Out>& y, uint64_t task_index,
+//                                    const fbr::ErrSink& es, uint32_t attempt) { ... y.push(h); ... }
+//     };
+//     FBR_EXPORT_RECORD_BODY(Tokens, "tokens_u32", tokens_entry, 0)
+//
+// The emitter goes where Res& r goes in every form above (head record or range() index, items, broadcast block, group).
+// A group body takes fbr::Emit<Out, G>& and calls the collective y.push_if(g, pred, v) on every lane: lanes whose pred holds
+// append v in rank order.  y.n is the number of values pushed so far.  Each map runs the body twice per task -- a count
+// pass (y.data is nullptr), then, once the counts are scanned into offsets, an emit pass that writes each task's values
+// at their final place -- so a task's values depend only on its inputs and task_index, never on attempt.  A one-thread body
+// may define `static uint64_t count(...)` (run()'s parameters without y, es and attempt), which the count pass calls
+// instead of run().  A task that pushes another number of values in the emit pass reports FBR_TASK_EMIT, and values past
+// its count are never written.  FBR_EXPORT_RECORD_BODY sets FBR_BODY_EMIT, writes out_bytes, and reports result_bytes 8
+// (each task's uint64 end offset) with result kind FBR_RES_OFFSETS.
 #pragma once
 #include "fiber_b200.h"
 #include "kernels.cuh"      // fiber_b200/csrc: dispatch_thread_kernel, WaveParams, ErrSink, TaskError
 
+#include <algorithm>
 #include <type_traits>
 
 namespace fbr_body_export {
+using fbr_body_launch_fn = void (*)(const void* wave_params, int grid, void* cuda_stream);
+using fbr_body_occupancy_fn = int (*)(int index_mode);
 // CTAs of `kernel` per SM, at least 1 (a failed query leaves no sticky error behind)
 inline int occupancy_of(const void* kernel, int threads, size_t smem) {
     int occ = 0;
@@ -208,18 +234,40 @@ int occupancy_record(int index_mode) {
     }
     return occupancy_of(k, fbr::record::kThreads, smem);
 }
+// emit bodies: the count pass when wp.emit_values is nullptr, else the emit pass; the occupancy is the smaller of the two
+template <class B>
+void launch_emit(const void* wpv, int grid, void* sv) {
+    if (((const fbr::WaveParams*)wpv)->emit_values == nullptr) launch_record<fbr::record::EmitPass<B, false>>(wpv, grid, sv);
+    else launch_record<fbr::record::EmitPass<B, true>>(wpv, grid, sv);
+}
+template <class B>
+int occupancy_emit(int index_mode) {
+    return std::min(occupancy_record<fbr::record::EmitPass<B, false>>(index_mode), occupancy_record<fbr::record::EmitPass<B, true>>(index_mode));
+}
+template <class B>
+constexpr fbr_body_launch_fn record_launch() {
+    if constexpr (fbr::record::EmitOf<B>::kOn) return launch_emit<B>;
+    else return launch_record<B>;
+}
+template <class B>
+constexpr fbr_body_occupancy_fn record_occupancy() {
+    if constexpr (fbr::record::EmitOf<B>::kOn) return occupancy_emit<B>;
+    else return occupancy_record<B>;
+}
 template <class B>
 constexpr bool record_body_ok() {
     static_assert(std::is_trivially_copyable<typename B::Arg>::value && std::is_trivially_copyable<typename B::Res>::value,
                   "record bodies: Arg and Res are trivially copyable");
     static_assert(!B::kIndexArg || std::is_same<typename B::Arg, int64_t>::value, "record bodies with kIndexArg take Arg = int64_t");
+    static_assert(fbr::record::EmitOf<B>::kOn || !std::is_same<typename B::Res, fbr::NoRes>::value,
+                  "record bodies: Res = fbr::NoRes needs an Out element type (an emit body)");
     return true;
 }
 // the flags a record body's descriptor carries on top of the exported ones: broadcast bodies need a block and take it
 template <class B>
 constexpr uint32_t record_flags() {
     return FBR_BODY_RECORD | (fbr::record::BroadcastOf<B>::kOn ? (FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST) : 0u) |
-           (fbr::record::ItemsOf<B>::kOn ? FBR_BODY_ITEMS : 0u);
+           (fbr::record::ItemsOf<B>::kOn ? FBR_BODY_ITEMS : 0u) | (fbr::record::EmitOf<B>::kOn ? FBR_BODY_EMIT : 0u);
 }
 // the descriptor's group_threads: kGroup of a group body, 0 for a one-thread body
 template <class B>
@@ -242,13 +290,13 @@ constexpr uint32_t record_group() {
     extern "C" const fbr_body_module_t* entry(void) {                                                            \
         static const fbr_body_module_t m = {FBR_BODY_MODULE_ABI, (uint32_t)sizeof(fbr::WaveParams), body_name,   \
                                             fbr::record::Layout<Body>::A, fbr::record::Layout<Body>::R,          \
-                                            (uint32_t)FBR_RES_BYTES,                                             \
+                                            (uint32_t)(fbr::record::EmitOf<Body>::kOn ? FBR_RES_OFFSETS : FBR_RES_BYTES), \
                                             (uint32_t)(body_flags) | fbr_body_export::record_flags<Body>(),      \
                                             fbr::record::Layout<Body>::kUnit,                                    \
-                                            fbr_body_export::launch_record<Body>, fbr_body_export::occupancy_record<Body>, \
+                                            fbr_body_export::record_launch<Body>(), fbr_body_export::record_occupancy<Body>(), \
                                             fbr::record::BroadcastOf<Body>::kElem, fbr::record::BroadcastOf<Body>::kStage, \
                                             fbr_body_export::record_group<Body>(),                               \
-                                            fbr::record::ItemsOf<Body>::kElem};                                  \
+                                            fbr::record::ItemsOf<Body>::kElem, fbr::record::EmitOf<Body>::kElem}; \
         return &m;                                                                                               \
     }
 
