@@ -242,7 +242,6 @@ struct Worker {
     int numa_node = -1;                    // host NUMA node the GPU hangs off (-1 unknown)
     int sm_count = 0;
     cudaStream_t s_in = nullptr, s_comp = nullptr, s_out = nullptr;
-    cudaStream_t s_out2 = nullptr;         // FBR_TWO_OUT_STREAMS=1: copy-outs alternate between s_out and s_out2 (by staging half)
     cudaStream_t s_gath = nullptr;         // higher-priority stream for gathers that overlap the next dispatch
     bool prev_wave_overlap = false;        // the previous wave used only its half of the ring
     cudaStream_t s_push = nullptr;         // a stream of the ROOT worker's device: its copy engine pushes this worker's argument waves
@@ -306,6 +305,23 @@ struct PartCtx {                          // constants of one worker's block of 
     uint64_t item_first = 0, item_base = 0, item_count = 0;
 };
 
+// A worker block of an emit map's emit pass: the part-local exclusive offsets its scan produced (count + 1 of them, the last
+// is the block's total) and where its values go.  Blocks are contiguous, so block k's values start at the totals of the
+// blocks before it (base).
+// Where the emit pass writes a block's values:
+//   - FBR_RESULTS_ON_DEVICE: d_values, an engine-owned device buffer of the block's exact size;
+//   - host-resident values of a block that may re-dispatch units (resilient, FBR_FULL_WINDOW): d_values too, copied to the
+//     pinned segment (host) in one piece once no unit is lost any more;
+//   - other host-resident values: wave by wave into the worker's d_vals staging half, each wave's span copied to `host`
+//     behind its kernel; h_offs (a pinned copy of the block's offsets) gives the host every wave's span before it launches.
+struct EmitBlock {
+    uint64_t* d_offs = nullptr;           // null: not an emit pass
+    uint64_t* h_offs = nullptr;           // pinned: the block's count + 1 offsets (waves staged through d_vals)
+    void* d_values = nullptr;
+    uint8_t* host = nullptr;              // the block's first value in the pinned values segment (host-resident maps)
+    uint64_t base = 0, total = 0;
+};
+
 struct SeqPart {
     int worker = 0;
     uint64_t first = 0, count = 0;        // task block of this worker inside the map
@@ -325,30 +341,7 @@ struct SeqPart {
     bool finalized = false;               // resilient: window copied back to the host
     bool first_wave_pending = true;       // the block's first wave must wait for what submit_part put on s_in
     PartCtx cx;
-};
-
-// One worker block of an emit map: the part-local exclusive offsets its scan produced (count + 1 of them, the last is the
-// block's total) and where its values go.  Blocks are contiguous, so block k's values start at the totals of the blocks
-// before it (base).
-// Where the emit pass writes a block's values:
-//   - FBR_RESULTS_ON_DEVICE: d_values, an engine-owned device buffer of the block's exact size;
-//   - host-resident values of a block that may re-dispatch units (resilient, FBR_FULL_WINDOW): d_values too, copied to the
-//     pinned segment (host) in one piece once no unit is lost any more;
-//   - other host-resident values: wave by wave into the worker's d_vals staging half, each wave's span copied to `host`
-//     behind its kernel; h_offs (a pinned copy of the block's offsets) gives the host every wave's span before it launches.
-struct EmitPart {
-    int worker = 0;
-    uint64_t first = 0, count = 0, base = 0, total = 0;
-    uint64_t* d_offs = nullptr;
-    void* d_values = nullptr;
-    uint8_t* host = nullptr;              // the block's first value in the pinned values segment (host-resident maps)
-    uint64_t* h_offs = nullptr;           // pinned: the block's count + 1 offsets (waves staged through d_vals)
-};
-struct EmitPlan {
-    std::vector<EmitPart> parts;
-    uint32_t out_bytes = 0;
-    void* values = nullptr;               // pinned values segment (host-resident results)
-    uint64_t n_values = 0;
+    EmitBlock emit;
 };
 
 struct SeqState {
@@ -374,7 +367,9 @@ struct SeqState {
     bool release_pending = false;          // fbr_result_release arrived while they were waiting: the last one out frees the seq
     int dead_worker = -1;                  // a worker died under this map and the map could not be re-dispatched
     int dead_error = 0;
-    EmitPlan emit;                         // emit maps: per-block offsets and values (empty parts for every other map)
+    bool emit_pass = false;                // the emit pass of an emit map: its blocks carry the offsets their workers counted
+    void* values = nullptr;                // emit pass: pinned values segment (host-resident results) ...
+    uint64_t n_values = 0;                 // ... and the map's number of values
 };
 
 struct SharedBlock {
@@ -554,7 +549,6 @@ static int worker_init(fbr_pool* p, Worker& w, int device) {
     CK(cudaStreamCreateWithFlags(&w.s_in, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&w.s_comp, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&w.s_out, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&w.s_out2, cudaStreamNonBlocking));
     {
         int lo_prio = 0, hi_prio = 0;
         CK(cudaDeviceGetStreamPriorityRange(&lo_prio, &hi_prio));
@@ -607,7 +601,6 @@ static void worker_destroy(Worker& w) {
     if (w.s_in) cudaStreamSynchronize(w.s_in);
     if (w.s_comp) cudaStreamSynchronize(w.s_comp);
     if (w.s_out) cudaStreamSynchronize(w.s_out);
-    if (w.s_out2) { cudaStreamSynchronize(w.s_out2); cudaStreamDestroy(w.s_out2); }
     if (w.s_gath) { cudaStreamSynchronize(w.s_gath); cudaStreamDestroy(w.s_gath); }
     if (w.s_push) {                        // lives on the root worker's device
         cudaSetDevice(w.push_root_device);
@@ -840,20 +833,18 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
     wp.item_first = item_first;
     wp.item_base = item_base;
     wp.item_count = item_count;
-    const EmitPart* emit = nullptr;
+    const EmitBlock& emit = part.emit;
     uint64_t v_lo = 0, v_hi = 0;            // staged emit waves: the wave's span of the block's values
-    for (const EmitPart& e : st.emit.parts)
-        if (e.worker == part.worker) emit = &e;
-    if (emit) {
-        wp.emit_offs = emit->d_offs;
-        wp.emit_first = emit->first;
-        wp.emit_base = emit->base;
-        if (emit->h_offs) {
-            v_lo = emit->h_offs[wave_first - emit->first];
-            v_hi = emit->h_offs[wave_first - emit->first + wt];
-            wp.emit_values = w.d_vals[half] - v_lo * st.emit.out_bytes;     // the wave's first value lands at d_vals[half]
+    if (emit.d_offs) {
+        wp.emit_offs = emit.d_offs;
+        wp.emit_first = part.first;
+        wp.emit_base = emit.base;
+        if (emit.h_offs) {
+            v_lo = emit.h_offs[wave_first - part.first];
+            v_hi = emit.h_offs[wave_first - part.first + wt];
+            wp.emit_values = w.d_vals[half] - v_lo * body.out_bytes;     // the wave's first value lands at d_vals[half]
         } else {
-            wp.emit_values = (uint8_t*)emit->d_values;
+            wp.emit_values = (uint8_t*)emit.d_values;
         }
     }
     int occ_d = worker_occ(w, st.func_id, body, d.arg_stride == 0);
@@ -963,24 +954,21 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
         cudaEvent_t wd;
         CK(cudaEventCreateWithFlags(&wd, cudaEventDisableTiming));
         if (!cx.full_window) {
-            // one copy-out stream by default; alternating two (FBR_TWO_OUT_STREAMS=1) is kept for experiments
-            static const bool two_out = getenv("FBR_TWO_OUT_STREAMS") && atoi(getenv("FBR_TWO_OUT_STREAMS")) != 0;
-            cudaStream_t so = (half && two_out) ? w.s_out2 : w.s_out;
-            CK(cudaStreamWaitEvent(so, w.ev_comp[rw], 0));
+            CK(cudaStreamWaitEvent(w.s_out, w.ev_comp[rw], 0));
             if (cx.peer_out) {      // this worker's copy engine writes the wave into the root's ordered output (posted NVLink writes)
-                CK(cudaMemcpyPeerAsync((uint8_t*)st.out + wave_first * cx.R, p->workers[0].device, w.d_out[half], w.device, wt * cx.R, so));
+                CK(cudaMemcpyPeerAsync((uint8_t*)st.out + wave_first * cx.R, p->workers[0].device, w.d_out[half], w.device, wt * cx.R, w.s_out));
                 STAT_ADD(p, peer_push_bytes, wt * cx.R);
             } else {
-                CK(cudaMemcpyAsync((uint8_t*)st.out + wave_first * cx.R, w.d_out[half], wt * cx.R, cudaMemcpyDeviceToHost, so));
+                CK(cudaMemcpyAsync((uint8_t*)st.out + wave_first * cx.R, w.d_out[half], wt * cx.R, cudaMemcpyDeviceToHost, w.s_out));
                 STAT_ADD(p, d2h_bytes, wt * cx.R);
             }
-            if (emit && emit->h_offs && v_hi > v_lo) {   // the wave's values, exactly its span, into the pinned segment
-                const uint64_t ob = st.emit.out_bytes;
-                CK(cudaMemcpyAsync(emit->host + v_lo * ob, w.d_vals[half], (v_hi - v_lo) * ob, cudaMemcpyDeviceToHost, so));
+            if (v_hi > v_lo) {   // the wave's values, exactly its span, into the pinned segment
+                const uint64_t ob = body.out_bytes;
+                CK(cudaMemcpyAsync(emit.host + v_lo * ob, w.d_vals[half], (v_hi - v_lo) * ob, cudaMemcpyDeviceToHost, w.s_out));
                 STAT_ADD(p, d2h_bytes, (v_hi - v_lo) * ob);
             }
-            CK(cudaEventRecord(w.ev_out[half], so));
-            CK(cudaEventRecord(wd, so));
+            CK(cudaEventRecord(w.ev_out[half], w.s_out));
+            CK(cudaEventRecord(wd, w.s_out));
         } else {
             CK(cudaEventRecord(wd, direct ? w.s_comp : s_g));
         }
@@ -996,38 +984,42 @@ static int finish_round(fbr_pool* p, SeqState& st, SeqPart& part, bool copy_wind
     const PartCtx& cx = part.cx;
     const int slot = part.ctrl_slot;
     const int last_rw = (int)((w.wave_no - 1) % kRecWindows);
-    // A block whose results never pass through the copy-out stream (device-resident output, zero-copy stores into the
-    // pinned segment) finishes on the compute stream itself: its control block follows its last kernel without a
-    // cross-stream hop.  Everything else finishes on s_out, behind its copy-outs.
-    // (Off: a copy on the compute stream puts a DMA hop between back-to-back kernels of pipelined maps, which costs
-    // them what a blocking map() gains.  FBR_FINISH_ON_COMP=1 enables it for A/B runs.)
-    static const bool finish_on_comp = getenv("FBR_FINISH_ON_COMP") && atoi(getenv("FBR_FINISH_ON_COMP")) != 0;
-    const bool on_comp = finish_on_comp && cx.direct && cx.full_window && !cx.resilient && (cx.zero_copy || cx.out_dev || cx.keep_on_device);
-    cudaStream_t sf = on_comp ? w.s_comp : w.s_out;
-    if (!on_comp) {
-        CK(cudaStreamWaitEvent(w.s_out, w.ev_comp[last_rw], 0));
-        CK(cudaStreamWaitEvent(w.s_out, w.ev_out[0], 0));      // copy-outs issued on either out stream are complete
-        CK(cudaStreamWaitEvent(w.s_out, w.ev_out[1], 0));
-    }
+    // Every block finishes on s_out, behind its copy-outs, even one without any: finishing on the compute stream puts a
+    // DMA hop between back-to-back kernels of pipelined maps, which costs them what a blocking map() gains.
+    CK(cudaStreamWaitEvent(w.s_out, w.ev_comp[last_rw], 0));
     if (copy_window && cx.full_window && !cx.out_dev && !cx.keep_on_device && !cx.zero_copy && part.count) {
-        CK(cudaMemcpyAsync((uint8_t*)st.out + part.first * cx.R, cx.window_base, part.count * cx.R, cudaMemcpyDeviceToHost, sf));
+        CK(cudaMemcpyAsync((uint8_t*)st.out + part.first * cx.R, cx.window_base, part.count * cx.R, cudaMemcpyDeviceToHost, w.s_out));
         STAT_ADD(p, d2h_bytes, part.count * cx.R);
     }
-    if (copy_window)
-        for (const EmitPart& e : st.emit.parts)
-            if (e.worker == part.worker && e.host && e.d_values && e.total) {
-                CK(cudaMemcpyAsync(e.host, e.d_values, e.total * st.emit.out_bytes, cudaMemcpyDeviceToHost, sf));
-                STAT_ADD(p, d2h_bytes, e.total * st.emit.out_bytes);
-            }
-    CK(cudaMemcpyAsync(&w.h_ctrl[slot], &w.d_ctrl[slot], sizeof(SeqCtrl), cudaMemcpyDeviceToHost, sf));
+    const EmitBlock& e = part.emit;
+    if (copy_window && e.host && e.d_values && e.total) {
+        const uint64_t vbytes = e.total * body_of(st.func_id)->out_bytes;
+        CK(cudaMemcpyAsync(e.host, e.d_values, vbytes, cudaMemcpyDeviceToHost, w.s_out));
+        STAT_ADD(p, d2h_bytes, vbytes);
+    }
+    CK(cudaMemcpyAsync(&w.h_ctrl[slot], &w.d_ctrl[slot], sizeof(SeqCtrl), cudaMemcpyDeviceToHost, w.s_out));
     if (cx.resilient && part.lost_cap)
-        CK(cudaMemcpyAsync(part.h_lost, part.d_lost, sizeof(LostUnit) * part.lost_cap, cudaMemcpyDeviceToHost, sf));
+        CK(cudaMemcpyAsync(part.h_lost, part.d_lost, sizeof(LostUnit) * part.lost_cap, cudaMemcpyDeviceToHost, w.s_out));
     // one event per part for its whole life, re-recorded every round: another waiter may hold the handle
     // (fbr_result_wait blocks on it outside the pool lock), so it must never be destroyed under it
     if (!part.done) CK(cudaEventCreateWithFlags(&part.done, cudaEventDisableTiming));
-    CK(cudaEventRecord(part.done, sf));
+    CK(cudaEventRecord(part.done, w.s_out));
     return FBR_OK;
 }
+
+// A variable-length stream of a block that travels wave by wave through a worker's two ring_bytes staging halves:
+// host-resident items in (d_items), host-staged emit values out (d_vals).
+struct StagedStream {
+    const uint64_t* offs;       // host offsets rebased to the block: offs[t] belongs to task part.first + t
+    uint64_t elem_bytes;
+    bool header;                // the wave's wt + 1 offsets travel ahead of its data, in a 256 B-rounded header
+    const char* too_large;      // error for a claim unit no half holds: its tasks [t0, t1), its data bytes, ring_bytes
+    uint64_t data_bytes(uint64_t t0, uint64_t t1) const { return (offs[t1] - offs[t0]) * elem_bytes; }
+    // what tasks [t0, t1) of the block take of a staging half
+    uint64_t staged_bytes(uint64_t t0, uint64_t t1) const {
+        return (header ? round_up((t1 - t0 + 1) * sizeof(uint64_t), 256) : 0) + data_bytes(t0, t1);
+    }
+};
 
 static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& body) {
     Worker& w = p->workers[part.worker];
@@ -1205,9 +1197,7 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
         if (body.result_kind == FBR_RES_BITS8 && !cx.host_args) n_waves = 6;
         if (const char* e = getenv("FBR_WAVES")) n_waves = std::max<uint64_t>(1, (uint64_t)atoll(e));                          // tuning knob
         const uint64_t share = round_up((part.count + n_waves - 1) / n_waves, unit);
-        static const bool pyr = getenv("FBR_PYRAMID") && atoi(getenv("FBR_PYRAMID")) != 0;
-        if (!(pyr && (cx.peer_push || cx.peer_out)))      // (the pyramid schedule uses the whole staging half)
-            cx.wave_tasks_cap = std::min(cx.wave_tasks_cap, std::max(min_wave_tasks, share));
+        cx.wave_tasks_cap = std::min(cx.wave_tasks_cap, std::max(min_wave_tasks, share));
     }
 
     // staging
@@ -1239,92 +1229,43 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
         cx.sum_kind = 1;   // the dispatch kernel folds sum(results) while they are in registers
     }
 
-    // Wave schedule of a block whose results stream out (host segment or the root GPU): the chain of copy-outs is the
-    // critical path when a wave's copy (transfer + set-up) takes longer than its kernel.  Equal waves are the default.
-    // Opt-in alternatives (each extra wave costs chain latency): opening the block with a quarter-size and a
-    // half-size wave so the first copy starts earlier (FBR_RAMP=1), halving the LAST waves to shrink the exposed
-    // tail copy (FBR_TAPER=1).
-    static const bool taper_on = getenv("FBR_TAPER") && atoi(getenv("FBR_TAPER")) != 0;
-    static const bool ramp_on = getenv("FBR_RAMP") && atoi(getenv("FBR_RAMP")) != 0;
-    const bool streaming_out = !cx.full_window && !cx.host_args;
-    const bool taper = taper_on && streaming_out;
-    const bool ramp = ramp_on && streaming_out && part.count > 4 * cx.wave_tasks_cap;
-    const uint64_t min_tail_tasks = round_up(std::max<uint64_t>(1, (256ull << 10) / std::max<uint32_t>(1, R)), unit);
-    // Blocks streamed over NVLink by copy engines (root-resident maps).  Raw peer copies are faster in large pieces
-    // than in 64 MB ones, which suggests a pyramid of waves -- doubling from cap/16 up to the staging capacity,
-    // halving again towards the end: few large copies, short fill and drain.  Equal waves stay the default
-    // (FBR_PYRAMID=1 enables the pyramid).
-    static const bool pyramid_on = getenv("FBR_PYRAMID") && atoi(getenv("FBR_PYRAMID")) != 0;
-    const bool pyramid = pyramid_on && (cx.peer_push || cx.peer_out);
-    const uint64_t pyr_base = round_up(std::max<uint64_t>(unit, cx.wave_tasks_cap / 16), unit);
-    if (cx.host_items) {
-        // before any wave launches: every claim unit's offsets and items must fit one staging half
-        const uint64_t* o = st.items.offsets;
-        for (uint64_t t0 = part.first; t0 < part.first + part.count; t0 += unit) {
-            const uint64_t t1 = std::min<uint64_t>(t0 + unit, part.first + part.count);
-            const uint64_t ib = (o[t1] - o[t0]) * st.items.item_bytes;
-            if (round_up((t1 - t0 + 1) * sizeof(uint64_t), 256) + ib > p->ring_bytes)
-                return fail(FBR_EINVAL, "the claim unit of tasks [%llu, %llu) carries %llu item bytes, more than a staging half of "
-                            "ring_bytes %llu holds with its offsets: raise ring_bytes or split the items",
-                            (unsigned long long)t0, (unsigned long long)t1, (unsigned long long)ib, (unsigned long long)p->ring_bytes);
-        }
-    }
-    // emit maps whose values stream wave by wave: each wave's values must fit one staging half, so every claim unit's must
-    const EmitPart* emit = nullptr;
-    for (const EmitPart& e : st.emit.parts)
-        if (e.worker == part.worker && e.h_offs) emit = &e;
-    const uint64_t ob = st.emit.out_bytes;
-    if (emit) {
-        for (int i = 0; i < 2; ++i)
-            if (!w.d_vals[i]) CK(cudaMalloc((void**)&w.d_vals[i], p->ring_bytes));
-        const uint64_t* o = emit->h_offs;
+    // before any wave launches: every claim unit of every staged stream must fit one staging half
+    std::vector<StagedStream> streams;
+    if (cx.host_items)
+        streams.push_back({st.items.offsets + part.first, st.items.item_bytes, true,
+                           "the claim unit of tasks [%llu, %llu) carries %llu item bytes, more than a staging half of "
+                           "ring_bytes %llu holds with its offsets: raise ring_bytes or split the items"});
+    if (part.emit.h_offs)
+        streams.push_back({part.emit.h_offs, body.out_bytes, false,
+                           "the claim unit of tasks [%llu, %llu) emits %llu value bytes, more than a staging half of "
+                           "ring_bytes %llu holds: raise ring_bytes or use results=\"device\""});
+    for (const StagedStream& s : streams)
         for (uint64_t t0 = 0; t0 < part.count; t0 += unit) {
             const uint64_t t1 = std::min<uint64_t>(t0 + unit, part.count);
-            if ((o[t1] - o[t0]) * ob > p->ring_bytes)
-                return fail(FBR_EINVAL, "the claim unit of tasks [%llu, %llu) emits %llu value bytes, more than a staging half of "
-                            "ring_bytes %llu holds: raise ring_bytes or use results=\"device\"", (unsigned long long)(part.first + t0),
-                            (unsigned long long)(part.first + t1), (unsigned long long)((o[t1] - o[t0]) * ob), (unsigned long long)p->ring_bytes);
+            if (s.staged_bytes(t0, t1) > p->ring_bytes)
+                return fail(FBR_EINVAL, s.too_large, (unsigned long long)(part.first + t0), (unsigned long long)(part.first + t1),
+                            (unsigned long long)s.data_bytes(t0, t1), (unsigned long long)p->ring_bytes);
         }
-    }
+    if (part.emit.h_offs)
+        for (int i = 0; i < 2; ++i)
+            if (!w.d_vals[i]) CK(cudaMalloc((void**)&w.d_vals[i], p->ring_bytes));
     uint64_t done_tasks = 0;
-    uint32_t wave_idx = 0;
     while (done_tasks < part.count) {
         uint64_t wt = std::min<uint64_t>(cx.wave_tasks_cap, part.count - done_tasks);
-        const uint64_t left = part.count - done_tasks;
-        if (ramp && wave_idx < 2) wt = std::min(left, round_up(cx.wave_tasks_cap >> (2 - wave_idx), unit));
-        if (pyramid) {
-            const uint64_t up = wave_idx < 8 ? pyr_base << wave_idx : cx.wave_tasks_cap;
-            const uint64_t down = std::max(pyr_base, round_up(left / 2, unit));
-            wt = std::min(std::min(left, cx.wave_tasks_cap), std::min(up, down));
-        }
-        ++wave_idx;
-        if (taper && left <= 2 * cx.wave_tasks_cap && left > min_tail_tasks)
-            wt = std::min(left, std::max(min_tail_tasks, round_up(left / 2, unit)));
-        if (cx.host_items) {
-            // the wave's offsets and item span must fit one staging half: the most whole units (or the rest of the block)
-            // that do, found by binary search over the host offsets
-            const uint64_t* o = st.items.offsets;
-            const uint64_t f = part.first + done_tasks;
+        if (!streams.empty()) {
+            // the most whole units (or the rest of the block) whose wave fits one staging half in every stream, at least
+            // one unit (each fits: checked above), by binary search over the host offsets
             auto fits = [&](uint64_t tasks) {
-                return round_up((tasks + 1) * sizeof(uint64_t), 256) + (o[f + tasks] - o[f]) * st.items.item_bytes <= p->ring_bytes;
+                for (const StagedStream& s : streams)
+                    if (s.staged_bytes(done_tasks, done_tasks + tasks) > p->ring_bytes) return false;
+                return true;
             };
             uint64_t lo_u = 0, hi_u = (wt + unit - 1) / unit;               // fits(lo_u units) holds (0 tasks always fit)
             while (lo_u < hi_u) {
                 const uint64_t mid = (lo_u + hi_u + 1) / 2;
                 if (fits(std::min<uint64_t>(mid * unit, wt))) lo_u = mid; else hi_u = mid - 1;
             }
-            wt = std::min<uint64_t>(std::max<uint64_t>(lo_u, 1) * unit, wt);     // every unit fits (checked above)
-        }
-        if (emit) {
-            // the most whole units (or the rest of the block) whose values fit one staging half, by binary search over the
-            // block's offsets
-            const uint64_t* o = emit->h_offs + done_tasks;
-            uint64_t lo_u = 0, hi_u = (wt + unit - 1) / unit;
-            while (lo_u < hi_u) {
-                const uint64_t mid = (lo_u + hi_u + 1) / 2;
-                if ((o[std::min<uint64_t>(mid * unit, wt)] - o[0]) * ob <= p->ring_bytes) lo_u = mid; else hi_u = mid - 1;
-            }
-            wt = std::min<uint64_t>(std::max<uint64_t>(lo_u, 1) * unit, wt);     // every unit fits (checked above)
+            wt = std::min<uint64_t>(std::max<uint64_t>(lo_u, 1) * unit, wt);
         }
         const uint32_t n_units = (uint32_t)((wt + unit - 1) / unit);
         const uint64_t wno = w.wave_no++;
@@ -1472,8 +1413,8 @@ static void on_worker_death(fbr_pool* p, int wi, cudaError_t err) {
         if (!touched) continue;
         // device-resident arguments / outputs of a map live on worker 0
         const bool on_w0 = (st.flags & (FBR_ARGS_DEVICE | FBR_OUT_DEVICE)) != 0;
-        // an emit map's blocks carry the offsets of the workers that counted them: it is failed, not re-cut
-        if (!(st.flags & FBR_RESILIENT) || live.empty() || (on_w0 && p->workers[0].dead) || !st.emit.parts.empty()) {
+        // an emit pass's blocks carry the offsets of the workers that counted them: it is failed, not re-cut
+        if (!(st.flags & FBR_RESILIENT) || live.empty() || (on_w0 && p->workers[0].dead) || st.emit_pass) {
             st.dead_worker = wi;
             st.dead_error = (int)err;
             continue;
@@ -1508,6 +1449,18 @@ static void on_worker_death(fbr_pool* p, int wi, cudaError_t err) {
     }
 }
 
+// A block's emit buffers.  The device ones go with a dead worker's context; the pinned offsets are host memory.
+static void free_emit_block(fbr_pool* p, int worker, EmitBlock& e) {
+    Worker& w = p->workers[worker];
+    if (!w.dead) {
+        cudaSetDevice(w.device);
+        if (e.d_offs) cudaFreeAsync(e.d_offs, w.s_in);
+        if (e.d_values) cudaFreeAsync(e.d_values, w.s_in);
+    }
+    if (e.h_offs) pinned_release(p, e.h_offs);
+    e = EmitBlock();
+}
+
 static void free_seq(fbr_pool* p, SeqState& st) {
     for (auto& part : st.graveyard)        // device-side resources died with the worker's context
         if (part.h_lost) cudaFreeHost(part.h_lost);
@@ -1516,6 +1469,7 @@ static void free_seq(fbr_pool* p, SeqState& st) {
         Worker& w = p->workers[part.worker];
         if (w.dead) {                      // nothing on a dead context can be freed (or needs to be)
             if (part.h_lost) cudaFreeHost(part.h_lost);
+            free_emit_block(p, part.worker, part.emit);
             continue;
         }
         cudaSetDevice(w.device);
@@ -1531,20 +1485,12 @@ static void free_seq(fbr_pool* p, SeqState& st) {
         if (part.d_items) cudaFreeAsync(part.d_items, w.s_in);
         if (part.d_item_offs) cudaFreeAsync(part.d_item_offs, w.s_in);
         if (part.d_lost) cudaFreeAsync(part.d_lost, w.s_in);
+        free_emit_block(p, part.worker, part.emit);
         if (part.h_lost) cudaFreeHost(part.h_lost);
         if (part.ctrl_slot >= 0) w.ctrl_free.push_back(part.ctrl_slot);
     }
-    for (const EmitPart& e : st.emit.parts) {
-        Worker& w = p->workers[e.worker];
-        if (w.dead) continue;
-        cudaSetDevice(w.device);
-        if (e.d_offs) cudaFreeAsync(e.d_offs, w.s_in);
-        if (e.d_values) cudaFreeAsync(e.d_values, w.s_in);
-        if (e.h_offs) pinned_release(p, e.h_offs);
-    }
-    st.emit.parts.clear();
-    if (st.emit.values) pinned_release(p, st.emit.values);
-    st.emit.values = nullptr;
+    if (st.values) pinned_release(p, st.values);
+    st.values = nullptr;
     if (st.own_out && st.out && !numa_pinned_release(p, st.out)) pinned_release(p, st.out);
 }
 
@@ -1855,7 +1801,6 @@ int fbr_pool_join(fbr_pool_t* p) {
         CK(cudaStreamSynchronize(w.s_comp));
         CK(cudaStreamSynchronize(w.s_gath));
         CK(cudaStreamSynchronize(w.s_out));
-        CK(cudaStreamSynchronize(w.s_out2));
     }
     return FBR_OK;
 }
@@ -1964,64 +1909,146 @@ int fbr_map_submit_items(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items
     return map_submit(p, d, it, seq_out);
 }
 
-static int map_submit_plan(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out,
-                           EmitPlan* plan);
+// Submits one map.  The emit pass of an emit map passes `counted`, the count pass's blocks with their emit state, and
+// `values`, the pinned values segment of n_values values: it runs over exactly those blocks and takes both over.
+static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out,
+                           std::vector<SeqPart>* counted = nullptr, void** values = nullptr, uint64_t n_values = 0);
 static int emit_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out);
+static void harvest(fbr_pool* p, SeqState& st);
 
 static int map_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out) {
     const BodyEntry* b = body_of(d->func_id);
     if (b && (b->flags & FBR_BODY_EMIT)) return emit_submit(p, d, items, seq_out);
-    return map_submit_plan(p, d, items, seq_out, nullptr);
+    return map_submit_pass(p, d, items, seq_out);
+}
+
+// Emit map, step 2: scan_counts_kernel turns each block of the count pass `cseq` into an entry of `blocks` (task order)
+// with its offsets and, in *totals, its total; `scanned` gets an event per scan.  With `host_offs` the host also gets a
+// pinned copy of each block's offsets, to cut the emit pass's waves by.
+static int emit_scan(fbr_pool_t* p, uint64_t cseq, bool host_offs, std::vector<SeqPart>& blocks, uint64_t** totals,
+                     std::vector<std::pair<int, cudaEvent_t>>& scanned) {
+    std::lock_guard<std::mutex> g(p->mu);
+    auto it = p->seqs.find(cseq);
+    if (it == p->seqs.end()) return fail(FBR_ENOENT, "count pass of an emit map was released");
+    std::vector<const SeqPart*> parts;
+    for (auto& part : it->second->parts) parts.push_back(&part);
+    std::sort(parts.begin(), parts.end(), [](const SeqPart* a, const SeqPart* b) { return a->first < b->first; });
+    // one total per block, written by its scan into pinned memory (mapped into every device's address space)
+    int rc = pinned_acquire(p, sizeof(uint64_t) * std::max<size_t>(1, parts.size()), (void**)totals);
+    if (rc != FBR_OK) return rc;
+    for (size_t k = 0; k < parts.size(); ++k) {
+        const SeqPart& part = *parts[k];
+        Worker& w = p->workers[part.worker];
+        const uint64_t tiles = part.count / scan::kTile + 1;
+        if (tiles >= (1ull << 31)) return fail(FBR_EINVAL, "emit map block of %llu tasks is too large to scan", (unsigned long long)part.count);
+        const uint64_t obytes = (part.count + 1) * sizeof(uint64_t);
+        SeqPart b;
+        b.worker = part.worker;
+        b.first = part.first;
+        b.count = part.count;
+        CK(cudaSetDevice(w.device));
+        CK(cudaMallocAsync((void**)&b.emit.d_offs, obytes, w.s_comp));
+        blocks.push_back(std::move(b));
+        EmitBlock& e = blocks.back().emit;
+        void* scratch = nullptr;
+        CK(cudaMallocAsync(&scratch, (tiles + 1) * sizeof(uint64_t), w.s_comp));
+        cudaMemsetAsync(scratch, 0, (tiles + 1) * sizeof(uint64_t), w.s_comp);
+        scan_counts_kernel<<<(unsigned)tiles, scan::kThreads, 0, w.s_comp>>>(
+            (const uint64_t*)part.cx.window_base, part.count, e.d_offs, (unsigned long long*)scratch,
+            (uint32_t*)((uint64_t*)scratch + tiles), *totals + k);
+        const cudaError_t launched = cudaGetLastError();
+        cudaFreeAsync(scratch, w.s_comp);
+        if (launched != cudaSuccess) return fail(FBR_ECUDA, "scan_counts_kernel: %s", cudaGetErrorString(launched));
+        if (host_offs) {
+            rc = pinned_acquire(p, obytes, (void**)&e.h_offs);
+            if (rc != FBR_OK) return rc;
+            CK(cudaMemcpyAsync(e.h_offs, e.d_offs, obytes, cudaMemcpyDeviceToHost, w.s_comp));
+        }
+        cudaEvent_t ev;
+        CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        scanned.push_back({w.device, ev});
+        CK(cudaEventRecord(ev, w.s_comp));
+    }
+    return FBR_OK;
+}
+
+// Emit map, step 3: the blocks' totals give each block its base and the map its n_values.  Host-resident values go to
+// one pinned segment (*values); a block whose values do not stream through the staging halves (no h_offs: values kept
+// on the device, or units that may be re-dispatched) is written to a device buffer of its own.
+static int emit_place(fbr_pool_t* p, const BodyEntry& body, bool on_device, std::vector<SeqPart>& blocks,
+                      const uint64_t* totals, void** values, uint64_t* n_values) {
+    std::lock_guard<std::mutex> g(p->mu);
+    const uint64_t ob = body.out_bytes;
+    for (size_t k = 0; k < blocks.size(); ++k) {
+        blocks[k].emit.total = totals[k];
+        blocks[k].emit.base = *n_values;
+        *n_values += totals[k];
+    }
+    if (*n_values >= (1ull << 62) / std::max<uint32_t>(1, body.out_bytes))
+        return fail(FBR_EINVAL, "body %s: the map's count pass gave %llu values, too many to place", body.name.c_str(),
+                    (unsigned long long)*n_values);
+    if (!on_device) {
+        int rc = pinned_acquire(p, *n_values * ob, values);
+        if (rc != FBR_OK) return rc;
+        for (SeqPart& b : blocks) b.emit.host = (uint8_t*)*values + b.emit.base * ob;
+    }
+    for (SeqPart& b : blocks)
+        if (!b.emit.h_offs) {
+            Worker& w = p->workers[b.worker];
+            CK(cudaSetDevice(w.device));
+            CK(cudaMallocAsync(&b.emit.d_values, std::max<uint64_t>(16, b.emit.total * ob), w.s_comp));
+        }
+    return FBR_OK;
 }
 
 // An emit map: the count pass is an ordinary map of the body whose records (the tasks' counts) stay on the device; once it
 // is done, scan_counts_kernel turns each block's counts into its offsets and total, the host sizes the values segment from
-// the totals, and the emit pass runs as a second ordinary map over the same blocks (`plan`).
+// the totals, and the emit pass runs as a second ordinary map over the same blocks.
 static int emit_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out) {
     const BodyEntry& body = *body_of(d->func_id);
     if (d->out || (d->flags & FBR_OUT_DEVICE))
         return fail(FBR_EINVAL, "body %s emits variable-length results: its maps own their output (no out, no FBR_OUT_DEVICE)", body.name.c_str());
+    const bool on_device = (d->flags & FBR_RESULTS_ON_DEVICE) != 0;
+    const bool whole_block = (d->flags & (FBR_RESILIENT | FBR_FULL_WINDOW)) != 0;   // units may be re-dispatched: no waves
+    // 1. the count pass
     fbr_map_desc_t cd = *d;
     cd.flags |= FBR_RESULTS_ON_DEVICE;
     uint64_t cseq = 0;
-    int rc = map_submit_plan(p, &cd, items, &cseq, nullptr);
+    int rc = map_submit_pass(p, &cd, items, &cseq);
     if (rc != FBR_OK) return rc;
     fbr_result_t cres;
     rc = fbr_result_wait(p, cseq, -1, &cres);
-    if (rc != FBR_OK && rc != FBR_ETASK) {
-        const std::string msg = g_err;
-        fbr_result_release(p, cseq);
-        g_err = msg;
-        return rc;
-    }
-    EmitPlan plan;
-    plan.out_bytes = body.out_bytes;
-    const bool on_device = (d->flags & FBR_RESULTS_ON_DEVICE) != 0;
-    const bool whole_block = (d->flags & (FBR_RESILIENT | FBR_FULL_WINDOW)) != 0;   // units may be re-dispatched: no waves
+    // 2. scan each block, then one wait per block outside the pool lock: then every total is in
+    std::vector<SeqPart> blocks;                       // the count pass's blocks, each with its emit state
     uint64_t* totals = nullptr;
-    // drop the count pass, the totals (and, on failure, what the plan holds so far) under the pool lock
-    auto drop = [&](bool with_plan) {
+    std::vector<std::pair<int, cudaEvent_t>> scanned;  // (device, event after its block's scan)
+    if (rc == FBR_OK) rc = emit_scan(p, cseq, !on_device && !whole_block, blocks, &totals, scanned);
+    for (auto& s : scanned) {
+        cudaSetDevice(s.first);
+        if (rc == FBR_OK && cudaEventSynchronize(s.second) != cudaSuccess) rc = fail(FBR_ECUDA, "waiting for scan_counts_kernel failed");
+        cudaEventDestroy(s.second);
+    }
+    // 3. size and place the values
+    void* values = nullptr;
+    uint64_t n_values = 0;
+    if (rc == FBR_OK) rc = emit_place(p, body, on_device, blocks, totals, &values, &n_values);
+    {
+        // the count pass and the totals are done with; if the count pass failed, the map is born finished with its error
+        // (fbr_result_wait reports it)
         std::lock_guard<std::mutex> g(p->mu);
-        if (totals) pinned_release(p, totals);
+        uint32_t err_code = 0;
+        uint64_t err_task = 0;
         auto it = p->seqs.find(cseq);
         if (it != p->seqs.end()) {
-            free_seq(p, *it->second);
+            SeqState& cs = *it->second;
+            err_code = cs.err_code;
+            err_task = cs.err_task;
+            if (rc != FBR_ETASK) harvest(p, cs);   // as fbr_result_release does (a no-op once the wait succeeded)
+            free_seq(p, cs);
             p->seqs.erase(it);
         }
-        if (with_plan) {
-            SeqState tmp;
-            tmp.emit = std::move(plan);
-            free_seq(p, tmp);
-        }
-    };
-    std::vector<std::pair<int, cudaEvent_t>> scanned;   // (device, event after its block's scan)
-    {
-        std::lock_guard<std::mutex> g(p->mu);
-        auto it = p->seqs.find(cseq);
-        if (it == p->seqs.end()) return fail(FBR_ENOENT, "count pass of an emit map was released");
-        SeqState& cs = *it->second;
+        if (totals) pinned_release(p, totals);
         if (rc == FBR_ETASK) {
-            // the count pass failed: the map is born finished, with the count pass's error (fbr_result_wait reports it)
             std::unique_ptr<SeqState> st(new SeqState());
             st->seq = ++p->next_seq;
             st->n_tasks = d->n_tasks;
@@ -2031,112 +2058,28 @@ static int emit_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_d
             st->result_kind = body.result_kind;
             st->desc = *d;
             st->finished = true;
-            st->err_code = cs.err_code;
-            st->err_task = cs.err_task;
-            free_seq(p, cs);
-            p->seqs.erase(it);
+            st->err_code = err_code;
+            st->err_task = err_task;
             p->stats.tasks_submitted += d->n_tasks;
             *seq_out = st->seq;
             p->seqs[st->seq] = std::move(st);
             return FBR_OK;
         }
-        std::vector<SeqPart*> parts;
-        for (auto& part : cs.parts) parts.push_back(&part);
-        std::sort(parts.begin(), parts.end(), [](const SeqPart* a, const SeqPart* b) { return a->first < b->first; });
-        // one total per block, written by its scan into pinned memory (mapped into every device's address space)
-        rc = pinned_acquire(p, sizeof(uint64_t) * std::max<size_t>(1, parts.size()), (void**)&totals);
-        auto scan_all = [&]() -> int {
-            for (size_t k = 0; k < parts.size() && rc == FBR_OK; ++k) {
-                const SeqPart& part = *parts[k];
-                Worker& w = p->workers[part.worker];
-                const uint64_t tiles = part.count / scan::kTile + 1;
-                if (tiles >= (1ull << 31)) return fail(FBR_EINVAL, "emit map block of %llu tasks is too large to scan", (unsigned long long)part.count);
-                EmitPart e;
-                e.worker = part.worker;
-                e.first = part.first;
-                e.count = part.count;
-                CK(cudaSetDevice(w.device));
-                CK(cudaMallocAsync((void**)&e.d_offs, (part.count + 1) * sizeof(uint64_t), w.s_comp));
-                plan.parts.push_back(e);
-                void* scratch = nullptr;
-                CK(cudaMallocAsync(&scratch, (tiles + 1) * sizeof(uint64_t), w.s_comp));
-                cudaMemsetAsync(scratch, 0, (tiles + 1) * sizeof(uint64_t), w.s_comp);
-                scan_counts_kernel<<<(unsigned)tiles, scan::kThreads, 0, w.s_comp>>>(
-                    (const uint64_t*)part.cx.window_base, part.count, plan.parts.back().d_offs, (unsigned long long*)scratch,
-                    (uint32_t*)((uint64_t*)scratch + tiles), totals + k);
-                const cudaError_t launched = cudaGetLastError();
-                cudaFreeAsync(scratch, w.s_comp);
-                if (launched != cudaSuccess) return fail(FBR_ECUDA, "scan_counts_kernel: %s", cudaGetErrorString(launched));
-                if (!on_device && !whole_block) {
-                    // the host cuts the emit pass's waves from the block's offsets
-                    EmitPart& ep = plan.parts.back();
-                    int r = pinned_acquire(p, (part.count + 1) * sizeof(uint64_t), (void**)&ep.h_offs);
-                    if (r != FBR_OK) return r;
-                    CK(cudaMemcpyAsync(ep.h_offs, ep.d_offs, (part.count + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, w.s_comp));
-                }
-                cudaEvent_t ev;
-                CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-                scanned.push_back({w.device, ev});
-                CK(cudaEventRecord(ev, w.s_comp));
-            }
-            return rc;
-        };
-        rc = scan_all();
     }
-    // one wait per block, outside the pool lock: then every total is in and the blocks' bases are known
-    for (auto& s : scanned) {
-        cudaSetDevice(s.first);
-        if (rc == FBR_OK && cudaEventSynchronize(s.second) != cudaSuccess) rc = fail(FBR_ECUDA, "waiting for scan_counts_kernel failed");
-        cudaEventDestroy(s.second);
-    }
-    if (rc == FBR_OK) {
-        std::lock_guard<std::mutex> g(p->mu);
-        for (size_t k = 0; k < plan.parts.size(); ++k) {
-            EmitPart& e = plan.parts[k];
-            e.total = totals[k];
-            e.base = plan.n_values;
-            plan.n_values += e.total;
-        }
-        auto place = [&]() -> int {
-            if (plan.n_values >= (1ull << 62) / std::max<uint32_t>(1, plan.out_bytes))
-                return fail(FBR_EINVAL, "body %s: the map's count pass gave %llu values, too many to place", body.name.c_str(),
-                            (unsigned long long)plan.n_values);
-            if (!on_device) {
-                int r = pinned_acquire(p, plan.n_values * plan.out_bytes, &plan.values);
-                if (r != FBR_OK) return r;
-                for (EmitPart& e : plan.parts) e.host = (uint8_t*)plan.values + e.base * plan.out_bytes;
-            }
-            if (on_device || whole_block)
-                for (EmitPart& e : plan.parts) {
-                    Worker& w = p->workers[e.worker];
-                    CK(cudaSetDevice(w.device));
-                    CK(cudaMallocAsync(&e.d_values, std::max<uint64_t>(16, e.total * plan.out_bytes), w.s_comp));
-                }
-            return FBR_OK;
-        };
-        rc = place();
-    }
-    if (rc != FBR_OK) {
-        const std::string msg = g_err;
-        drop(true);
-        g_err = msg;
-        return rc;
-    }
-    drop(false);
-    rc = map_submit_plan(p, d, items, seq_out, &plan);
-    if (rc != FBR_OK) {
+    // 4. the emit pass
+    if (rc == FBR_OK) rc = map_submit_pass(p, d, items, seq_out, &blocks, &values, n_values);
+    if (rc != FBR_OK) {   // free what the emit pass did not take over
         const std::string msg = g_err;
         std::lock_guard<std::mutex> g(p->mu);
-        SeqState tmp;
-        tmp.emit = std::move(plan);
-        free_seq(p, tmp);
+        for (SeqPart& b : blocks) free_emit_block(p, b.worker, b.emit);
+        if (values) pinned_release(p, values);
         g_err = msg;
     }
     return rc;
 }
 
-static int map_submit_plan(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out,
-                           EmitPlan* plan) {
+static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out,
+                           std::vector<SeqPart>* counted, void** values, uint64_t n_values) {
     std::lock_guard<std::mutex> g(p->mu);
     if (p->state != ST_RUN) return fail(FBR_ESTATE, "Pool is not running");
     if (!body_of(d->func_id)) return fail(FBR_EINVAL, "bad func_id %d", d->func_id);
@@ -2234,20 +2177,24 @@ static int map_submit_plan(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_ite
         // contiguous task blocks per live worker, cut on claim-unit boundaries (block partition ==
         // PUSH round-robin with chunk = block, SURVEY.md 8(e))
         cut_blocks(p, body, *d, 0, d->n_tasks, live, d->attempt, st->parts);
-        if (plan) {
+        if (counted) {
             // the emit pass runs over the blocks the count pass counted
-            bool same = plan->parts.size() == st->parts.size();
+            bool same = counted->size() == st->parts.size();
             for (size_t k = 0; same && k < st->parts.size(); ++k) {
-                const EmitPart& e = plan->parts[k];
+                const SeqPart& c = (*counted)[k];
                 const SeqPart& part = st->parts[k];
-                same = e.worker == part.worker && e.first == part.first && e.count == part.count;
+                same = c.worker == part.worker && c.first == part.first && c.count == part.count;
             }
             if (!same) {
                 free_seq(p, *st);
                 return fail(FBR_ECUDA, "body %s: the pool's workers changed between the count and the emit pass", body.name.c_str());
             }
-            st->emit = std::move(*plan);
-            *plan = EmitPlan();
+            for (size_t k = 0; k < st->parts.size(); ++k) st->parts[k].emit = (*counted)[k].emit;
+            counted->clear();
+            st->emit_pass = true;
+            st->values = *values;
+            *values = nullptr;
+            st->n_values = n_values;
         }
         if (need_segment && live.size() > 1) {
             // several GPUs fill one segment: bind each worker's block to its GPU's NUMA node
@@ -2527,8 +2474,8 @@ int fbr_result_values(fbr_pool_t* p, uint64_t seq, void** values, uint64_t* n_va
     if (it == p->seqs.end()) return fail(FBR_ENOENT, "unknown seq %llu", (unsigned long long)seq);
     const SeqState& st = *it->second;
     if (!(body_of(st.func_id)->flags & FBR_BODY_EMIT)) return fail(FBR_EINVAL, "seq %llu is not a map of an emit body", (unsigned long long)seq);
-    *values = st.emit.values;
-    *n_values = st.emit.n_values;
+    *values = st.values;
+    *n_values = st.n_values;
     return FBR_OK;
 }
 
@@ -2540,23 +2487,24 @@ int fbr_result_fetch_values(fbr_pool_t* p, uint64_t seq, uint64_t first, uint64_
     SeqState& st = *it->second;
     if (!(body_of(st.func_id)->flags & FBR_BODY_EMIT) || !(st.flags & FBR_RESULTS_ON_DEVICE))
         return fail(FBR_EINVAL, "seq %llu is not an emit map that keeps its results on the device", (unsigned long long)seq);
-    if (first + count > st.emit.n_values || first + count < first) return fail(FBR_EINVAL, "range out of bounds");
-    const uint64_t ob = st.emit.out_bytes;
+    if (first + count > st.n_values || first + count < first) return fail(FBR_EINVAL, "range out of bounds");
+    const uint64_t ob = body_of(st.func_id)->out_bytes;
     for (auto& part : st.parts) {
         CK(cudaSetDevice(p->workers[part.worker].device));
         CK(cudaEventSynchronize(part.done));
     }
-    for (const EmitPart& e : st.emit.parts) {
+    for (auto& part : st.parts) {
+        const EmitBlock& e = part.emit;
         const uint64_t lo = std::max(first, e.base), hi = std::min(first + count, e.base + e.total);
         if (lo >= hi) continue;
-        Worker& w = p->workers[e.worker];
+        Worker& w = p->workers[part.worker];
         CK(cudaSetDevice(w.device));
         CK(cudaMemcpyAsync((uint8_t*)host_dst + (lo - first) * ob, (const uint8_t*)e.d_values + (lo - e.base) * ob, (hi - lo) * ob, cudaMemcpyDeviceToHost, w.s_out));
         p->stats.d2h_bytes += (hi - lo) * ob;
     }
-    for (const EmitPart& e : st.emit.parts) {
-        CK(cudaSetDevice(p->workers[e.worker].device));
-        CK(cudaStreamSynchronize(p->workers[e.worker].s_out));
+    for (auto& part : st.parts) {
+        CK(cudaSetDevice(p->workers[part.worker].device));
+        CK(cudaStreamSynchronize(p->workers[part.worker].s_out));
     }
     return FBR_OK;
 }
