@@ -17,7 +17,7 @@ from . import config  # noqa: F401
 from .config import init, reset  # noqa: F401
 from .queues import Connection, Pipe  # noqa: F401
 from .queues import SimpleQueuePush as _SimpleQueuePush
-from .registry import Ragged, bind, body_names, device_body, device_initializer, register_module  # noqa: F401
+from .registry import Columns, Ragged, bind, body_names, device_body, device_initializer, register_module  # noqa: F401
 
 __version__ = "0.1.0"
 

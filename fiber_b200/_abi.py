@@ -22,6 +22,7 @@ FBR_BODY_INDEX_ARG, FBR_BODY_NEEDS_SHARED, FBR_BODY_SUMMABLE, FBR_BODY_INDEX_ONL
     FBR_BODY_ITEMS = 0x1, 0x2, 0x4, 0x8, 0x10, 0x20, 0x40
 FBR_BODY_EMIT = 0x80
 FBR_BODY_MODULE_ABI = 4
+MAX_ITEM_STREAMS = 4        # item streams of one items body (fbr_map_submit_items_n)
 # pool flags
 FBR_POOL_TIMING, FBR_POOL_OVERLAP = 0x1, 0x2
 # map flags
@@ -36,10 +37,10 @@ FBR_TASK_EMIT = 4
 SYMBOLS = [
     "fbr_abi_version", "fbr_last_error", "fbr_device_count",
     "fbr_body_count", "fbr_body_info", "fbr_body_lookup", "fbr_register_body", "fbr_body_shared_info",
-    "fbr_body_items_info", "fbr_body_emit_info",
+    "fbr_body_items_info", "fbr_body_emit_info", "fbr_body_items_streams",
     "fbr_pool_create", "fbr_pool_close", "fbr_pool_terminate", "fbr_pool_join", "fbr_pool_destroy",
     "fbr_pool_n_workers", "fbr_pool_worker_device",
-    "fbr_map_submit", "fbr_map_submit_items", "fbr_shared_put", "fbr_shared_drop", "fbr_plan_query",
+    "fbr_map_submit", "fbr_map_submit_items", "fbr_map_submit_items_n", "fbr_shared_put", "fbr_shared_drop", "fbr_plan_query",
     "fbr_result_wait", "fbr_result_poll", "fbr_result_data", "fbr_result_fetch", "fbr_result_release",
     "fbr_result_values", "fbr_result_fetch_values",
     "fbr_host_alloc", "fbr_host_free", "fbr_device_alloc", "fbr_device_free",
@@ -150,6 +151,7 @@ def load():
         "fbr_body_shared_info": (i32, [i32, P(u32), P(u32)]),
         "fbr_body_items_info": (i32, [i32, P(u32)]),
         "fbr_body_emit_info": (i32, [i32, P(u32)]),
+        "fbr_body_items_streams": (i32, [i32, P(u32), P(u32)]),
         "fbr_pool_create": (i32, [i32, P(i32), u64, u32, P(vp)]),
         "fbr_pool_close": (i32, [vp]),
         "fbr_pool_terminate": (i32, [vp]),
@@ -159,6 +161,7 @@ def load():
         "fbr_pool_worker_device": (i32, [vp, i32, P(i32)]),
         "fbr_map_submit": (i32, [vp, P(MapDesc), P(u64)]),
         "fbr_map_submit_items": (i32, [vp, P(MapDesc), P(ItemsDesc), P(u64)]),
+        "fbr_map_submit_items_n": (i32, [vp, P(MapDesc), P(ItemsDesc), u32, P(u64)]),
         "fbr_shared_put": (i32, [vp, vp, u64, P(u64)]),
         "fbr_shared_drop": (i32, [vp, u64]),
         "fbr_plan_query": (i32, [i32, u64, u32, u64, i32, i32, i32, P(Plan)]),

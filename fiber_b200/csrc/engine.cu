@@ -170,7 +170,8 @@ struct BodyEntry {
     int max_ctas_per_sm = 0;   // 0 = as many as fit; streaming read+write bodies run best with few, fat streams
     void* module = nullptr;    // dlopen handle of a registered body (never closed: kernels may be in flight)
     uint32_t shared_elem_bytes = 0, shared_stage_bytes = 0;   // FBR_BODY_BROADCAST record bodies
-    uint32_t item_bytes = 0;                                  // FBR_BODY_ITEMS record bodies
+    uint32_t item_streams = 0;                                // FBR_BODY_ITEMS record bodies: 1 to 4 item streams ...
+    uint32_t item_bytes[kMaxItemStreams] = {};                // ... and the element size of each
     uint32_t out_bytes = 0;                                   // FBR_BODY_EMIT record bodies
 };
 
@@ -254,7 +255,7 @@ struct Worker {
     SlotHeader* d_headers = nullptr;   // kRecCapacity
     uint8_t* d_ring = nullptr;         // result ring arena (ring_bytes)
     uint8_t* d_args[2] = {nullptr, nullptr};
-    uint8_t* d_items[2] = {nullptr, nullptr};   // items bodies, host-resident items: a wave's offsets slice, then its item span
+    uint8_t* d_items[2] = {nullptr, nullptr};   // items bodies, host-resident items: each stream's offsets slice, then its item span
     uint8_t* d_vals[2] = {nullptr, nullptr};    // emit bodies, host-resident values: a wave's values before their D2H copy
     uint8_t* d_out[2] = {nullptr, nullptr};
     uint32_t* d_tickets = nullptr;
@@ -290,8 +291,8 @@ struct PartCtx {                          // constants of one worker's block of 
                                           // out-staging halves and PUSHED there by this worker's copy engine (the D2H machinery)
     bool peer_push = false;               // arguments live on worker 0 (another GPU): worker 0's copy engine PUSHES each wave's
                                           // records into this worker's staging halves over NVLink (host_args machinery)
-    bool host_items = false;              // items bodies, host-resident items, not resilient: each wave copies its offsets slice
-                                          // and item span into the worker's d_items staging half
+    bool host_items = false;              // items bodies, host-resident items, not resilient: each wave copies each stream's
+                                          // offsets slice and item span into the worker's d_items staging half
     bool direct = false;                  // contiguous, unshuffled, non-resilient block: the dispatch kernel stores every
                                           // unit at its final index (no ring, no task records, no gather launch)
     const uint8_t* d_shared = nullptr;
@@ -299,10 +300,11 @@ struct PartCtx {                          // constants of one worker's block of 
     const uint8_t* args_full = nullptr;   // device-resident arguments of the whole map (args_dev / resilient)
     uint64_t wave_tasks_cap = 0;
     uint64_t args_limit_bytes = 0;        // host arguments end here (n_items records); 0 = n_tasks * arg_stride
-    // items bodies: where the kernel finds the part's items and offsets for the whole map (WaveParams::items ...)
-    const uint8_t* items = nullptr;
-    const uint64_t* item_offs = nullptr;
-    uint64_t item_first = 0, item_base = 0, item_count = 0;
+    // items bodies: where the kernel finds the part's items and offsets of each stream for the whole map (WaveParams::items
+    // ..., more_items)
+    const uint8_t* items[kMaxItemStreams] = {};
+    const uint64_t* item_offs[kMaxItemStreams] = {};
+    uint64_t item_first = 0, item_base[kMaxItemStreams] = {}, item_count[kMaxItemStreams] = {};
 };
 
 // A worker block of an emit map's emit pass: the part-local exclusive offsets its scan produced (count + 1 of them, the last
@@ -333,8 +335,8 @@ struct SeqPart {
     void* d_shared_tmp = nullptr;         // per-seq device copy of a host shared block
     void* d_window = nullptr;             // FULL_WINDOW device output
     void* d_args_full = nullptr;          // resilient: device copy of all argument records
-    void* d_items = nullptr;              // items bodies with host-resident items: the part's item span ...
-    void* d_item_offs = nullptr;          // ... and its count + 1 offsets, on the device for the part's whole life
+    void* d_items[kMaxItemStreams] = {};      // resilient items bodies with host-resident items: each stream's item span ...
+    void* d_item_offs[kMaxItemStreams] = {};  // ... and its count + 1 offsets, on the device for the part's whole life
     LostUnit* d_lost = nullptr;           // resilient: units whose worker "died" (filled by gather)
     LostUnit* h_lost = nullptr;           // pinned mirror
     uint32_t lost_cap = 0, attempt = 0;
@@ -360,7 +362,8 @@ struct SeqState {
     uint32_t n_waves = 0;
     uint32_t redispatched_units = 0;
     fbr_map_desc_t desc;
-    fbr_items_desc_t items;                // items bodies (fbr_map_submit_items); zero otherwise
+    fbr_items_desc_t items[kMaxItemStreams];   // items bodies (fbr_map_submit_items_n): one per stream; zero otherwise
+    uint32_t n_item_streams = 0;
     std::vector<SeqPart> parts;
     std::vector<SeqPart> graveyard;        // parts that were running on a worker when it died (their blocks were re-dispatched)
     int waiters = 0;                       // threads inside fbr_result_wait for this seq (they hold event handles outside the lock)
@@ -697,6 +700,45 @@ static void shuffle_records(TaskRecord* r, uint32_t n, uint64_t seed) {
 // ------------------------------------------------------------------------------------------------
 // wave pipeline for one worker's block of one map
 // ------------------------------------------------------------------------------------------------
+// A variable-length stream of a block that travels wave by wave through a worker's two ring_bytes staging halves:
+// host-resident items in (d_items: the n item streams of the map share each half), host-staged emit values out (d_vals).
+// In a wave's half the n segments follow one another, each starting on a 256 B boundary: its 256 B-rounded header of
+// wt + 1 offsets (items), then its data.
+struct StagedStream {
+    uint32_t n;                                 // segments sharing a half (1, or the K item streams of an items map)
+    const uint64_t* offs[kMaxItemStreams];      // host offsets rebased to the block: offs[k][t] belongs to task part.first + t
+    uint64_t elem_bytes[kMaxItemStreams];
+    bool header;                // the wave's wt + 1 offsets travel ahead of each segment's data, in a 256 B-rounded header
+    const char* too_large;      // error for a claim unit no half holds: its tasks [t0, t1), its data bytes, ring_bytes
+    uint64_t seg_data(uint32_t k, uint64_t t0, uint64_t t1) const { return (offs[k][t1] - offs[k][t0]) * elem_bytes[k]; }
+    uint64_t data_bytes(uint64_t t0, uint64_t t1) const {
+        uint64_t b = 0;
+        for (uint32_t k = 0; k < n; ++k) b += seg_data(k, t0, t1);
+        return b;
+    }
+    uint64_t header_bytes(uint64_t t0, uint64_t t1) const { return header ? round_up((t1 - t0 + 1) * sizeof(uint64_t), 256) : 0; }
+    // where segment k of the wave of tasks [t0, t1) starts in its half
+    uint64_t seg_start(uint32_t k, uint64_t t0, uint64_t t1) const {
+        uint64_t at = 0;
+        for (uint32_t j = 0; j < k; ++j) at = round_up(at + header_bytes(t0, t1) + seg_data(j, t0, t1), 256);
+        return at;
+    }
+    // what tasks [t0, t1) of the block take of a staging half
+    uint64_t staged_bytes(uint64_t t0, uint64_t t1) const { return seg_start(n - 1, t0, t1) + header_bytes(t0, t1) + seg_data(n - 1, t0, t1); }
+};
+
+// the host-resident item streams of block `part` of an items map, as they are staged
+static StagedStream staged_items(const SeqState& st, const SeqPart& part) {
+    StagedStream s{st.n_item_streams, {}, {}, true,
+                   "the claim unit of tasks [%llu, %llu) carries %llu item bytes, more than a staging half of "
+                   "ring_bytes %llu holds with its offsets: raise ring_bytes or split the items"};
+    for (uint32_t k = 0; k < s.n; ++k) {
+        s.offs[k] = st.items[k].offsets + part.first;
+        s.elem_bytes[k] = st.items[k].item_bytes;
+    }
+    return s;
+}
+
 // One wave: `n_units` claim units -> copy-in, dispatch, gather, (streaming parts) copy-out.
 // `wave_first`/`wt` describe the contiguous task window of a regular wave; a re-dispatch wave
 // (arbitrary lost units) passes contiguous=false.  `have_records`: the caller wrote the wave's task
@@ -763,21 +805,31 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
         }
         wave_args = w.d_args[half];
     }
-    // items of a streaming wave: its wt + 1 offsets at the start of the staging half, its item span 256 B further on
-    const uint8_t* wave_items = cx.items;
-    const uint64_t* wave_offs = cx.item_offs;
-    uint64_t item_first = cx.item_first, item_base = cx.item_base, item_count = cx.item_count;
+    // items of a streaming wave, stream by stream in the staging half (StagedStream): its wt + 1 offsets, then its item span
+    // one 256 B-rounded header further on
+    const uint8_t* wave_items[kMaxItemStreams];
+    const uint64_t* wave_offs[kMaxItemStreams];
+    uint64_t item_first = cx.item_first, item_base[kMaxItemStreams], item_count[kMaxItemStreams];
+    for (uint32_t k = 0; k < kMaxItemStreams; ++k) {
+        wave_items[k] = cx.items[k]; wave_offs[k] = cx.item_offs[k]; item_base[k] = cx.item_base[k]; item_count[k] = cx.item_count[k];
+    }
     if (cx.host_items) {
-        const fbr_items_desc_t& it = st.items;
-        const uint64_t lo = it.offsets[wave_first], hi = it.offsets[wave_first + wt];
-        const uint64_t obytes = (wt + 1) * sizeof(uint64_t), ioff = round_up(obytes, 256), ibytes = (hi - lo) * it.item_bytes;
-        CK(cudaMemcpyAsync(w.d_items[half], it.offsets + wave_first, obytes, cudaMemcpyHostToDevice, w.s_in));
-        if (ibytes)
-            CK(cudaMemcpyAsync(w.d_items[half] + ioff, (const uint8_t*)it.items + lo * it.item_bytes, ibytes, cudaMemcpyHostToDevice, w.s_in));
-        STAT_ADD(p, h2d_bytes, obytes + ibytes);
-        wave_offs = (const uint64_t*)w.d_items[half];
-        wave_items = w.d_items[half] + ioff;
-        item_first = wave_first; item_base = lo; item_count = hi;
+        const StagedStream s = staged_items(st, part);
+        const uint64_t t0 = wave_first - part.first, t1 = t0 + wt;
+        const uint64_t obytes = (wt + 1) * sizeof(uint64_t), hbytes = s.header_bytes(t0, t1);
+        for (uint32_t k = 0; k < s.n; ++k) {
+            const fbr_items_desc_t& it = st.items[k];
+            const uint64_t lo = it.offsets[wave_first], hi = it.offsets[wave_first + wt];
+            const uint64_t at = s.seg_start(k, t0, t1), ibytes = s.seg_data(k, t0, t1);
+            CK(cudaMemcpyAsync(w.d_items[half] + at, it.offsets + wave_first, obytes, cudaMemcpyHostToDevice, w.s_in));
+            if (ibytes)
+                CK(cudaMemcpyAsync(w.d_items[half] + at + hbytes, (const uint8_t*)it.items + lo * it.item_bytes, ibytes, cudaMemcpyHostToDevice, w.s_in));
+            STAT_ADD(p, h2d_bytes, obytes + ibytes);
+            wave_offs[k] = (const uint64_t*)(w.d_items[half] + at);
+            wave_items[k] = w.d_items[half] + at + hbytes;
+            item_base[k] = lo; item_count[k] = hi;
+        }
+        item_first = wave_first;
     }
     if (in_copies) CK(cudaEventRecord(w.ev_rec_h2d[rw], w.s_in));
 
@@ -828,11 +880,12 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
     wp.syn_func = (uint32_t)st.func_id;
     wp.syn_attempt = part.attempt;
     wp.n_items = d.n_items ? d.n_items : ~0ull;
-    wp.items = wave_items;
-    wp.item_offs = wave_offs;
+    wp.items = wave_items[0];
+    wp.item_offs = wave_offs[0];
     wp.item_first = item_first;
-    wp.item_base = item_base;
-    wp.item_count = item_count;
+    wp.item_base = item_base[0];
+    wp.item_count = item_count[0];
+    for (uint32_t k = 1; k < st.n_item_streams; ++k) wp.more_items[k - 1] = ItemStream{wave_items[k], wave_offs[k], item_base[k], item_count[k]};
     const EmitBlock& emit = part.emit;
     uint64_t v_lo = 0, v_hi = 0;            // staged emit waves: the wave's span of the block's values
     if (emit.d_offs) {
@@ -1007,20 +1060,6 @@ static int finish_round(fbr_pool* p, SeqState& st, SeqPart& part, bool copy_wind
     return FBR_OK;
 }
 
-// A variable-length stream of a block that travels wave by wave through a worker's two ring_bytes staging halves:
-// host-resident items in (d_items), host-staged emit values out (d_vals).
-struct StagedStream {
-    const uint64_t* offs;       // host offsets rebased to the block: offs[t] belongs to task part.first + t
-    uint64_t elem_bytes;
-    bool header;                // the wave's wt + 1 offsets travel ahead of its data, in a 256 B-rounded header
-    const char* too_large;      // error for a claim unit no half holds: its tasks [t0, t1), its data bytes, ring_bytes
-    uint64_t data_bytes(uint64_t t0, uint64_t t1) const { return (offs[t1] - offs[t0]) * elem_bytes; }
-    // what tasks [t0, t1) of the block take of a staging half
-    uint64_t staged_bytes(uint64_t t0, uint64_t t1) const {
-        return (header ? round_up((t1 - t0 + 1) * sizeof(uint64_t), 256) : 0) + data_bytes(t0, t1);
-    }
-};
-
 static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& body) {
     Worker& w = p->workers[part.worker];
     const fbr_map_desc_t& d = st.desc;
@@ -1132,26 +1171,33 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
     // wave by wave through the worker's d_items staging halves (run_wave); a resilient map may re-dispatch any unit at
     // any time, so it copies its part's whole item span and count + 1 offsets to the device once, like d_args_full
     if (body.flags & FBR_BODY_ITEMS) {
-        const fbr_items_desc_t& it = st.items;
         if (cx.args_dev) {
-            cx.items = (const uint8_t*)it.items;
-            cx.item_offs = it.offsets;
-            cx.item_first = 0; cx.item_base = 0; cx.item_count = it.n_items;
+            for (uint32_t k = 0; k < st.n_item_streams; ++k) {
+                const fbr_items_desc_t& it = st.items[k];
+                cx.items[k] = (const uint8_t*)it.items;
+                cx.item_offs[k] = it.offsets;
+                cx.item_base[k] = 0; cx.item_count[k] = it.n_items;
+            }
+            cx.item_first = 0;
         } else if (!cx.resilient) {
             cx.host_items = true;
             for (int i = 0; i < 2; ++i)
                 if (!w.d_items[i]) CK(cudaMalloc((void**)&w.d_items[i], p->ring_bytes));
         } else {
-            const uint64_t lo = it.offsets[part.first], hi = it.offsets[part.first + part.count];
-            const uint64_t ibytes = (hi - lo) * it.item_bytes, obytes = (part.count + 1) * sizeof(uint64_t);
-            CK(cudaMallocAsync(&part.d_items, std::max<uint64_t>(16, ibytes), w.s_in));
-            CK(cudaMallocAsync(&part.d_item_offs, obytes, w.s_in));
-            if (ibytes) CK(cudaMemcpyAsync(part.d_items, (const uint8_t*)it.items + lo * it.item_bytes, ibytes, cudaMemcpyHostToDevice, w.s_in));
-            CK(cudaMemcpyAsync(part.d_item_offs, it.offsets + part.first, obytes, cudaMemcpyHostToDevice, w.s_in));
-            STAT_ADD(p, h2d_bytes, ibytes + obytes);
-            cx.items = (const uint8_t*)part.d_items;
-            cx.item_offs = (const uint64_t*)part.d_item_offs;
-            cx.item_first = part.first; cx.item_base = lo; cx.item_count = hi;
+            for (uint32_t k = 0; k < st.n_item_streams; ++k) {
+                const fbr_items_desc_t& it = st.items[k];
+                const uint64_t lo = it.offsets[part.first], hi = it.offsets[part.first + part.count];
+                const uint64_t ibytes = (hi - lo) * it.item_bytes, obytes = (part.count + 1) * sizeof(uint64_t);
+                CK(cudaMallocAsync(&part.d_items[k], std::max<uint64_t>(16, ibytes), w.s_in));
+                CK(cudaMallocAsync(&part.d_item_offs[k], obytes, w.s_in));
+                if (ibytes) CK(cudaMemcpyAsync(part.d_items[k], (const uint8_t*)it.items + lo * it.item_bytes, ibytes, cudaMemcpyHostToDevice, w.s_in));
+                CK(cudaMemcpyAsync(part.d_item_offs[k], it.offsets + part.first, obytes, cudaMemcpyHostToDevice, w.s_in));
+                STAT_ADD(p, h2d_bytes, ibytes + obytes);
+                cx.items[k] = (const uint8_t*)part.d_items[k];
+                cx.item_offs[k] = (const uint64_t*)part.d_item_offs[k];
+                cx.item_base[k] = lo; cx.item_count[k] = hi;
+            }
+            cx.item_first = part.first;
         }
     }
 
@@ -1181,9 +1227,10 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
     // wave w overlaps the kernels of wave w+1 instead of trailing one monolithic launch.
     if (!cx.full_window || cx.host_args || cx.host_items) {
         uint64_t bytes_per_task = std::max<uint64_t>(R, cx.host_args ? d.arg_stride : 0);
-        if (cx.host_items && part.count) {
-            const uint64_t mean = (st.items.offsets[part.first + part.count] - st.items.offsets[part.first]) * st.items.item_bytes / part.count;
-            bytes_per_task = std::max<uint64_t>(bytes_per_task, mean + sizeof(uint64_t));
+        if (cx.host_items && part.count) {   // the mean item bytes and offsets of a task, over every stream
+            const StagedStream s = staged_items(st, part);
+            const uint64_t mean = s.data_bytes(0, part.count) / part.count;
+            bytes_per_task = std::max<uint64_t>(bytes_per_task, mean + s.n * sizeof(uint64_t));
         }
         // a wave must carry enough kernel time to hide its launches: 8 MiB of byte results is tens of us of
         // pi dispatch; a byte of bit-packed results stands for 8 tasks, so 1 MiB is the same work
@@ -1231,12 +1278,9 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
 
     // before any wave launches: every claim unit of every staged stream must fit one staging half
     std::vector<StagedStream> streams;
-    if (cx.host_items)
-        streams.push_back({st.items.offsets + part.first, st.items.item_bytes, true,
-                           "the claim unit of tasks [%llu, %llu) carries %llu item bytes, more than a staging half of "
-                           "ring_bytes %llu holds with its offsets: raise ring_bytes or split the items"});
+    if (cx.host_items) streams.push_back(staged_items(st, part));
     if (part.emit.h_offs)
-        streams.push_back({part.emit.h_offs, body.out_bytes, false,
+        streams.push_back({1, {part.emit.h_offs}, {body.out_bytes}, false,
                            "the claim unit of tasks [%llu, %llu) emits %llu value bytes, more than a staging half of "
                            "ring_bytes %llu holds: raise ring_bytes or use results=\"device\""});
     for (const StagedStream& s : streams)
@@ -1482,8 +1526,10 @@ static void free_seq(fbr_pool* p, SeqState& st) {
         if (part.d_shared_tmp) cudaFreeAsync(part.d_shared_tmp, w.s_in);
         if (part.d_window) cudaFreeAsync(part.d_window, w.s_in);
         if (part.d_args_full) cudaFreeAsync(part.d_args_full, w.s_in);
-        if (part.d_items) cudaFreeAsync(part.d_items, w.s_in);
-        if (part.d_item_offs) cudaFreeAsync(part.d_item_offs, w.s_in);
+        for (uint32_t k = 0; k < kMaxItemStreams; ++k) {
+            if (part.d_items[k]) cudaFreeAsync(part.d_items[k], w.s_in);
+            if (part.d_item_offs[k]) cudaFreeAsync(part.d_item_offs[k], w.s_in);
+        }
         if (part.d_lost) cudaFreeAsync(part.d_lost, w.s_in);
         free_emit_block(p, part.worker, part.emit);
         if (part.h_lost) cudaFreeHost(part.h_lost);
@@ -1568,7 +1614,15 @@ int fbr_body_shared_info(int func_id, uint32_t* elem_bytes, uint32_t* stage_byte
 int fbr_body_items_info(int func_id, uint32_t* item_bytes) {
     const BodyEntry* bp = body_of(func_id);
     if (!item_bytes || !bp) return fail(FBR_EINVAL, "bad func_id %d", func_id);
-    *item_bytes = bp->item_bytes;
+    *item_bytes = bp->item_bytes[0];
+    return FBR_OK;
+}
+
+int fbr_body_items_streams(int func_id, uint32_t* n_streams, uint32_t item_bytes[4]) {
+    const BodyEntry* bp = body_of(func_id);
+    if (!n_streams || !item_bytes || !bp) return fail(FBR_EINVAL, "bad func_id %d", func_id);
+    *n_streams = bp->item_streams;
+    for (uint32_t k = 0; k < kMaxItemStreams; ++k) item_bytes[k] = bp->item_bytes[k];
     return FBR_OK;
 }
 
@@ -1604,6 +1658,15 @@ static std::string descriptor_error(const fbr_body_module_t* m, const char* modu
     else if (items && !is_record) why = "only record bodies take items (FBR_BODY_ITEMS)";
     else if (items && !record::item_elem_ok(m->item_bytes)) why = "the item size must be 1, 2 or a multiple of 4 up to 4096 bytes";
     else if (items && (m->flags & FBR_BODY_INDEX_ARG)) why = "an items body cannot take range() indices (FBR_BODY_INDEX_ARG)";
+    else if (m->item_streams > kMaxItemStreams) why = "takes at most 4 item streams (item_streams)";
+    else if (!items && m->item_streams > 1) why = "describes several item streams but lacks FBR_BODY_ITEMS";
+    for (uint32_t k = 1; k < kMaxItemStreams && !why; ++k) {
+        const uint32_t e = m->more_item_bytes[k - 1];
+        if (k < m->item_streams && !record::item_elem_ok(e))
+            why = "the item size of every stream must be 1, 2 or a multiple of 4 up to 4096 bytes";
+        else if (k >= m->item_streams && e)
+            why = "describes the item size of a stream past its item_streams";
+    }
     const bool emit = (m->flags & FBR_BODY_EMIT) != 0;
     if (why) {
     } else if (!emit && m->out_bytes) {
@@ -1682,7 +1745,9 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
     b.arg_bytes = m->arg_bytes; b.result_bytes = m->result_bytes; b.result_kind = m->result_kind;
     b.flags = m->flags; b.unit_tasks = m->unit_tasks;
     b.shared_elem_bytes = m->shared_elem_bytes; b.shared_stage_bytes = m->shared_stage_bytes;
-    b.item_bytes = m->item_bytes;
+    b.item_streams = (m->flags & FBR_BODY_ITEMS) ? std::max<uint32_t>(1, m->item_streams) : 0;
+    b.item_bytes[0] = m->item_bytes;
+    for (uint32_t k = 1; k < b.item_streams; ++k) b.item_bytes[k] = m->more_item_bytes[k - 1];
     b.out_bytes = m->out_bytes;
     b.launch = m->launch; b.occupancy = m->occupancy;
     b.module = h;
@@ -1861,33 +1926,58 @@ int fbr_shared_drop(fbr_pool_t* p, uint64_t handle) {
     return FBR_OK;
 }
 
-static int map_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out);
+static int map_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint32_t n_streams, uint64_t* seq_out);
 
 int fbr_map_submit(fbr_pool_t* p, const fbr_map_desc_t* d, uint64_t* seq_out) {
     if (!p || !d || !seq_out) return fail(FBR_EINVAL, "NULL argument");
     const BodyEntry* b = body_of(d->func_id);
     if (b && (b->flags & FBR_BODY_ITEMS))
         return fail(FBR_EINVAL, "body %s takes items: submit its maps with fbr_map_submit_items", b->name.c_str());
-    return map_submit(p, d, nullptr, seq_out);
+    return map_submit(p, d, nullptr, 0, seq_out);
 }
 
 int fbr_map_submit_items(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* it, uint64_t* seq_out) {
-    if (!p || !d || !it || !seq_out) return fail(FBR_EINVAL, "NULL argument");
+    return fbr_map_submit_items_n(p, d, it, 1, seq_out);
+}
+
+int fbr_map_submit_items_n(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* streams, uint32_t n_streams, uint64_t* seq_out) {
+    if (!p || !d || !streams || !seq_out) return fail(FBR_EINVAL, "NULL argument");
     const BodyEntry* b = body_of(d->func_id);
     if (!b) return fail(FBR_EINVAL, "bad func_id %d", d->func_id);
     if (!(b->flags & FBR_BODY_ITEMS))
         return fail(FBR_EINVAL, "body %s takes no items: submit its maps with fbr_map_submit", b->name.c_str());
-    if (it->item_bytes != b->item_bytes)
-        return fail(FBR_EINVAL, "item_bytes %u does not match body %s (%u)", it->item_bytes, b->name.c_str(), b->item_bytes);
-    if (d->n_tasks && !it->offsets) return fail(FBR_EINVAL, "offsets is NULL");
-    if (it->n_items && !it->items) return fail(FBR_EINVAL, "items is NULL");
+    if (n_streams != b->item_streams)
+        return fail(FBR_EINVAL, "body %s takes %u item stream%s, not %u%s", b->name.c_str(), b->item_streams,
+                    b->item_streams == 1 ? "" : "s", n_streams, n_streams == 1 ? " (fbr_map_submit_items_n submits several)" : "");
+    for (uint32_t k = 0; k < n_streams; ++k) {
+        const fbr_items_desc_t* it = &streams[k];
+        // one-stream maps keep their messages; a multi-stream map's name the stream
+        const std::string sk = n_streams > 1 ? strf("stream %u: ", k) : std::string();
+        const char* sp = sk.c_str();
+        if (it->item_bytes != b->item_bytes[k])
+            return fail(FBR_EINVAL, "%sitem_bytes %u does not match body %s (%u)", sp, it->item_bytes, b->name.c_str(), b->item_bytes[k]);
+        if (d->n_tasks && !it->offsets) return fail(FBR_EINVAL, "%soffsets is NULL", sp);
+        if (it->n_items && !it->items) return fail(FBR_EINVAL, "%sitems is NULL", sp);
+        if (d->flags & FBR_ARGS_DEVICE) {
+            // a body may load its items as vectors as wide as the largest power of two dividing item_bytes, up to 16 B (a double,
+            // a 16 B struct); this is the alignment required, which can be stricter than alignof(Item) (four floats: 16, not 4)
+            const uint32_t e = it->item_bytes, align = std::min<uint32_t>(16u, e & (~e + 1u));
+            if ((uintptr_t)it->items % align)
+                return fail(FBR_EINVAL, "%sdevice-resident items of body %s must be %u-byte aligned", sp, b->name.c_str(), align);
+            if ((uintptr_t)it->offsets % 8) return fail(FBR_EINVAL, "%sdevice-resident offsets must be 8-byte aligned", sp);
+        } else if (d->n_tasks) {
+            // the kernel trusts host-resident offsets: check them before anything launches
+            const uint64_t* o = it->offsets;
+            for (uint64_t j = 0; j < d->n_tasks; ++j)
+                if (o[j] > o[j + 1])
+                    return fail(FBR_EINVAL, "%soffsets decrease at task %llu (%llu > %llu)", sp, (unsigned long long)j,
+                                (unsigned long long)o[j], (unsigned long long)o[j + 1]);
+            if (o[d->n_tasks] > it->n_items)
+                return fail(FBR_EINVAL, "%soffsets[%llu] = %llu is past n_items %llu", sp, (unsigned long long)d->n_tasks,
+                            (unsigned long long)o[d->n_tasks], (unsigned long long)it->n_items);
+        }
+    }
     if (d->flags & FBR_ARGS_DEVICE) {
-        // a body may load its items as vectors as wide as the largest power of two dividing item_bytes, up to 16 B (a double,
-        // a 16 B struct); this is the alignment required, which can be stricter than alignof(Item) (four floats: 16, not 4)
-        const uint32_t e = it->item_bytes, align = std::min<uint32_t>(16u, e & (~e + 1u));
-        if ((uintptr_t)it->items % align)
-            return fail(FBR_EINVAL, "device-resident items of body %s must be %u-byte aligned", b->name.c_str(), align);
-        if ((uintptr_t)it->offsets % 8) return fail(FBR_EINVAL, "device-resident offsets must be 8-byte aligned");
         int nw = 0;
         {
             std::lock_guard<std::mutex> g(p->mu);
@@ -1895,31 +1985,21 @@ int fbr_map_submit_items(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items
         }
         if (nw != 1)
             return fail(FBR_EINVAL, "device-resident items (FBR_ARGS_DEVICE) need a one-worker pool; this pool has %d workers", nw);
-    } else if (d->n_tasks) {
-        // the kernel trusts host-resident offsets: check them before anything launches
-        const uint64_t* o = it->offsets;
-        for (uint64_t j = 0; j < d->n_tasks; ++j)
-            if (o[j] > o[j + 1])
-                return fail(FBR_EINVAL, "offsets decrease at task %llu (%llu > %llu)", (unsigned long long)j,
-                            (unsigned long long)o[j], (unsigned long long)o[j + 1]);
-        if (o[d->n_tasks] > it->n_items)
-            return fail(FBR_EINVAL, "offsets[%llu] = %llu is past n_items %llu", (unsigned long long)d->n_tasks,
-                        (unsigned long long)o[d->n_tasks], (unsigned long long)it->n_items);
     }
-    return map_submit(p, d, it, seq_out);
+    return map_submit(p, d, streams, n_streams, seq_out);
 }
 
 // Submits one map.  The emit pass of an emit map passes `counted`, the count pass's blocks with their emit state, and
 // `values`, the pinned values segment of n_values values: it runs over exactly those blocks and takes both over.
-static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out,
+static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint32_t n_streams, uint64_t* seq_out,
                            std::vector<SeqPart>* counted = nullptr, void** values = nullptr, uint64_t n_values = 0);
-static int emit_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out);
+static int emit_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint32_t n_streams, uint64_t* seq_out);
 static void harvest(fbr_pool* p, SeqState& st);
 
-static int map_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out) {
+static int map_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint32_t n_streams, uint64_t* seq_out) {
     const BodyEntry* b = body_of(d->func_id);
-    if (b && (b->flags & FBR_BODY_EMIT)) return emit_submit(p, d, items, seq_out);
-    return map_submit_pass(p, d, items, seq_out);
+    if (b && (b->flags & FBR_BODY_EMIT)) return emit_submit(p, d, items, n_streams, seq_out);
+    return map_submit_pass(p, d, items, n_streams, seq_out);
 }
 
 // Emit map, step 2: scan_counts_kernel turns each block of the count pass `cseq` into an entry of `blocks` (task order)
@@ -2004,7 +2084,7 @@ static int emit_place(fbr_pool_t* p, const BodyEntry& body, bool on_device, std:
 // An emit map: the count pass is an ordinary map of the body whose records (the tasks' counts) stay on the device; once it
 // is done, scan_counts_kernel turns each block's counts into its offsets and total, the host sizes the values segment from
 // the totals, and the emit pass runs as a second ordinary map over the same blocks.
-static int emit_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out) {
+static int emit_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint32_t n_streams, uint64_t* seq_out) {
     const BodyEntry& body = *body_of(d->func_id);
     if (d->out || (d->flags & FBR_OUT_DEVICE))
         return fail(FBR_EINVAL, "body %s emits variable-length results: its maps own their output (no out, no FBR_OUT_DEVICE)", body.name.c_str());
@@ -2014,7 +2094,7 @@ static int emit_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_d
     fbr_map_desc_t cd = *d;
     cd.flags |= FBR_RESULTS_ON_DEVICE;
     uint64_t cseq = 0;
-    int rc = map_submit_pass(p, &cd, items, &cseq);
+    int rc = map_submit_pass(p, &cd, items, n_streams, &cseq);
     if (rc != FBR_OK) return rc;
     fbr_result_t cres;
     rc = fbr_result_wait(p, cseq, -1, &cres);
@@ -2067,7 +2147,7 @@ static int emit_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_d
         }
     }
     // 4. the emit pass
-    if (rc == FBR_OK) rc = map_submit_pass(p, d, items, seq_out, &blocks, &values, n_values);
+    if (rc == FBR_OK) rc = map_submit_pass(p, d, items, n_streams, seq_out, &blocks, &values, n_values);
     if (rc != FBR_OK) {   // free what the emit pass did not take over
         const std::string msg = g_err;
         std::lock_guard<std::mutex> g(p->mu);
@@ -2078,7 +2158,7 @@ static int emit_submit(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_d
     return rc;
 }
 
-static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint64_t* seq_out,
+static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_items_desc_t* items, uint32_t n_streams, uint64_t* seq_out,
                            std::vector<SeqPart>* counted, void** values, uint64_t n_values) {
     std::lock_guard<std::mutex> g(p->mu);
     if (p->state != ST_RUN) return fail(FBR_ESTATE, "Pool is not running");
@@ -2152,8 +2232,9 @@ static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_ite
         st->result_kind = body.result_kind;
         st->out = d->out;
         st->desc = *d;
-        if (items) st->items = *items;
-        else memset(&st->items, 0, sizeof st->items);
+        memset(st->items, 0, sizeof st->items);
+        st->n_item_streams = items ? n_streams : 0;
+        for (uint32_t k = 0; k < st->n_item_streams; ++k) st->items[k] = items[k];
         const bool need_segment = !st->out && d->n_tasks && !(d->flags & FBR_RESULTS_ON_DEVICE);
         // host allocations fail with the sticky error too once a context of this process has died: tell the two apart
         auto died_meanwhile = [&]() {

@@ -18,6 +18,7 @@
 #include <string.h>
 
 #include <type_traits>
+#include <utility>
 
 #include "bodies.cuh"
 
@@ -48,6 +49,16 @@ struct SlotHeader {
 };
 static_assert(sizeof(SlotHeader) == 16, "slot header layout is part of the ABI");
 constexpr uint32_t kUnitLost = 0x80000000u;
+
+// Item stream k >= 1 of a multi-stream items record body (stream 0 lives in WaveParams::items ...): the same fields, with
+// the map index of offs[0] shared with stream 0 (item_first), since every stream is cut at the same tasks
+struct ItemStream {
+    const uint8_t* items;
+    const uint64_t* offs;
+    uint64_t base;              // item index of items[0]
+    uint64_t count;             // offsets end here (the stream's n_items)
+};
+constexpr uint32_t kMaxItemStreams = 4;
 
 struct WaveParams {
     const TaskRecord* records;  // device task ring window of this wave; nullptr: the wave is a contiguous,
@@ -95,6 +106,9 @@ struct WaveParams {
     const uint64_t* emit_offs;
     uint64_t emit_first;
     uint64_t emit_base;
+    // items record bodies with K = 2 to 4 streams (Items = ItemTypes<...>): streams 1 .. K-1, read like stream 0 above.
+    // Appended after every other field, so their offsets stay where one-stream kernels expect them
+    ItemStream more_items[kMaxItemStreams - 1];
 };
 
 // Task record of ticket t: from the device task ring, or computed (contiguous wave).
@@ -966,6 +980,10 @@ struct Items {
     uint64_t n;
 };
 
+// The element types of a multi-stream items record body, one per stream: `using Items = fbr::ItemTypes<uint8_t, float>;`
+template <class... T>
+struct ItemTypes {};
+
 // The Arg of an items record body without a fixed head record: run() then takes no argument record.
 struct NoArg {};
 
@@ -1048,21 +1066,65 @@ struct GroupOf<B, std::void_t<decltype(B::kGroup)>> {
     static_assert(kG == 2 || kG == 4 || kG == 8 || kG == 16 || kG == 32, "group record bodies: kGroup is 2, 4, 8, 16 or 32");
 };
 
-// A record body opts into variable-length items with `using Item = <element>;`: run() then takes a const Items<Item>&
-// after the argument record (or first, when Arg is NoArg).
+// A record body opts into variable-length items with `using Item = <element>;` (one stream) or `using Items =
+// fbr::ItemTypes<T0, T1[, T2[, T3]]>;` (2 to 4 streams, each with its own element type and offsets): run() then takes a
+// const Items<Tk>& per stream, in stream order, after the argument record (or first, when Arg is NoArg).  ItemsOf<B> is
+// the one place the streams' element types and sizes are defined.
+template <uint32_t k, class... T>
+struct TypeAt;
+template <uint32_t k, class T0, class... T>
+struct TypeAt<k, T0, T...> {
+    using type = typename TypeAt<k - 1, T...>::type;
+};
+template <class T0, class... T>
+struct TypeAt<0, T0, T...> {
+    using type = T0;
+};
 template <class B, class = void>
-struct ItemsOf {
+struct ItemDecl {                       // using Item = T: ItemTypes<T>
     static constexpr bool kOn = false;
-    static constexpr uint32_t kElem = 0;
+    using type = ItemTypes<>;
 };
 template <class B>
-struct ItemsOf<B, std::void_t<typename B::Item>> {
-    using T = typename B::Item;
+struct ItemDecl<B, std::void_t<typename B::Item>> {
     static constexpr bool kOn = true;
-    static constexpr uint32_t kElem = (uint32_t)sizeof(T);
-    static_assert(std::is_trivially_copyable<T>::value, "items bodies: Item is trivially copyable");
-    static_assert(item_elem_ok(kElem), "items bodies: sizeof(Item) is 1, 2 or a multiple of 4 up to 4096");
-    static_assert(!B::kIndexArg, "items bodies cannot take range() indices (kIndexArg)");
+    using type = ItemTypes<typename B::Item>;
+};
+template <class B, class = void>
+struct ItemsDecl {                      // using Items = ItemTypes<...>
+    static constexpr bool kOn = false;
+    using type = ItemTypes<>;
+};
+template <class B>
+struct ItemsDecl<B, std::void_t<typename B::Items>> {
+    static constexpr bool kOn = true;
+    using type = typename B::Items;
+};
+template <class L>
+struct ItemList;
+template <class... T>
+struct ItemList<ItemTypes<T...>> {
+    static constexpr uint32_t kStreams = (uint32_t)sizeof...(T);
+    template <uint32_t k>
+    using At = typename TypeAt<k, T...>::type;
+    // element size of stream k < kMaxItemStreams (0 past the last stream)
+    static constexpr uint32_t elem(uint32_t k) {
+        constexpr uint32_t e[kMaxItemStreams + 1] = {(uint32_t)sizeof(T)...};
+        return e[k];
+    }
+    static_assert((true && ... && std::is_trivially_copyable<T>::value), "items bodies: Item is trivially copyable");
+    static_assert((true && ... && item_elem_ok((uint32_t)sizeof(T))), "items bodies: sizeof(Item) is 1, 2 or a multiple of 4 up to 4096");
+};
+template <class B>
+struct ItemsOf : ItemList<typename std::conditional<ItemsDecl<B>::kOn, typename ItemsDecl<B>::type, typename ItemDecl<B>::type>::type> {
+    using List = ItemList<typename std::conditional<ItemsDecl<B>::kOn, typename ItemsDecl<B>::type, typename ItemDecl<B>::type>::type>;
+    static constexpr bool kOn = List::kStreams > 0;
+    static constexpr uint32_t kElem = List::elem(0);   // stream 0
+    static_assert(!(ItemDecl<B>::kOn && ItemsDecl<B>::kOn),
+                  "items bodies declare `using Item = T;` (one stream) or `using Items = fbr::ItemTypes<...>;` (2 to 4), not both");
+    static_assert(!ItemsDecl<B>::kOn || (List::kStreams >= 2 && List::kStreams <= kMaxItemStreams),
+                  "items bodies: fbr::ItemTypes<...> lists 2 to 4 element types (one stream: `using Item = T;`)");
+    static_assert(!kOn || !B::kIndexArg, "items bodies cannot take range() indices (kIndexArg)");
 };
 
 // A record body opts into variable-length results with `using Out = <element>;` and `using Res = NoRes;`: run() then takes
@@ -1169,11 +1231,51 @@ __device__ __forceinline__ Group<G> group_of(uint32_t ct) {
     return Group<G>{ct % G, (G == 32 ? 0xffffffffu : ((1u << G) - 1u) << ((ct & 31u) & ~(G - 1u)))};
 }
 
+// Stream k of an items map's wave: stream 0 from WaveParams::items ..., the others from more_items
+template <uint32_t k>
+__device__ __forceinline__ ItemStream item_stream(const WaveParams& wp) {
+    if constexpr (k == 0) return ItemStream{wp.items, wp.item_offs, wp.item_base, wp.item_count};
+    else return wp.more_items[k - 1];
+}
+
+// The item streams of a unit of an items body: o[k] are stream k's offsets from the unit's first task on
+template <uint32_t K>
+struct UnitItems {
+    const uint64_t* o[K];
+};
+template <size_t... k>
+__device__ __forceinline__ UnitItems<sizeof...(k)> unit_items(const WaveParams& wp, uint64_t first, std::index_sequence<k...>) {
+    return UnitItems<sizeof...(k)>{{(item_stream<k>(wp).offs + (first - wp.item_first))...}};
+}
+// Task i's span [a[k], b[k]) in each stream k, read from the unit's offsets; true (a bad argument) when any stream's
+// offsets decrease or leave [base, count]
+template <uint32_t K>
+struct TaskSpans {
+    uint64_t a[K], b[K];
+};
+template <size_t... k>
+__device__ __forceinline__ bool bad_spans(const WaveParams& wp, const UnitItems<sizeof...(k)>& u, uint32_t i, std::index_sequence<k...>,
+                                           TaskSpans<sizeof...(k)>& t) {
+    bool bad = false;
+    ((t.a[k] = u.o[k][i], t.b[k] = u.o[k][i + 1],
+      bad = bad || t.a[k] > t.b[k] || t.a[k] < item_stream<k>(wp).base || t.b[k] > item_stream<k>(wp).count), ...);
+    return bad;
+}
+// f(the K views of task spans t, in stream order)
+template <class B, class F, size_t... k>
+__device__ __forceinline__ void with_items(const WaveParams& wp, const TaskSpans<sizeof...(k)>& t, std::index_sequence<k...>, F&& f) {
+    using It = ItemsOf<B>;
+    f(Items<typename It::template At<k>>{reinterpret_cast<const typename It::template At<k>*>(
+                                             item_stream<k>(wp).items + (t.a[k] - item_stream<k>(wp).base) * sizeof(typename It::template At<k>)),
+                                         t.b[k] - t.a[k]}...);
+}
+
 // One unit of a record body: group g = ct / G runs tasks g, g + C/G, ... (G = 1: one thread per task).  All G lanes of a
 // group see the same i, so the group stays converged through B::run.  run() gets, in order: the head argument (a range()
-// index, a record from `in`, or none for NoArg), the task's items, the result, the broadcast block `sh` (bodies that have
-// one), the group (G > 1), then task_index, es and attempt.  An items task reads offsets o[i], o[i+1] and its items from
-// global memory; one whose offsets decrease or leave [item_base, item_count] reports TASK_BADARG and its body is not called.
+// index, a record from `in`, or none for NoArg), the task's items (one view per stream), the result, the broadcast block
+// `sh` (bodies that have one), the group (G > 1), then task_index, es and attempt.  An items task reads offsets o[i],
+// o[i+1] of each stream and its items from global memory; one whose offsets decrease or leave [base, count] in any stream
+// reports TASK_BADARG and its body is not called.
 // An emit body's task that pushed another number of values than it counted lowers *emit_err (the unit's word, in shared
 // memory) to its (task_index << 8 | TASK_EMIT): the kernel reports it only if the unit was not lost, since a faulting
 // attempt's values are discarded.
@@ -1185,10 +1287,12 @@ __device__ __forceinline__ void run_unit(const WaveParams& wp, const TaskRecord&
     using Res = ResultRecord<B>;
     constexpr uint32_t G = GroupOf<B>::kG, C = kConsumers;
     const uint64_t g0 = wp.index_base + rec.first;
-    const uint64_t* const o = wp.item_offs + (rec.first - wp.item_first);   // items bodies: the unit's offsets
+    constexpr uint32_t K = ItemsOf<B>::kStreams > 0 ? ItemsOf<B>::kStreams : 1u;
+    using Streams = std::make_index_sequence<K>;
+    const UnitItems<K> u = unit_items(wp, rec.first, Streams{});   // items bodies: the unit's offsets in each stream
     for (uint32_t i = ct / G; i < rec.count; i += C / G) {
         auto res = [&]() -> Res& { return *reinterpret_cast<Res*>(out + (size_t)i * L::R); };
-        auto call = [&](Res& r, const auto&... head) {  // head: the head argument, then the items
+        auto call = [&](Res& r, const auto&... head) {  // head: the head argument, then the items of each stream
             if constexpr (EmitOf<B>::kOn) {
                 // emit bodies: the count pass records the task's count, the emit pass its global end offset (the span the
                 // count pass gave, so the offsets stay consistent); a task that pushed another number reports TASK_EMIT
@@ -1226,15 +1330,15 @@ __device__ __forceinline__ void run_unit(const WaveParams& wp, const TaskRecord&
         if constexpr (kIndex) {
             call(res(), (Arg)(wp.index_start + (int64_t)(rec.first + i) * wp.index_step));
         } else if constexpr (ItemsOf<B>::kOn) {
-            using T = typename ItemsOf<B>::T;
-            const uint64_t a = o[i], b = o[i + 1];
-            if (a > b || a < wp.item_base || b > wp.item_count) {
+            TaskSpans<K> t;
+            if (bad_spans(wp, u, i, Streams{}, t)) {
                 if (ct % G == 0) es.report(TASK_BADARG, g0 + i);
                 continue;
             }
-            const Items<T> x{reinterpret_cast<const T*>(wp.items + (a - wp.item_base) * sizeof(T)), b - a};
-            if constexpr (L::kNoArg) call(res(), x);
-            else call(res(), *reinterpret_cast<const Arg*>(in + (size_t)i * L::A), x);
+            with_items<B>(wp, t, Streams{}, [&](const auto&... x) {
+                if constexpr (L::kNoArg) call(res(), x...);
+                else call(res(), *reinterpret_cast<const Arg*>(in + (size_t)i * L::A), x...);
+            });
         } else {
             call(res(), *reinterpret_cast<const Arg*>(in + (size_t)i * L::A));
         }

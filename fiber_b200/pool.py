@@ -753,13 +753,13 @@ class Pool:
         d.attempt = self._attempt
         d.flags = flags
         seq = ctypes.c_uint64(0)
-        if enc.n and enc.items is not None:
-            values, offsets = enc.items
-            keep += [values, offsets]
-            it = _abi.ItemsDesc()
-            it.items, it.offsets = values.ctypes.data, offsets.ctypes.data
-            it.n_items, it.item_bytes = len(values), values.dtype.itemsize
-            _abi.check(eng.lib.fbr_map_submit_items(eng.handle, ctypes.byref(d), ctypes.byref(it), ctypes.byref(seq)))
+        if enc.n and enc.streams is not None:
+            streams = (_abi.ItemsDesc * len(enc.streams))()
+            for it, (values, offsets) in zip(streams, enc.streams):
+                keep += [values, offsets]
+                it.items, it.offsets = values.ctypes.data, offsets.ctypes.data
+                it.n_items, it.item_bytes = len(values), values.dtype.itemsize
+            _abi.check(eng.lib.fbr_map_submit_items_n(eng.handle, ctypes.byref(d), streams, len(streams), ctypes.byref(seq)))
         elif enc.n:
             _abi.check(eng.lib.fbr_map_submit(eng.handle, ctypes.byref(d), ctypes.byref(seq)))
         self.sent_tasks += enc.n
@@ -800,8 +800,8 @@ class Pool:
 
     def _submit_proc(self, spec, kind, items, chunksize, single=False):
         """Process-isolated workers: the map is cut into blocks that worker processes pull (procpool.py)."""
-        if not isinstance(items, (range, list, np.ndarray, registry.Ragged)):
-            items = list(items)         # a Ragged stays one: its blocks are slices with rebased offsets
+        if not isinstance(items, (range, list, np.ndarray, registry.Ragged, registry.Columns)):
+            items = list(items)         # a Ragged (or Columns) stays one: its blocks are slices with rebased offsets
         if kind == "map" and len(items):
             spec.encode_map(items[:1] if not isinstance(items, range) else items)      # argument validation up front
         twin = registry.BITS_TWIN.get(spec.name) if (self._results_bits and kind != "apply") else None
@@ -831,7 +831,7 @@ class Pool:
         spec = self._spec_of(func)
         self.lazy_start_workers(func)
         if self._proc is not None:
-            return self._submit_proc(spec, "starmap", list(iterable), chunksize)
+            return self._submit_proc(spec, "starmap", iterable if isinstance(iterable, registry.Columns) else list(iterable), chunksize)
         enc = spec.encode_starmap(iterable)
         if self._results_bits and spec.name in registry.BITS_TWIN:
             return self._submit_bits(func, spec, enc, _abi.FBR_STARMAP, chunksize)

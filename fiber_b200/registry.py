@@ -58,7 +58,10 @@ def device_body(name, source=None, entry="fbr_body_entry", args="i64", bits_entr
     A task's items are a 1-D array of the element dtype (or a 1-D array / list whose values the dtype holds exactly: floats
     into an integer dtype or integers out of its range raise ``TypeError``), or, for a 1-byte
     element, ``bytes`` / ``bytearray`` / ``memoryview`` / ``str`` (sent as UTF-8).  ``map(f, Ragged(values, offsets))``
-    passes a whole ragged array without a copy.
+    passes a whole ragged array without a copy.  A body with 2 to 4 item streams (``using Items = fbr::ItemTypes<...>;``)
+    takes a list of pairs, one per stream in order, e.g. ``items=[("a", "u1"), ("b", "u1")]``: the item parameters then
+    come in that order after the broadcast parameter, each stream with its own element dtype and the same rules, and
+    ``starmap(f, Columns(ra, rb))`` passes two ``Ragged`` columns without a copy.
 
     An EMIT record body (``using Out = ...;`` and ``using Res = fbr::NoRes;`` in its struct) returns a variable-length array
     per task: ``out="<u4"`` describes one element (``result=`` is not passed).  A task's value reads as a list, or, with
@@ -98,7 +101,8 @@ def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_
     (``group_threads`` > 1 in its module descriptor: several threads per task, records up to 32 KB) registers like any
     other record body.  Items bodies (``FBR_BODY_ITEMS``) take ``items=(parameter name, element dtype)``, whose size must
     be the module's item size, and ``args=None`` when they have no head record; ``items`` is refused for every other
-    body (``ValueError``).  Emit bodies (``FBR_BODY_EMIT``) take ``out=<element dtype>``, whose size must be the module's
+    body (``ValueError``).  A body with several item streams takes ``items=[(name, dtype), ...]``, one pair per stream
+    in order: the count and every size must match ``fbr_body_items_streams`` (``ValueError``).  Emit bodies (``FBR_BODY_EMIT``) take ``out=<element dtype>``, whose size must be the module's
     out size, and ``out_as`` ("list", or "bytes" / "str" for 1-byte elements) instead of ``result``; ``out`` is refused for
     every other body (``ValueError``)."""
     import ctypes
@@ -148,15 +152,16 @@ def register_module(name, module_path, entry="fbr_body_entry", args="i64", bits_
     if info.flags & _abi.FBR_BODY_RECORD:
         if result is None:
             raise ValueError("record body %s: pass result=<dtype> (its %d-byte result record)" % (name, info.result_bytes))
-        elem, stage, ib = ctypes.c_uint32(0), ctypes.c_uint32(0), ctypes.c_uint32(0)
+        elem, stage = ctypes.c_uint32(0), ctypes.c_uint32(0)
         if has_shared:
             _abi.check(L.fbr_body_shared_info(fid.value, ctypes.byref(elem), ctypes.byref(stage)))
         if has_items:
-            _abi.check(L.fbr_body_items_info(fid.value, ctypes.byref(ib)))
+            ns, ib = ctypes.c_uint32(0), (ctypes.c_uint32 * _abi.MAX_ITEM_STREAMS)()
+            _abi.check(L.fbr_body_items_streams(fid.value, ctypes.byref(ns), ib))
             # args left at its default means no head record for a body that has none
             head = None if (isinstance(args, str) and args == "i64" and info.arg_bytes == 0) else args
-            record = _Items(info, items, head, result, shared, ib.value, elem.value, stage.value)
-            items = (record.item_name, record.item_dtype)
+            record = _Items(info, items, head, result, shared, list(ib)[:ns.value], elem.value, stage.value)
+            items = record.layouts()[3]
         elif has_shared:
             record = _Broadcast(info, args, result, shared, elem.value, stage.value)
         else:
@@ -237,14 +242,19 @@ def body_name_of(func):
 class Encoded:
     """Fixed-layout form of one map's arguments."""
     __slots__ = ("n", "args", "arg_stride", "index_start", "index_step", "shared", "task_index_base", "keepalive", "n_items",
-                 "items")
+                 "streams")
 
     def __init__(self, n, args=None, arg_stride=0, index_start=0, index_step=1, shared=None, task_index_base=0, n_items=0):
         self.n, self.args, self.arg_stride = n, args, arg_stride
         self.index_start, self.index_step = index_start, index_step
         self.shared, self.task_index_base = shared, task_index_base
         self.n_items = n_items     # bit-packed twins: argument items of the whole map (8 per task, the last may be short)
-        self.items = None          # items bodies: (values, uint64 offsets) -- task j reads values[offsets[j]:offsets[j+1]]
+        self.streams = None        # items bodies: per stream (values, uint64 offsets) -- task j reads values[offsets[j]:offsets[j+1]]
+
+    @property
+    def items(self):
+        """Stream 0 of an items body's map (its only stream for a one-stream body), or None."""
+        return self.streams[0] if self.streams else None
 
 
 def _as_i64(values, what):
@@ -545,11 +555,7 @@ class _Record(BodySpec):
             if vals[j] is not _MISSING:
                 raise TypeError("%s() got multiple values for argument %r" % (self.name, k))
             vals[j] = v
-        missing = [repr(names[j]) for j, v in enumerate(vals) if v is _MISSING]
-        if missing:
-            listed = missing[0] if len(missing) == 1 else "%s and %s" % (", ".join(missing[:-1]) + ("," if len(missing) > 2 else ""), missing[-1])
-            raise TypeError("%s() missing %d required positional argument%s: %s"
-                            % (self.name, len(missing), "" if len(missing) == 1 else "s", listed))
+        _check_missing(self.name, [names[j] for j, v in enumerate(vals) if v is _MISSING])
         return vals
 
     def _columns(self, columns):
@@ -614,6 +620,15 @@ class _Record(BodySpec):
         if vals.dtype.kind in "iub" and vals.dtype.itemsize <= 4:
             return int(vals.sum(dtype=np.int64))         # exact: fewer than 2^31 values of at most 32 bits
         return sum(vals.tolist())                        # Python's left-to-right sum, as over the reference's list
+
+
+def _check_missing(name, missing):
+    """Python's TypeError for a call of ``name`` that leaves the parameters ``missing`` without a value."""
+    if missing:
+        missing = [repr(m) for m in missing]
+        listed = missing[0] if len(missing) == 1 else "%s and %s" % (", ".join(missing[:-1]) + ("," if len(missing) > 2 else ""), missing[-1])
+        raise TypeError("%s() missing %d required positional argument%s: %s"
+                        % (name, len(missing), "" if len(missing) == 1 else "s", listed))
 
 
 def _same_bytes(a, b):
@@ -839,58 +854,126 @@ def _encode_items(name, dtype, xs):
     return values, offsets
 
 
+class Columns:
+    """``n`` argument tuples held as columns: ``starmap(f, Columns(ra, rb, thresholds))`` calls ``f(ra[i], rb[i],
+    thresholds[i])`` for every i.  Column k is the function's parameter k after the broadcast parameter (tasks under
+    Columns read the pool initializer's block): a ``Ragged`` for an items parameter, passed to the engine without a copy
+    where ``zip(ra, rb)`` would build a tuple and an array per task, or a 1-D array or list for a head-record field.  All
+    columns have the same length.  A slice is the Columns of the columns' slices (a Ragged's offsets rebased), and a
+    Columns pickles, so process-isolated pools ship each block's slice."""
+
+    def __init__(self, *columns):
+        if not columns:
+            raise ValueError("Columns: pass at least one column")
+        n = len(columns[0])
+        for k, c in enumerate(columns):
+            if len(c) != n:
+                raise ValueError("Columns: column %d has %d entries, column 0 has %d" % (k, len(c), n))
+        self.columns = columns
+
+    def __len__(self):
+        return len(self.columns[0])
+
+    def __getitem__(self, i):
+        if isinstance(i, slice):
+            return Columns(*(c[i] for c in self.columns))
+        return tuple(c[i] for c in self.columns)
+
+    def __iter__(self):
+        return (self[i] for i in range(len(self)))
+
+    def __reduce__(self):
+        return (Columns, self.columns)
+
+
+def _is_item_pair(x):
+    return isinstance(x, (tuple, list)) and len(x) == 2 and isinstance(x[0], str) and x[0].isidentifier()
+
+
 class _Items(_Broadcast):
-    """A record body whose task also takes one variable-length array (``FBR_BODY_ITEMS``): ``item_name`` is its
-    parameter, ``item_dtype`` one element.  The parameters are the broadcast parameter (bodies with a Shared type), the
-    items, then the argument dtype's fields (none when ``args`` is None: the body has no head record).  ``map(f, xs)``
-    passes one items array per task (bodies without a head record); ``starmap`` / ``apply_async`` bind the items like any
-    other parameter."""
+    """A record body whose task also takes 1 to 4 variable-length arrays (``FBR_BODY_ITEMS``), one per item stream:
+    ``item_names`` are their parameters and ``item_dtypes`` their elements, in stream order (``item_name`` /
+    ``item_dtype``: stream 0).  The parameters are the broadcast parameter (bodies with a Shared type), the items of each
+    stream, then the argument dtype's fields (none when ``args`` is None: the body has no head record).  ``map(f, xs)``
+    passes one items array per task (one-stream bodies without a head record); ``starmap`` / ``apply_async`` bind the
+    items like any other parameter, and ``starmap(f, Columns(...))`` takes whole columns."""
 
     def __init__(self, info, items, args, result, shared, item_bytes, shared_elem=0, shared_stage=0):
+        # item_bytes: the element size of each of the body's streams
         if args is None and info.arg_bytes:
             raise ValueError("%s: args=None, but the body's head record is %d bytes" % (info.name.decode(), info.arg_bytes))
         _Record.__init__(self, info, args, result)
         self.shared_name = self.shared_dtype = None
         if shared is not None:
             self._init_shared(shared, shared_elem, shared_stage)
-        if not (isinstance(items, (tuple, list)) and len(items) == 2 and isinstance(items[0], str) and items[0].isidentifier()):
-            raise ValueError("%s: items= is (<parameter name>, <element dtype>), got %r" % (self.name, items))
-        self.item_name = items[0]
-        if self.item_name == self.shared_name or (self.params is not None and self.item_name in self.params):
-            raise ValueError("%s: the items parameter %r is also another parameter" % (self.name, self.item_name))
-        self.item_dtype = _record_dtype(items[1], "item", self.name)
-        if self.item_dtype.itemsize != item_bytes:
-            raise ValueError("%s: item dtype %s is %d bytes, the body's Item is %d"
-                             % (self.name, self.item_dtype, self.item_dtype.itemsize, item_bytes))
+        k = len(item_bytes)
+        pairs = [items] if _is_item_pair(items) else list(items) if isinstance(items, (tuple, list)) else []
+        if not pairs or not all(_is_item_pair(p) for p in pairs):
+            raise ValueError(("%s: items= is (<parameter name>, <element dtype>), got %r" if k == 1 else
+                              "%s: items= is a list of (<parameter name>, <element dtype>) pairs, one per item stream, got %r")
+                             % (self.name, items))
+        if len(pairs) != k:
+            raise ValueError("%s: items= describes %d item stream%s, the body takes %d"
+                             % (self.name, len(pairs), "" if len(pairs) == 1 else "s", k))
+        self.item_names = tuple(p[0] for p in pairs)
+        for j, n in enumerate(self.item_names):
+            if n == self.shared_name or (self.params is not None and n in self.params) or n in self.item_names[:j]:
+                raise ValueError("%s: the items parameter %r is also another parameter" % (self.name, n))
+        self.item_dtypes = tuple(_record_dtype(p[1], "item", self.name) for p in pairs)
+        for j, (d, b) in enumerate(zip(self.item_dtypes, item_bytes)):
+            if d.itemsize != b:
+                raise ValueError(("%s: item dtype %s is %d bytes, the body's Item is %d" if k == 1 else
+                                  "%%s: item dtype %%s is %%d bytes, the body's stream %d item is %%d" % j)
+                                 % (self.name, d, d.itemsize, b))
+        self.item_name, self.item_dtype = self.item_names[0], self.item_dtypes[0]
 
     def layouts(self):
         shared = (self.shared_name, self.shared_dtype) if self.shared_name is not None else None
-        return (self.arg_dtype, self.res_dtype, shared, (self.item_name, self.item_dtype))
+        items = tuple(zip(self.item_names, self.item_dtypes))
+        return (self.arg_dtype, self.res_dtype, shared, items[0] if len(items) == 1 else items)
 
-    def _with_items(self, enc, xs):
-        enc.items = _encode_items(self.name, self.item_dtype, xs)
-        enc.n = len(enc.items[1]) - 1
+    def _with_items(self, enc, columns):
+        enc.streams = [_encode_items(self.name, d, xs) for d, xs in zip(self.item_dtypes, columns)]
+        enc.n = len(enc.streams[0][1]) - 1
         return enc
 
+    def encode_starmap(self, items):
+        if isinstance(items, Columns):
+            return self._encode_columns(items)
+        return super().encode_starmap(items)
+
+    def _encode_columns(self, c):
+        k, want = len(self.item_names), len(self.item_names) + len(self._fields)
+        if len(c.columns) != want:
+            raise TypeError("%s() takes %d argument%s after the broadcast parameter, got %d columns"
+                            % (self.name, want, "" if want == 1 else "s", len(c.columns)))
+        enc = Encoded(0) if self.arg_dtype is None else self._columns(list(c.columns[k:]))
+        return self._with_items(enc, c.columns[:k])
+
     def _encode(self, items, fast, apply=False):
+        k = len(self.item_names)
         if fast:
-            if self.arg_dtype is None:      # map(f, xs): each item is one task's items; a broadcast block is the initializer's
-                return self._with_items(Encoded(0), items)
+            if self.arg_dtype is None and k == 1:   # map(f, xs): each item is one task's items; a broadcast block is the initializer's
+                return self._with_items(Encoded(0), [items])
             items = [(it,) for it in items]
-        xs, rows, block = [], [], None
-        for args, kwds, block in self._calls(items, apply, 1 + len(self._fields)):    # the items and the record's fields
+        xs, rows, block = [[] for _ in range(k)], [], None
+        for args, kwds, block in self._calls(items, apply, k + len(self._fields)):    # the items and the record's fields
             kwds = dict(kwds)
-            if self.item_name in kwds:
-                x = kwds.pop(self.item_name)
-            elif args:
-                x, args = args[0], tuple(args[1:])
-            else:
-                raise TypeError("%s() missing 1 required positional argument: %r" % (self.name, self.item_name))
-            xs.append(x)
+            missing = []
+            for j, name in enumerate(self.item_names):
+                if name in kwds:
+                    xs[j].append(kwds.pop(name))
+                elif args:
+                    xs[j].append(args[0])
+                    args = tuple(args[1:])
+                else:
+                    missing.append(name)
+            _check_missing(self.name, missing)
             if self.arg_dtype is None:
                 if args or kwds:
+                    n = k + (self.shared_name is not None)
                     raise TypeError("%s() takes %d positional argument%s but more were given (unexpected %s)"
-                                    % (self.name, 1 + (self.shared_name is not None), "" if self.shared_name is None else "s",
+                                    % (self.name, n, "" if n == 1 else "s",
                                        ", ".join([repr(a) for a in args] + list(map(repr, kwds)))))
             else:
                 rows.append(self._bind(args, kwds))

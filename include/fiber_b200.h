@@ -130,6 +130,12 @@ typedef struct fbr_body_module {
     /* FBR_BODY_EMIT record bodies: sizeof(Out) (1, 2 or a multiple of 4 up to 4096).  0 (or left out of a hand-written
        descriptor) for every other body */
     uint32_t out_bytes;
+    /* FBR_BODY_ITEMS record bodies: the number of item streams each task takes (the body's Items = fbr::ItemTypes<...>:
+       2, 3 or 4; 0 or 1 = one stream, `using Item`), and the element sizes of streams 1 to 3 (stream 0's is item_bytes;
+       each 1, 2 or a multiple of 4 up to 4096; 0 past the last stream).  0 (or left out of a hand-written descriptor) for
+       every other body */
+    uint32_t item_streams;
+    uint32_t more_item_bytes[3];
 } fbr_body_module_t;
 typedef const fbr_body_module_t* (*fbr_body_entry_fn)(void);
 int fbr_register_body(const char* name, const char* module_path, const char* entry, int* func_id);
@@ -137,8 +143,12 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
  * passes a block of shared_bytes > 0, a multiple of elem_bytes; blocks up to stage_bytes are staged into shared memory
  * once per CTA, larger ones are read from global memory. */
 int fbr_body_shared_info(int func_id, uint32_t* elem_bytes, uint32_t* stage_bytes);
-/* Item size of a FBR_BODY_ITEMS body (0 for other bodies).  The dispatch kernel reads each task's items from global memory. */
+/* Item size of a FBR_BODY_ITEMS body (0 for other bodies; stream 0's for a multi-stream body).  The dispatch kernel reads
+ * each task's items from global memory. */
 int fbr_body_items_info(int func_id, uint32_t* item_bytes);
+/* Item streams of a FBR_BODY_ITEMS body (1 to 4; 0 for other bodies) and the element size of each (item_bytes[k] for
+ * stream k, 0 past the last stream). */
+int fbr_body_items_streams(int func_id, uint32_t* n_streams, uint32_t item_bytes[4]);
 /* Value size of a FBR_BODY_EMIT body (0 for other bodies). */
 int fbr_body_emit_info(int func_id, uint32_t* out_bytes);
 
@@ -232,15 +242,24 @@ int fbr_map_submit(fbr_pool_t* pool, const fbr_map_desc_t* desc, uint64_t* seq);
  * FBR_TASK_BADARG.  Host-resident items and offsets stream to the device wave by wave through two staging halves of
  * ring_bytes each (a resilient map copies its whole block once); a claim unit whose offsets and items do not fit one
  * half is refused with FBR_EINVAL before anything launches.
- * fbr_map_submit refuses items bodies and fbr_map_submit_items every other body (FBR_EINVAL). */
+ * fbr_map_submit refuses items bodies and fbr_map_submit_items every other body (FBR_EINVAL).
+ *
+ * One fbr_items_desc_t describes one item stream.  A body with K streams (fbr_body_items_streams) takes K of them, in
+ * stream order, through fbr_map_submit_items_n: each has its own items, offsets, n_items and element size, all the checks
+ * above apply to each, and task j reads [offsets[j], offsets[j+1]) of every stream.  FBR_ARGS_DEVICE applies to every
+ * stream of the map.  Host-resident streams share the same two staging halves: in a wave's half, stream k's offsets and
+ * item span follow stream k-1's, each stream starting on a 256 B boundary, and a claim unit whose K streams do not fit one
+ * half together is refused.  fbr_map_submit_items is fbr_map_submit_items_n with n_streams = 1. */
 typedef struct fbr_items_desc {
     const void* items;        /* item array: host, or device on worker 0 with FBR_ARGS_DEVICE */
     const uint64_t* offsets;  /* n_tasks + 1 non-decreasing item indices: task j reads items [offsets[j], offsets[j+1]) */
     uint64_t n_items;         /* items in `items`; every offset is <= n_items */
-    uint32_t item_bytes;      /* must equal the body's */
+    uint32_t item_bytes;      /* must equal the body's element size of this stream */
     uint32_t pad;
 } fbr_items_desc_t;
 int fbr_map_submit_items(fbr_pool_t* pool, const fbr_map_desc_t* desc, const fbr_items_desc_t* items, uint64_t* seq);
+int fbr_map_submit_items_n(fbr_pool_t* pool, const fbr_map_desc_t* desc, const fbr_items_desc_t* streams, uint32_t n_streams,
+                           uint64_t* seq);
 
 /* Broadcast argument blocks (initargs / arguments every task shares, e.g. the parzen sample array
  * the reference pickles into each of its 102 task messages, SURVEY.md 3.2): uploaded once to every

@@ -109,6 +109,30 @@
 // array are legal on x.data.  All G lanes of a group body get the same x.  Items bodies cannot have kIndexArg.
 // FBR_EXPORT_RECORD_BODY sets FBR_BODY_ITEMS and writes item_bytes.
 //
+// A task may take 2 to 4 variable-length arrays (two strings to compare, two token lists to intersect, a series and its
+// weights): the body lists their element types, which may differ, and run() gets one view per stream, in order, where the
+// single x goes above.  Each stream has its own offsets, so each task's arrays have their own lengths:
+//
+//     struct CommonPrefix {                               // length of the common prefix of two byte strings
+//         using Items = fbr::ItemTypes<uint8_t, uint8_t>; // not together with `using Item`
+//         using Arg = fbr::NoArg;
+//         struct Res { uint32_t n; };
+//         static constexpr bool kIndexArg = false, kCanFault = false;
+//         __device__ static void run(const fbr::Items<uint8_t>& a, const fbr::Items<uint8_t>& b, Res& r, uint64_t task_index,
+//                                    const fbr::ErrSink& es, uint32_t attempt) {
+//             uint32_t k = 0;
+//             while (k < a.n && k < b.n && a.data[k] == b.data[k]) ++k;
+//             r.n = k;
+//         }
+//     };
+//     FBR_EXPORT_RECORD_BODY(CommonPrefix, "common_prefix_u1", common_prefix_entry, 0)
+//
+// The full signature is run([const Arg& a,] const fbr::Items<T0>& x0, ..., const fbr::Items<Tk-1>& xk-1, Res& r |
+// Emit<Out[,G]>& y, [Broadcast], [Group], task_index, es, attempt), and an emit body's count() takes the same leading
+// parameters.  All G lanes of a group get the same views.  A task whose offsets decrease or leave their stream's items in
+// any stream reports FBR_TASK_BADARG without its body being called.  FBR_EXPORT_RECORD_BODY writes item_streams and the
+// element sizes of streams 1 to 3.
+//
 // An EMIT record body's task returns a variable-length array (a document's tokens, an integer's prime factors): it declares
 // the element type and Res = fbr::NoRes, and run() appends to an emitter where other record bodies write Res& r:
 //
@@ -281,8 +305,8 @@ constexpr uint32_t record_group() {
 // body_flags, which carry FBR_BODY_INDEX_ARG exactly when Body::kIndexArg is true (a range() map of a body without the
 // index instantiation would read no arguments).  unit_tasks is the number of tasks whose records fill one shared-memory
 // stage of dispatch_record_kernel.  A body with a Shared type also gets FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST and
-// its element size and staging budget; a body with kGroup gets group_threads = kGroup; a body with an Item type gets
-// FBR_BODY_ITEMS and its item size.
+// its element size and staging budget; a body with kGroup gets group_threads = kGroup; a body with an Item type (or an
+// Items = fbr::ItemTypes<...> list) gets FBR_BODY_ITEMS, its item streams and their item sizes.
 #define FBR_EXPORT_RECORD_BODY(Body, body_name, entry, body_flags)                                                \
     static_assert(fbr_body_export::record_body_ok<Body>(), "record body");                                       \
     static_assert((((body_flags) & FBR_BODY_INDEX_ARG) != 0) == Body::kIndexArg,                                 \
@@ -296,7 +320,10 @@ constexpr uint32_t record_group() {
                                             fbr_body_export::record_launch<Body>(), fbr_body_export::record_occupancy<Body>(), \
                                             fbr::record::BroadcastOf<Body>::kElem, fbr::record::BroadcastOf<Body>::kStage, \
                                             fbr_body_export::record_group<Body>(),                               \
-                                            fbr::record::ItemsOf<Body>::kElem, fbr::record::EmitOf<Body>::kElem}; \
+                                            fbr::record::ItemsOf<Body>::kElem, fbr::record::EmitOf<Body>::kElem, \
+                                            fbr::record::ItemsOf<Body>::kStreams,                                \
+                                            {fbr::record::ItemsOf<Body>::elem(1), fbr::record::ItemsOf<Body>::elem(2), \
+                                             fbr::record::ItemsOf<Body>::elem(3)}};                              \
         return &m;                                                                                               \
     }
 
