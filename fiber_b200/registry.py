@@ -1032,6 +1032,9 @@ class _Parzen(BodySpec):
         if px.shape[1] != 1:
             # the reference evaluates `np.abs(row) > 1/2` on a length-p row, which raises for p != 1
             raise ValueError("The truth value of an array with more than one element is ambiguous")
+        if xs.shape[0] == 0:
+            # the reference's `k_n / len(x_samples)` (examples/parzen_estimation.py:15); the kernel would return 0.0 / 0.0
+            raise ZeroDivisionError("division by zero")
         hdr = np.zeros((), dtype=self.HEADER)
         hdr["n_samples"], hdr["dims"], hdr["power"], hdr["elem_bytes"] = xs.shape[0], xs.shape[1], px.shape[1], self.elem.itemsize
         hdr["point_x"][: px.shape[0]] = px[:, 0].astype(np.float64)

@@ -154,6 +154,24 @@ def test_encoder_parzen_shared_block():
         s.encode_starmap([(xs, px, 0.1), (xs[:100], px, 0.2)])
 
 
+def test_encoder_parzen_empty_samples_divide_by_zero():
+    """The reference divides k_n by len(x_samples): an empty sample set raises ZeroDivisionError, on the encoder's
+    side here, before any block is built or any task runs (the kernel would compute 0.0 / 0.0)."""
+    from oracle import bodies as B
+    px = np.array([[0.1], [0.2], [0.3]])
+    with pytest.raises(ZeroDivisionError):
+        B.parzen_estimation(np.zeros((0, 3)), px, 0.5)
+    for name in ("parzen_f64", "parzen_f32"):
+        s = registry.spec(name)
+        with pytest.raises(ZeroDivisionError, match="division by zero"):
+            s.encode_apply((np.zeros((0, 3)), px, 0.5), {})
+        with pytest.raises(ZeroDivisionError):
+            s.encode_starmap([(np.zeros((0, 3)), px, w) for w in (0.5, 1.0)])
+        with pytest.raises(ZeroDivisionError):
+            s.shared_block(np.zeros((0, 3)), px)
+        assert len(s.encode_apply((np.zeros((1, 3)), px, 0.5), {}).shared) == 80 + 3 * s.elem.itemsize
+
+
 def test_encoder_payload():
     from oracle import cref
     recs = cref.payload_records(10, 4)

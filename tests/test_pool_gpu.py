@@ -205,6 +205,60 @@ def test_parzen_f32_tolerance(pool, golden, record_property):
     assert mismatches == cpu_mismatches <= 2
 
 
+def _parzen_case(dims, n, seed):
+    """n samples in `dims` dimensions around a point_x whose entries are not exact in fp32 (0.1, 0.2, ...): normal samples,
+    samples exactly on |q| = 1/2 for h = 1/2 in every dimension (inside), a NaN sample (inside, as in the reference) and
+    +-inf samples (outside)."""
+    rng = np.random.default_rng(seed)
+    px = (0.1 * np.arange(1, dims + 1)).reshape(dims, 1)
+    xs = px[:, 0] + rng.standard_normal((n, dims)) * 0.6
+    for i in range(0, n, 7):                                # x = px +- h/2 where that is exact in fp64 and in fp32
+        x = px[:, 0] + np.where(rng.random(dims) < 0.5, -0.25, 0.25)
+        exact = ((px[:, 0] - x) / 0.5 == np.sign(px[:, 0] - x) * 0.5) & \
+                ((px[:, 0].astype(np.float32) - x.astype(np.float32)) / np.float32(0.5) == np.sign(px[:, 0] - x) * 0.5)
+        xs[i] = np.where(exact, x, px[:, 0])
+    if n > 3:
+        xs[1, dims - 1] = np.nan
+        xs[2, 0], xs[3, dims // 2] = np.inf, -np.inf
+    return xs, px
+
+
+PARZEN_WIDTHS = [2.0 ** -20, 0.5, 1.0, 3.7, 2.0 ** 20]
+
+
+@pytest.mark.parametrize("dims", [1, 2, 3, 5, 8])
+def test_parzen_dims_and_sample_counts(pool, dims):
+    """Both parzen bodies beyond the example's 10 000 x 2 samples at point 0: every dimension count the device body takes
+    (dims == 2 has its own path: 1024 samples per round and a tail loop; the rest a loop over 256 threads), sample counts
+    around those strides, a point_x that is not exact in fp32, boundary, NaN and infinite samples, and extreme widths.
+    parzen_f64 is bit-exact against the reference's arithmetic; parzen_f32's k_n equals the fp32 C restatement's."""
+    from oracle import bodies as B, cref
+    on_boundary = 0
+    for n in (1, 31, 255, 256, 257, 1023, 1024, 1025, 4097):
+        xs, px = _parzen_case(dims, n, seed=dims * 10000 + n)
+        on_boundary += int((np.abs((px[:, 0] - xs) / 0.5) == 0.5).all(axis=1).sum())
+        got = pool.starmap(W.parzen_estimation, [(xs, px, w) for w in PARZEN_WIDTHS], 1)
+        got32 = pool.starmap(W.parzen_estimation_f32, [(xs, px, w) for w in PARZEN_WIDTHS], 1)
+        for w, r64, r32 in zip(PARZEN_WIDTHS, got, got32):
+            want = B.parzen_estimation(xs, px, w)
+            k64 = cref.parzen_count(xs, px, w)
+            assert B.parzen_count_np(xs, px, w) == k64 and want == (w, (k64 / n) / w), (dims, n, w)
+            assert tuple(r64) == want, (dims, n, w, tuple(r64), want)
+            assert r32[0] == w and int(round(r32[1] * w * n)) == cref.parzen_count(xs, px, w, np.float32), (dims, n, w)
+    assert on_boundary > 0
+
+
+def test_parzen_empty_samples_raise_zero_division(pool):
+    """The reference divides by len(x_samples): a map over an empty sample set raises ZeroDivisionError, and the pool
+    goes on."""
+    for func in (W.parzen_estimation, W.parzen_estimation_f32):
+        with pytest.raises(ZeroDivisionError):
+            pool.apply(func, (np.zeros((0, 3)), np.zeros((3, 1)), 0.5))
+        with pytest.raises(ZeroDivisionError):
+            pool.starmap(func, [(np.zeros((0, 2)), np.zeros((2, 1)), w) for w in (0.5, 1.0)])
+    assert pool.apply(W.parzen_estimation, (np.zeros((2, 1)), np.zeros((1, 1)), 0.5)) == (0.5, 2.0)
+
+
 # ---- synthetic 4 KB payload map ---------------------------------------------------------------------
 def test_payload_map_golden(pool, golden):
     from oracle import bodies as B

@@ -9,6 +9,7 @@ import fiber_b200
 from fiber_b200 import _abi, registry
 from fiber_b200.pool import ResultArray
 
+from . import layout_bodies as LB
 from . import record_bodies as RB
 
 
@@ -69,16 +70,101 @@ def test_registration_rejects_bad_layouts():
 
 def test_plan_keeps_every_unit_16_byte_aligned():
     lib = _abi.load()
-    for name in ("polar_f64", "mix_i32x3", "row_stats_u32", "splitmix_pair", "scale5_f64"):
+    for name in ("polar_f64", "mix_i32x3", "row_stats_u32", "splitmix_pair", "scale5_f64") + tuple(LB.BY_NAME):
         s = registry.spec(name)
         for n in (1, 7, 1000, 10 ** 6, 10 ** 8):
             for cs in (1, 3, 7, 32, 100, 5000):
                 p = _abi.Plan()
                 assert lib.fbr_plan_query(s.func_id, n, cs, 0, 1, 0, 132, ctypes.byref(p)) == 0
                 assert p.unit_tasks * s.result_bytes % 16 == 0 and p.unit_tasks * s.arg_bytes % 16 == 0, (name, n, cs)
-                assert p.slot_stride == p.unit_tasks * s.result_bytes
+                assert p.slot_stride == p.unit_tasks * s.result_bytes and p.unit_tasks % LB.align_tasks(s.arg_bytes, s.result_bytes) == 0
                 info = _abi.BodyInfo()
                 assert lib.fbr_body_info(s.func_id, ctypes.byref(info)) == 0 and p.unit_tasks <= info.unit_tasks
+
+
+def _gather_route(slot_stride, unit, R, resilient):
+    """The gather kernel the wave planner picks for a map's full units (engine.cu, the rows_ok / bulk_ok lines):
+    gather_bulk_kernel for 16 KB multiples (not on resilient maps), gather_rows_kernel for 4 KB multiples, else
+    gather_ordered_kernel (flat)."""
+    rows = unit * R == slot_stride and slot_stride % 4096 == 0
+    if rows and not resilient and slot_stride % 16384 == 0:
+        return "bulk"
+    return "rows" if rows else "flat"
+
+
+# (A, R, G, kAlign, kUnit, gather route of a full unit at the default chunksize) of the fixed-record layouts
+LAYOUT_TABLE = {
+    "lay_a4_r4": (4, 4, 1, 4, 1024, "rows"), "lay_a4_r4096": (4, 4096, 1, 4, 8, "bulk"),
+    "lay_a4092_r4": (4092, 4, 1, 4, 8, "flat"), "lay_a8_r24": (8, 24, 1, 2, 1024, "rows"),
+    "lay_a24_r8": (24, 8, 1, 2, 1024, "rows"), "lay_a12_r4096": (12, 4096, 1, 4, 8, "bulk"),
+    "lay_a4096_r12": (4096, 12, 1, 4, 8, "flat"), "lay_a2052_r2052": (2052, 2052, 1, 4, 8, "flat"),
+    "lay_a20_r20": (20, 20, 1, 4, 1024, "rows"), "lay_i8_r4096": (8, 4096, 1, 2, 8, "bulk"),
+    "lay_i8_r12": (8, 12, 1, 4, 1024, "rows"), "lay_a8_r16384_g2": (8, 16384, 2, 2, 2, "bulk"),
+    "lay_a16384_r8_g2": (16384, 8, 2, 2, 2, "flat"), "lay_a4_r8188_g4": (4, 8188, 4, 4, 4, "flat"),
+    "lay_a8188_r4_g4": (8188, 4, 4, 4, 4, "flat"), "lay_a32768_r32768_g32": (32768, 32768, 32, 1, 1, "bulk"),
+    "lay_a16_r32768_g32": (16, 32768, 32, 1, 1, "bulk"), "lay_a32768_r16_g8": (32768, 16, 8, 1, 1, "flat"),
+    "lay_a20_r36_g16": (20, 36, 16, 4, 512, "flat"), "lay_i8_r16384_g32": (8, 16384, 32, 2, 2, "bulk"),
+    "lay_i8_r8184_g8": (8, 8184, 8, 2, 4, "flat"),
+}
+
+
+def test_layout_sweep_reaches_every_layout_rule():
+    """The generated sweep bodies (tests/layout_bodies.py) land where they claim: the restated Layout<B>::kUnit and
+    align_tasks match what the module reports, the planner's slot stride gives the gather route of the table, and the
+    sweep as a whole reaches every kAlign class, group size, gather route (resilient maps too), staged and global broadcast
+    blocks, and every item and Out size class.  A change to any of these rules fails here instead of thinning the sweep."""
+    lib = _abi.load()
+    routes = {False: set(), True: set()}
+    for b in LB.LAYOUTS:
+        s = registry.spec(b.name)
+        info = _abi.BodyInfo()
+        assert lib.fbr_body_info(s.func_id, ctypes.byref(info)) == 0
+        assert (info.arg_bytes, info.result_bytes, info.unit_tasks) == (b.A, b.R, b.k_unit), b.name
+        assert info.flags & _abi.FBR_BODY_RECORD and bool(info.flags & _abi.FBR_BODY_INDEX_ARG) == b.index
+        assert b.smem <= LB.SMEM_BUDGET, b.name
+        p = _abi.Plan()
+        assert lib.fbr_plan_query(s.func_id, 10 ** 6, 0, 0, 1, 0, 132, ctypes.byref(p)) == 0
+        assert p.unit_tasks == b.k_unit and p.slot_stride == b.k_unit * b.R, b.name
+        for resilient in (False, True):
+            if resilient or not b.fault:
+                routes[resilient].add(_gather_route(p.slot_stride, p.unit_tasks, b.R, resilient))
+        if b.name in LAYOUT_TABLE:
+            A, R, G, al, unit, route = LAYOUT_TABLE[b.name]
+            assert (b.A, b.R, b.group, b.k_align, b.k_unit) == (A, R, G, al, unit), b.name
+            assert _gather_route(p.slot_stride, p.unit_tasks, R, False) == route, b.name
+    fixed = [LB.BY_NAME[n] for n in LAYOUT_TABLE]
+    assert {b.k_align for b in fixed} == {1, 2, 4}
+    assert {b.group for b in fixed} == {1, 2, 4, 8, 16, 32}
+    # the largest record of each kAlign class: 4096 B one-thread, 16 KB with kAlign 2, 8 KB with kAlign 4, 32 KB
+    for al, G, size in ((4, 1, 4096), (2, 2, 16384), (4, 4, 8188), (1, 32, 32768), (2, 32, 16384)):
+        assert any(b.k_align == al and b.group == G and max(b.A, b.R) == size for b in fixed), (al, G, size)
+    assert any(b.A == b.R == 32768 for b in fixed) and any(b.R >= 32 * b.A for b in fixed) and any(b.A >= 32 * b.R for b in fixed)
+    # a large slot that is not a multiple of 4 KB goes to the flat gather
+    assert any(b.k_unit * b.R > 16384 and b.k_unit * b.R % 4096 for b in fixed)
+    assert routes[False] == {"flat", "rows", "bulk"} and routes[True] == {"flat", "rows"}
+    faults = {_gather_route(b.k_unit * b.R, b.k_unit, b.R, False) for b in LB.LAYOUTS if b.fault}
+    assert faults == {"flat", "rows", "bulk"}                        # the bulk-sized slot goes to the rows kernel resilient
+    # broadcast blocks: never staged, staged, and a stage as large as the budget allows next to the layout's stages
+    stages = {b.shared[1] for b in LB.LAYOUTS if b.shared}
+    assert 0 in stages and 4096 in stages
+    assert any(b.smem == LB.SMEM_BUDGET for b in LB.LAYOUTS if b.shared)
+    assert {b.shared[0] for b in LB.LAYOUTS if b.shared} >= {4, 12, 4096}
+    for b in LB.LAYOUTS:
+        if b.shared:
+            elem, stage = ctypes.c_uint32(), ctypes.c_uint32()
+            assert lib.fbr_body_shared_info(registry.spec(b.name).func_id, ctypes.byref(elem), ctypes.byref(stage)) == 0
+            assert (elem.value, stage.value) == b.shared
+    items = [b for b in LB.LAYOUTS if b.items]
+    assert {b.items for b in items if len(b.items) == 1} >= {(1,), (2,), (8,), (12,), (4096,)}
+    assert (1, 2, 12, 4096) in {b.items for b in items}
+    assert {b.A for b in items} == {0, 12} and {8, 32} <= {b.group for b in items}
+    emits = [b for b in LB.LAYOUTS if b.out is not None]
+    assert {b.out[0] for b in emits} >= {1, 2, 8, 12, 4096}
+    assert {b.out[2] for b in emits if b.group == 1} == {True, False} and 32 in {b.group for b in emits}
+    assert any(b.items and b.shared and b.group > 1 for b in emits)
+    for b in emits:
+        ob = ctypes.c_uint32()
+        assert lib.fbr_body_emit_info(registry.spec(b.name).func_id, ctypes.byref(ob)) == 0 and ob.value == b.out[0]
 
 
 def test_encoders():
