@@ -11,7 +11,7 @@ is loaded on first use and its absence is a hard error (no CPU fallback).
 import multiprocessing as _mp
 
 from .meta import meta  # noqa: F401
-from .pool import ApplyResult, MapResult, Pool, ResultArray  # noqa: F401
+from .pool import ApplyResult, FoldResult, MapResult, Pool, ResultArray  # noqa: F401
 from .process import Process, active_children, device_process  # noqa: F401
 from . import config  # noqa: F401
 from .config import init, reset  # noqa: F401

@@ -173,6 +173,8 @@ struct BodyEntry {
     uint32_t item_streams = 0;                                // FBR_BODY_ITEMS record bodies: 1 to 4 item streams ...
     uint32_t item_bytes[kMaxItemStreams] = {};                // ... and the element size of each
     uint32_t out_bytes = 0;                                   // FBR_BODY_EMIT record bodies
+    void (*fold)(void*, uint64_t, void*, void*) = nullptr;    // FBR_BODY_FOLD record bodies: tree() over device records ...
+    std::vector<uint8_t> identity;                            // ... and identity(), result_bytes bytes
 };
 
 static std::mutex g_body_mu;
@@ -244,6 +246,8 @@ struct Worker {
     int sm_count = 0;
     cudaStream_t s_in = nullptr, s_comp = nullptr, s_out = nullptr;
     cudaStream_t s_gath = nullptr;         // higher-priority stream for gathers that overlap the next dispatch
+    cudaStream_t s_fold = nullptr;         // fbr_fold_values and the cross-block fold of fold maps: waited for under the pool lock,
+                                           // so it never queues behind the maps on the other streams
     bool prev_wave_overlap = false;        // the previous wave used only its half of the ring
     cudaStream_t s_push = nullptr;         // a stream of the ROOT worker's device: its copy engine pushes this worker's argument waves
     cudaStream_t s_push2 = nullptr;        // (waves alternate between the two, like the copy-outs)
@@ -267,15 +271,16 @@ struct Worker {
     cudaEvent_t ev_out[2];                 // out half's D2H finished
     uint64_t wave_no = 0;
     std::vector<int> occ, occ_index;   // per func_id: resident CTAs/SM of the explicit-argument / range() instantiation (0 = not asked yet)
+    std::vector<int> occ_fold, occ_fold_index;   // ... and of the fold pass of a fold body
     int occ_gather = 1, occ_fill = 1, occ_gather_rows = 1;
     std::vector<int> ctrl_free;        // free-list of control-block slots
 };
 
 // resident CTAs per SM of body `func_id` on this worker's device (current device must be w.device)
-static int worker_occ(Worker& w, int func_id, const BodyEntry& body, bool index_mode) {
-    std::vector<int>& v = index_mode ? w.occ_index : w.occ;
+static int worker_occ(Worker& w, int func_id, const BodyEntry& body, bool index_mode, bool fold) {
+    std::vector<int>& v = fold ? (index_mode ? w.occ_fold_index : w.occ_fold) : (index_mode ? w.occ_index : w.occ);
     if ((int)v.size() <= func_id) v.resize(func_id + 1, 0);
-    if (v[func_id] == 0) v[func_id] = std::max(1, body.occupancy(index_mode ? 1 : 0));
+    if (v[func_id] == 0) v[func_id] = std::max(1, body.occupancy((index_mode ? 1 : 0) | (fold ? 2 : 0)));
     return v[func_id];
 }
 
@@ -295,6 +300,8 @@ struct PartCtx {                          // constants of one worker's block of 
                                           // offsets slice and item span into the worker's d_items staging half
     bool direct = false;                  // contiguous, unshuffled, non-resilient block: the dispatch kernel stores every
                                           // unit at its final index (no ring, no task records, no gather launch)
+    bool fold = false;                    // FBR_FOLD: each unit writes its tree to d_fold, no result leaves the device
+    uint8_t* fold_total = nullptr;        // FBR_FOLD: the block's total, in the map's pinned segment
     const uint8_t* d_shared = nullptr;
     uint8_t* window_base = nullptr;       // device output of a FULL_WINDOW part
     const uint8_t* args_full = nullptr;   // device-resident arguments of the whole map (args_dev / resilient)
@@ -342,6 +349,7 @@ struct SeqPart {
     uint32_t lost_cap = 0, attempt = 0;
     bool finalized = false;               // resilient: window copied back to the host
     bool first_wave_pending = true;       // the block's first wave must wait for what submit_part put on s_in
+    void* d_fold = nullptr;               // FBR_FOLD: the partial of each claim unit, by its place in the block
     PartCtx cx;
     EmitBlock emit;
 };
@@ -373,6 +381,7 @@ struct SeqState {
     bool emit_pass = false;                // the emit pass of an emit map: its blocks carry the offsets their workers counted
     void* values = nullptr;                // emit pass: pinned values segment (host-resident results) ...
     uint64_t n_values = 0;                 // ... and the map's number of values
+    bool folded = false;                   // FBR_FOLD: the result record (out) holds tree() over the block totals
 };
 
 struct SharedBlock {
@@ -552,6 +561,7 @@ static int worker_init(fbr_pool* p, Worker& w, int device) {
     CK(cudaStreamCreateWithFlags(&w.s_in, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&w.s_comp, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&w.s_out, cudaStreamNonBlocking));
+    CK(cudaStreamCreateWithFlags(&w.s_fold, cudaStreamNonBlocking));
     {
         int lo_prio = 0, hi_prio = 0;
         CK(cudaDeviceGetStreamPriorityRange(&lo_prio, &hi_prio));
@@ -578,8 +588,8 @@ static int worker_init(fbr_pool* p, Worker& w, int device) {
     // synchronise with resident device processes, queues.cu); bodies registered later are asked on first use
     for (int f = 0, n = body_count(); f < n; ++f) {
         const BodyEntry& b = *body_of(f);
-        worker_occ(w, f, b, false);
-        if (b.flags & FBR_BODY_INDEX_ARG) worker_occ(w, f, b, true);
+        worker_occ(w, f, b, false, false);
+        if (b.flags & FBR_BODY_INDEX_ARG) worker_occ(w, f, b, true, false);
     }
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&w.occ_gather, (const void*)gather_ordered_kernel, kThreads, 0));
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&w.occ_fill, (const void*)payload_fill_kernel, kThreads, 0));
@@ -618,6 +628,7 @@ static void worker_destroy(Worker& w) {
     if (w.s_in) cudaStreamDestroy(w.s_in);
     if (w.s_comp) cudaStreamDestroy(w.s_comp);
     if (w.s_out) cudaStreamDestroy(w.s_out);
+    if (w.s_fold) { cudaStreamSynchronize(w.s_fold); cudaStreamDestroy(w.s_fold); }
     cudaFreeHost(w.h_records);
     cudaFree(w.d_records);
     cudaFree(w.d_headers);
@@ -664,7 +675,10 @@ static uint32_t pick_unit_record(const BodyEntry& b, uint32_t chunksize, uint64_
         const uint32_t m = chunksize / gcd_u32(chunksize, align) * align;   // lcm(chunksize, align)
         if (m <= pref) unit = pref / m * m;
     }
-    return std::max(align, unit / align * align);
+    unit = std::max(align, unit / align * align);
+    // fold maps: a power of two (align is one), so every unit is an aligned subtree of its block's tree()
+    if (chunksize == FBR_PLAN_FOLD) while (unit & (unit - 1)) unit &= unit - 1;
+    return unit;
 }
 
 static uint32_t pick_unit(const BodyEntry& b, uint32_t chunksize, uint64_t n_tasks, int sm_count, uint64_t ring_bytes) {
@@ -687,6 +701,12 @@ static uint32_t pick_unit(const BodyEntry& b, uint32_t chunksize, uint64_t n_tas
     unit = (uint32_t)round_up(unit, align);
     while (unit > align && (uint64_t)unit * per_task > ring_bytes) unit -= align;   // chunk-aligned unit too big for the ring
     return unit;
+}
+
+// the chunksize a map's units are picked for: a fold map's units ignore it (FBR_PLAN_FOLD)
+static uint32_t map_chunksize(const fbr_map_desc_t& d) {
+    if (d.flags & FBR_FOLD) return FBR_PLAN_FOLD;
+    return d.chunksize ? d.chunksize : 32u;
 }
 
 static void shuffle_records(TaskRecord* r, uint32_t n, uint64_t seed) {
@@ -900,7 +920,12 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
             wp.emit_values = (uint8_t*)emit.d_values;
         }
     }
-    int occ_d = worker_occ(w, st.func_id, body, d.arg_stride == 0);
+    if (cx.fold) {   // no unit stores results: each writes its tree to its place in d_fold
+        wp.ring = nullptr;
+        wp.fold_partials = (uint8_t*)part.d_fold;
+        wp.fold_first = part.first;
+    }
+    int occ_d = worker_occ(w, st.func_id, body, d.arg_stride == 0, cx.fold);
     if (body.max_ctas_per_sm) occ_d = std::min(occ_d, body.max_ctas_per_sm);
     if (ov && occ_d > 1) occ_d -= 1;     // leave SM slots for the concurrently running gather CTAs
     if (const char* e = getenv("FBR_DISPATCH_OCC")) occ_d = std::max(1, std::min(occ_d, atoi(e)));
@@ -936,7 +961,7 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
         gp.headers = hdr_base;
         gp.ring = ring_base;
         gp.n_units = n_units;
-        gp.slot_stride = cx.slot_stride;
+        gp.slot_stride = cx.fold ? 0u : cx.slot_stride;   // a fold wave's gather moves no payload, it only lists lost units
         gp.result_bytes = cx.R;
         gp.pad = 0;
         gp.out = out_window;
@@ -949,7 +974,7 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
         const int grid_g = (int)std::max<uint64_t>(1, std::min<uint64_t>((total_vec + kThreads * 4 - 1) / (kThreads * 4),
                                                                           (uint64_t)w.sm_count * w.occ_gather));
         // kernel choice for this wave (see kernels.cuh): TMA bulk pipeline, row streaming, or flat
-        const bool aligned = (((uintptr_t)gp.out & 15) == 0) && (((uint64_t)cx.unit * cx.R) == cx.slot_stride);
+        const bool aligned = !cx.fold && (((uintptr_t)gp.out & 15) == 0) && (((uint64_t)cx.unit * cx.R) == cx.slot_stride);
         const bool rows_ok = aligned && (cx.slot_stride % 4096 == 0) && getenv("FBR_GATHER_FLAT") == nullptr;
         const bool bulk_ok = rows_ok && !cx.resilient &&
                              (cx.slot_stride % bulk::kChunk == 0 || getenv("FBR_BULK_SMALL") != nullptr) &&   // 4 KB slots: the rows kernel
@@ -1040,9 +1065,13 @@ static int finish_round(fbr_pool* p, SeqState& st, SeqPart& part, bool copy_wind
     // Every block finishes on s_out, behind its copy-outs, even one without any: finishing on the compute stream puts a
     // DMA hop between back-to-back kernels of pipelined maps, which costs them what a blocking map() gains.
     CK(cudaStreamWaitEvent(w.s_out, w.ev_comp[last_rw], 0));
-    if (copy_window && cx.full_window && !cx.out_dev && !cx.keep_on_device && !cx.zero_copy && part.count) {
+    if (copy_window && cx.full_window && !cx.out_dev && !cx.keep_on_device && !cx.zero_copy && !cx.fold && part.count) {
         CK(cudaMemcpyAsync((uint8_t*)st.out + part.first * cx.R, cx.window_base, part.count * cx.R, cudaMemcpyDeviceToHost, w.s_out));
         STAT_ADD(p, d2h_bytes, part.count * cx.R);
+    }
+    if (copy_window && cx.fold && part.count) {   // the last round: the block's total from its units' partials
+        body_of(st.func_id)->fold(part.d_fold, (part.count + cx.unit - 1) / cx.unit, cx.fold_total, (void*)w.s_out);
+        CK(cudaGetLastError());
     }
     const EmitBlock& e = part.emit;
     if (copy_window && e.host && e.d_values && e.total) {
@@ -1069,7 +1098,8 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
     cx.resilient = (d.flags & FBR_RESILIENT) != 0;
     cx.args_dev = (d.flags & FBR_ARGS_DEVICE) != 0;
     cx.out_dev = (d.flags & FBR_OUT_DEVICE) != 0;
-    cx.keep_on_device = (d.flags & FBR_RESULTS_ON_DEVICE) != 0;
+    cx.fold = (d.flags & FBR_FOLD) != 0;
+    cx.keep_on_device = (d.flags & FBR_RESULTS_ON_DEVICE) != 0 && !cx.fold;
     {
         // Output resident on worker 0, computed by another worker: kernels storing over NVLink stay below what a
         // copy engine pushes at the peer-copy rate (TMA bulk or register stores alike).  So the block is
@@ -1087,7 +1117,8 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
         cx.zero_copy = zc != 0 && body.result_kind == FBR_RES_BITS8 && !cx.out_dev && !cx.resilient && !cx.keep_on_device &&
                        !(d.flags & (FBR_FULL_WINDOW | FBR_SHUFFLE | FBR_VIA_RING | FBR_NO_ZERO_COPY)) && st.out != nullptr;
     }
-    cx.full_window = (cx.out_dev && !cx.peer_out) || cx.resilient || cx.keep_on_device || (d.flags & FBR_FULL_WINDOW) || cx.zero_copy;
+    cx.full_window = (cx.out_dev && !cx.peer_out) || cx.resilient || cx.keep_on_device || (d.flags & FBR_FULL_WINDOW) || cx.zero_copy ||
+                     cx.fold;   // a fold block has no output window: nothing is staged or copied out
     cx.host_args = d.arg_stride != 0 && !cx.args_dev && !cx.resilient;
     {
         // device-resident arguments on worker 0, consumed by another worker: stream them through the staging halves,
@@ -1108,8 +1139,7 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
             cx.host_args = true;       // same wave / staging machinery as host-resident arguments
         }
     }
-    const uint32_t cs = d.chunksize ? d.chunksize : 32u;
-    cx.unit = pick_unit(body, cs, part.count, w.sm_count, p->ring_bytes);
+    cx.unit = pick_unit(body, map_chunksize(d), part.count, w.sm_count, p->ring_bytes);
     cx.slot_stride = (uint32_t)round_up((uint64_t)cx.unit * cx.R, 16);
     const uint32_t unit = cx.unit, R = cx.R;
     if ((body.flags & FBR_BODY_RECORD) && unit > body.unit_tasks)   // a unit must fit the kernel's shared-memory stage
@@ -1254,7 +1284,9 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
     if (!cx.full_window)
         for (int i = 0; i < 2; ++i)
             if (!w.d_out[i]) CK(cudaMalloc((void**)&w.d_out[i], p->ring_bytes));
-    if (cx.full_window) {
+    if (cx.fold) {
+        CK(cudaMallocAsync(&part.d_fold, std::max<uint64_t>(16, (part.count + unit - 1) / unit * R), w.s_in));
+    } else if (cx.full_window) {
         if (cx.out_dev) {
             cx.window_base = (uint8_t*)d.out + part.first * R;
         } else if (cx.zero_copy) {
@@ -1412,8 +1444,7 @@ static void cut_blocks(fbr_pool* p, const BodyEntry& body, const fbr_map_desc_t&
                        const std::vector<int>& workers, uint32_t attempt, std::vector<SeqPart>& out) {
     const int nw = (int)workers.size();
     if (nw == 0 || count == 0) return;
-    const uint32_t cs = d.chunksize ? d.chunksize : 32u;
-    const uint32_t unit = pick_unit(body, cs, (count + nw - 1) / nw, p->workers[workers[0]].sm_count, p->ring_bytes);
+    const uint32_t unit = pick_unit(body, map_chunksize(d), (count + nw - 1) / nw, p->workers[workers[0]].sm_count, p->ring_bytes);
     const uint64_t units_total = (count + unit - 1) / unit;
     const uint64_t units_per = (units_total + nw - 1) / nw;
     for (int i = 0; i < nw; ++i) {
@@ -1457,8 +1488,9 @@ static void on_worker_death(fbr_pool* p, int wi, cudaError_t err) {
         if (!touched) continue;
         // device-resident arguments / outputs of a map live on worker 0
         const bool on_w0 = (st.flags & (FBR_ARGS_DEVICE | FBR_OUT_DEVICE)) != 0;
-        // an emit pass's blocks carry the offsets of the workers that counted them: it is failed, not re-cut
-        if (!(st.flags & FBR_RESILIENT) || live.empty() || (on_w0 && p->workers[0].dead) || st.emit_pass) {
+        // an emit pass's blocks carry the offsets of the workers that counted them, and a fold map's order depends on its
+        // block cut: both are failed, not re-cut
+        if (!(st.flags & FBR_RESILIENT) || live.empty() || (on_w0 && p->workers[0].dead) || st.emit_pass || (st.flags & FBR_FOLD)) {
             st.dead_worker = wi;
             st.dead_error = (int)err;
             continue;
@@ -1531,6 +1563,7 @@ static void free_seq(fbr_pool* p, SeqState& st) {
             if (part.d_item_offs[k]) cudaFreeAsync(part.d_item_offs[k], w.s_in);
         }
         if (part.d_lost) cudaFreeAsync(part.d_lost, w.s_in);
+        if (part.d_fold) cudaFreeAsync(part.d_fold, w.s_in);
         free_emit_block(p, part.worker, part.emit);
         if (part.h_lost) cudaFreeHost(part.h_lost);
         if (part.ctrl_slot >= 0) w.ctrl_free.push_back(part.ctrl_slot);
@@ -1633,6 +1666,14 @@ int fbr_body_emit_info(int func_id, uint32_t* out_bytes) {
     return FBR_OK;
 }
 
+int fbr_body_fold_info(int func_id, void* identity, uint32_t* bytes) {
+    const BodyEntry* bp = body_of(func_id);
+    if (!bytes || !bp) return fail(FBR_EINVAL, "bad func_id %d", func_id);
+    *bytes = (uint32_t)bp->identity.size();
+    if (identity && !bp->identity.empty()) memcpy(identity, bp->identity.data(), bp->identity.size());
+    return FBR_OK;
+}
+
 int fbr_body_lookup(const char* name, int* func_id) {
     if (!name || !func_id) return fail(FBR_EINVAL, "NULL argument");
     for (int f = 0, n = body_count(); f < n; ++f)
@@ -1679,6 +1720,20 @@ static std::string descriptor_error(const fbr_body_module_t* m, const char* modu
         why = "the out size must be 1, 2 or a multiple of 4 up to 4096 bytes";
     } else if (emit && (m->flags & FBR_BODY_SUMMABLE)) {
         why = "an emit body's results cannot be folded on the device (FBR_BODY_SUMMABLE)";
+    }
+    const bool fold = (m->flags & FBR_BODY_FOLD) != 0;
+    if (why) {
+    } else if (fold != (m->fold != nullptr && m->identity != nullptr)) {
+        why = fold ? "sets FBR_BODY_FOLD but its descriptor lacks the fold entry or the identity record"
+                   : "describes a fold entry or an identity record but lacks FBR_BODY_FOLD";
+    } else if (fold && !is_record) {
+        why = "only record bodies fold their maps (FBR_BODY_FOLD)";
+    } else if (fold && emit) {
+        why = "an emit body cannot fold (FBR_BODY_FOLD with FBR_BODY_EMIT)";
+    } else if (fold && (m->flags & FBR_BODY_SUMMABLE)) {
+        why = "a fold body cannot also be FBR_BODY_SUMMABLE";
+    } else if (fold ? m->identity_bytes != m->result_bytes : m->identity_bytes != 0) {
+        why = fold ? "the identity record must be result_bytes long (identity_bytes)" : "describes an identity size but lacks FBR_BODY_FOLD";
     }
     if (why) return strf("module %s: body '%s' %s", module_path, name, why);
     const uint32_t group = m->group_threads;
@@ -1749,6 +1804,10 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
     b.item_bytes[0] = m->item_bytes;
     for (uint32_t k = 1; k < b.item_streams; ++k) b.item_bytes[k] = m->more_item_bytes[k - 1];
     b.out_bytes = m->out_bytes;
+    if (m->flags & FBR_BODY_FOLD) {
+        b.fold = m->fold;
+        b.identity.assign((const uint8_t*)m->identity, (const uint8_t*)m->identity + m->result_bytes);
+    }
     b.launch = m->launch; b.occupancy = m->occupancy;
     b.module = h;
     g_bodies.push_back(b);
@@ -2211,6 +2270,12 @@ static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_ite
     if ((d->flags & FBR_RESILIENT) && (d->flags & FBR_SHUFFLE)) return fail(FBR_EINVAL, "FBR_RESILIENT cannot be combined with FBR_SHUFFLE");
     if ((d->flags & FBR_WANT_SUM) && !(body.flags & FBR_BODY_SUMMABLE))
         return fail(FBR_EINVAL, "body %s results cannot be summed", body.name.c_str());
+    if (d->flags & FBR_FOLD) {
+        if (!(body.flags & FBR_BODY_FOLD)) return fail(FBR_EINVAL, "body %s has no combine(): its maps cannot fold (FBR_FOLD)", body.name.c_str());
+        if (d->out || (d->flags & (FBR_OUT_DEVICE | FBR_WANT_SUM | FBR_NO_ZERO_COPY)))
+            return fail(FBR_EINVAL, "a fold map (FBR_FOLD) of body %s owns its one result record: no out, FBR_OUT_DEVICE, "
+                        "FBR_WANT_SUM or FBR_NO_ZERO_COPY", body.name.c_str());
+    }
 
     // A submission can find out that a worker has died (its context rejects every call): the worker is
     // retired, maps in flight are re-dispatched or failed (on_worker_death) and this map is cut again over
@@ -2235,7 +2300,8 @@ static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_ite
         memset(st->items, 0, sizeof st->items);
         st->n_item_streams = items ? n_streams : 0;
         for (uint32_t k = 0; k < st->n_item_streams; ++k) st->items[k] = items[k];
-        const bool need_segment = !st->out && d->n_tasks && !(d->flags & FBR_RESULTS_ON_DEVICE);
+        const bool fold = (d->flags & FBR_FOLD) != 0;
+        const bool need_segment = !st->out && d->n_tasks && !(d->flags & FBR_RESULTS_ON_DEVICE) && !fold;
         // host allocations fail with the sticky error too once a context of this process has died: tell the two apart
         auto died_meanwhile = [&]() {
             bool any = false;
@@ -2258,6 +2324,14 @@ static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_ite
         // contiguous task blocks per live worker, cut on claim-unit boundaries (block partition ==
         // PUSH round-robin with chunk = block, SURVEY.md 8(e))
         cut_blocks(p, body, *d, 0, d->n_tasks, live, d->attempt, st->parts);
+        if (fold) {
+            // the result record, then each block's total in block order; pinned memory is mapped into every device, where
+            // each block's fold_tree_kernel writes its total
+            int rc = pinned_acquire(p, (1 + st->parts.size()) * (uint64_t)body.result_bytes, &st->out);
+            if (rc != FBR_OK) return rc;
+            st->own_out = true;
+            for (size_t k = 0; k < st->parts.size(); ++k) st->parts[k].cx.fold_total = (uint8_t*)st->out + (1 + k) * body.result_bytes;
+        }
         if (counted) {
             // the emit pass runs over the blocks the count pass counted
             bool same = counted->size() == st->parts.size();
@@ -2328,6 +2402,54 @@ static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_ite
         if (!died) { g_err = msg; return rc; }
     }
     return fail(FBR_ECUDA, "submission kept failing while workers died");
+}
+
+// tree() over n host records of fold body `body` into `out` (host), on the pool's first live worker; blocks until done.
+// The caller holds the pool lock: the work goes to the worker's own s_fold, where nothing else waits, so the wait is one
+// small launch long.  A worker whose context died on the way is retired (on_worker_death), and the fold fails with FBR_ECUDA.
+static int fold_host_records(fbr_pool* p, const BodyEntry& body, const void* values, uint64_t n, void* out) {
+    const uint64_t R = body.result_bytes;
+    if (n <= 1) {   // tree() of no record is the identity, of one record the record
+        memmove(out, n ? values : body.identity.data(), R);
+        return FBR_OK;
+    }
+    int wi = -1;
+    for (size_t i = 0; i < p->workers.size() && wi < 0; ++i)
+        if (!p->workers[i].dead) wi = (int)i;
+    if (wi < 0) return fail(FBR_ECUDA, "every worker of this pool has died");
+    Worker& w = p->workers[wi];
+    uint8_t* d = nullptr;   // the n records, then the result
+    cudaError_t e = cudaSetDevice(w.device);
+    if (e == cudaSuccess) e = cudaMallocAsync((void**)&d, (n + 1) * R, w.s_fold);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d, values, n * R, cudaMemcpyHostToDevice, w.s_fold);
+    if (e == cudaSuccess) {
+        body.fold(d, n, d + n * R, (void*)w.s_fold);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(out, d + n * R, R, cudaMemcpyDeviceToHost, w.s_fold);
+    if (d) cudaFreeAsync(d, w.s_fold);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(w.s_fold);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        cudaError_t why = e;
+        if (worker_context_dead(w, &why)) on_worker_death(p, wi, why);
+        return fail(FBR_ECUDA, "folding %llu records of body %s on worker %d: %s", (unsigned long long)n, body.name.c_str(), wi,
+                    cudaGetErrorString(e));
+    }
+    p->stats.h2d_bytes += n * R;
+    p->stats.d2h_bytes += R;
+    return FBR_OK;
+}
+
+// FBR_FOLD, once every block is done: the map's result record (out) is tree() over the block totals that follow it.  It
+// runs at completion rather than behind a cross-device event on worker 0, so a fold map never makes one worker's stream
+// wait for another's, and a dead worker fails the map before any other device depends on it
+static int fold_finish(fbr_pool* p, SeqState& st) {
+    if (st.folded) return FBR_OK;
+    const BodyEntry& body = *body_of(st.func_id);
+    const int rc = fold_host_records(p, body, (const uint8_t*)st.out + body.result_bytes, st.parts.size(), st.out);
+    st.folded = rc == FBR_OK;
+    return rc;
 }
 
 static void harvest(fbr_pool* p, SeqState& st) {
@@ -2467,6 +2589,10 @@ static int result_wait_locked_out(fbr_pool_t* p, uint64_t seq, int timeout_ms, f
         }
         if (more) continue;
         harvest(p, st);
+        if ((st.flags & FBR_FOLD) && !st.err_code) {
+            const int rc = fold_finish(p, st);
+            if (rc != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc;
+        }
         memset(res, 0, sizeof *res);
         res->seq = seq;
         res->n_tasks = st.n_tasks;
@@ -2544,6 +2670,14 @@ int fbr_result_poll(fbr_pool_t* p, uint64_t seq, uint64_t* n_done) {
         done += part_done;
         if (part_done < part.count) break;
     }
+    if (st.flags & FBR_FOLD) {   // the one result record is there once every block is: 0 tasks done until then
+        if (done < st.n_tasks) {
+            done = 0;
+        } else {
+            const int rc = fold_finish(p, st);
+            if (rc != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc;
+        }
+    }
     *n_done = done;
     return FBR_OK;
 }
@@ -2605,6 +2739,7 @@ int fbr_result_fetch(fbr_pool_t* p, uint64_t seq, uint64_t first, uint64_t count
     auto it = p->seqs.find(seq);
     if (it == p->seqs.end()) return fail(FBR_ENOENT, "unknown seq %llu", (unsigned long long)seq);
     SeqState& st = *it->second;
+    if (st.flags & FBR_FOLD) return fail(FBR_EINVAL, "seq %llu is a fold map: its one result record is fbr_result_t.data", (unsigned long long)seq);
     if (!(st.flags & FBR_RESULTS_ON_DEVICE)) return fail(FBR_EINVAL, "seq %llu does not keep its results on the device", (unsigned long long)seq);
     if (first + count > st.n_tasks) return fail(FBR_EINVAL, "range out of bounds");
     const uint64_t R = st.result_bytes;
@@ -2638,6 +2773,15 @@ int fbr_result_release(fbr_pool_t* p, uint64_t seq) {
     free_seq(p, *it->second);
     p->seqs.erase(it);
     return FBR_OK;
+}
+
+int fbr_fold_values(fbr_pool_t* p, int func_id, const void* values, uint64_t n, void* out) {
+    if (!p || !out || (n && !values)) return fail(FBR_EINVAL, "NULL argument");
+    const BodyEntry* bp = body_of(func_id);
+    if (!bp) return fail(FBR_EINVAL, "bad func_id %d", func_id);
+    if (!(bp->flags & FBR_BODY_FOLD)) return fail(FBR_EINVAL, "body %s has no combine(): it cannot fold", bp->name.c_str());
+    std::lock_guard<std::mutex> g(p->mu);
+    return fold_host_records(p, *bp, values, n, out);
 }
 
 int fbr_host_alloc(fbr_pool_t* p, uint64_t bytes, void** ptr) {

@@ -9,6 +9,7 @@
 //                        epilogue.  Replaces result_conn.send xN + _res_get + Inventory.get
 //                        (fiber/pool.py:814-824, 968-973, 666-679).
 //   payload_fill_kernel : synthetic 4 KB records for BASELINE.json config 4.
+//   fold_tree_kernel   : tree() over a fold body's records (a block's unit partials, block totals).
 //
 // Everything here is HBM-bound byte/integer work (no dense contraction => no tensor cores):
 // 16 B vector accesses, fully coalesced, grids sized as (SM count x resident CTAs).
@@ -109,6 +110,11 @@ struct WaveParams {
     // items record bodies with K = 2 to 4 streams (Items = ItemTypes<...>): streams 1 .. K-1, read like stream 0 above.
     // Appended after every other field, so their offsets stay where one-stream kernels expect them
     ItemStream more_items[kMaxItemStreams - 1];
+    // fold maps of record bodies with combine() (FoldPass): the unit of tasks [first, first + count) writes its tree to
+    // fold_partials + (first - fold_first) / syn_unit * sizeof(Res) -- its place in its block, never its ticket (syn_unit
+    // is a power of two)
+    uint8_t* fold_partials;
+    uint64_t fold_first;        // map index of the block's first task
 };
 
 // Task record of ticket t: from the device task ring, or computed (contiguous wave).
@@ -1163,6 +1169,47 @@ template <class B>
 struct EmitModeOf<B, std::void_t<decltype(B::kEmitValues)>> {
     static constexpr bool kValues = B::kEmitValues;
 };
+// A record body opts into fold maps with `__host__ __device__ static Res identity();` and `__device__ static void
+// combine(Res& acc, const Res& x);` (acc <- acc (+) x, called by one thread; either operand may be in shared or global
+// memory).  A fold map reduces its results with
+//     tree(x[0..c)): while c > 1: x[i] <- combine(x[2i], x[2i+1]) for every i with 2i+1 < c, an odd last element is
+//                    carried to x[c/2]; c <- ceil(c/2)
+// over each block's results in task order, then over the blocks' totals in block order; n = 0 gives identity().  Claim
+// units of a fold map hold a power of two of tasks and start at a multiple of it within their block, so a unit's tree is
+// an aligned subtree of its block's.  Its kernels are instantiated for FoldPass<B>.
+template <class B, class = void>
+struct FoldOf {
+    static constexpr bool kOn = false;
+};
+template <class B>
+struct FoldOf<B, std::void_t<decltype(&B::combine)>> {
+    using Res = typename B::Res;
+    static constexpr bool kOn = true;
+    static_assert(std::is_same<decltype(&B::combine), void (*)(Res&, const Res&)>::value,
+                  "fold bodies: combine is `static void combine(Res& acc, const Res& x)`");
+    static_assert(std::is_same<decltype(B::identity()), Res>::value,
+                  "fold bodies: `__host__ __device__ static Res identity()` is defined next to combine");
+    static_assert(!EmitOf<B>::kOn, "emit bodies cannot fold (combine)");
+    static_assert(std::is_default_constructible<Res>::value, "fold bodies: Res is default-constructible (the fold pass holds "
+                  "results in registers)");
+};
+template <class B>
+struct FoldPass : B {
+    static constexpr bool kFoldPass = true;
+};
+template <class B, class = void>
+struct FoldModeOf {
+    static constexpr bool kOn = false;
+    static constexpr int kCtas = 0;
+};
+template <class B>
+struct FoldModeOf<B, std::void_t<decltype(B::kFoldPass)>> {
+    static constexpr bool kOn = B::kFoldPass;
+    static constexpr int kCtas = sizeof(typename B::Res) > 16 ? 3 : 4;   // resident CTAs the fold pass asks ptxas for
+};
+// records per tile of fold_tree_kernel
+constexpr uint32_t kFoldTile = 512;
+
 // the fixed result record of one task: Res, or the uint64 count / end offset of an emit body
 template <class B>
 using ResultRecord = typename std::conditional<EmitOf<B>::kOn, uint64_t, typename B::Res>::type;
@@ -1346,8 +1393,11 @@ __device__ __forceinline__ void run_unit(const WaveParams& wp, const TaskRecord&
 }
 }  // namespace record
 
+// (a fold pass asks ptxas for 4 resident CTAs, 3 when its Res is over 16 bytes: left to itself ptxas packs it into 32
+// registers and spills, and a 24 B Res held in registers with its shuffled copy spills at the 56 registers of 4 CTAs)
 template <class B, bool kIndex>
-__global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const WaveParams wp) {
+__global__ void __launch_bounds__(record::kThreads, record::FoldModeOf<B>::kCtas)
+    dispatch_record_kernel(const WaveParams wp) {
     using namespace bulk;
     using L = record::Layout<B>;
     constexpr int kIn = record::kInStages, kOut = record::kOutStages;
@@ -1489,16 +1539,73 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
         asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&empty[sg])) : "memory");
         asm volatile("bar.sync 1, %0;" ::"n"(C) : "memory");
 
-        uint8_t* dst = wp.ring + (size_t)t * wp.slot_stride;
-        const uint32_t bytes = rec.count * L::R;
-        const uint32_t nbs = (reinterpret_cast<uintptr_t>(dst) & 15) == 0 ? (bytes & ~15u) : 0u;
-        if (ct == 0) {
-            // one group per unit, empty when the unit's results are all copied by hand (fewer than 16 bytes, or an
-            // unaligned destination): the wait above counts groups, and must count units
-            if (nbs) bulk_store(dst, out, nbs);
-            else asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        if constexpr (record::FoldModeOf<B>::kOn) {
+            // fold pass: the unit's tree in place in its OUT stage -- level s combines x[j] and x[j + s] for every j that
+            // is a multiple of 2s, which is tree()'s pairing, an odd last element staying where it is -- then its
+            // partial at the unit's place in the block.  No bulk group is committed, so the wait above never waits.
+            // Levels 1 and 2 stay within consumer ct's own records 4ct .. 4ct+3 (kMaxUnit = 4 * C), levels 4 .. 64 within
+            // its warp's 128 records, so only the levels from 128 on take a named barrier.  A Res of at most 32 bytes is
+            // folded in registers up to the warp's total (shuffles), which its lane 0 stores back in place of x[128 w].
+            static_assert(record::kMaxUnit == 4 * C, "fold pass: four records per consumer");
+            using Res = typename B::Res;
+            const uint32_t n = rec.count, j0 = 4u * ct;
+            auto x = [&](uint32_t j) -> Res& { return *reinterpret_cast<Res*>(out + (size_t)j * L::R); };
+            if constexpr (sizeof(Res) <= 32) {
+                constexpr uint32_t W = sizeof(Res) / 4;
+                uint32_t w[W] = {};
+                if (j0 < n) {
+                    Res a = x(j0);
+                    if (j0 + 1 < n) B::combine(a, x(j0 + 1));
+                    if (j0 + 3 < n) {
+                        Res b = x(j0 + 2);
+                        B::combine(b, x(j0 + 3));
+                        B::combine(a, b);
+                    } else if (j0 + 2 < n) {
+                        B::combine(a, x(j0 + 2));
+                    }
+                    memcpy(w, &a, sizeof(Res));
+                }
+                for (uint32_t d = 1; d < 32 && 4u * d < n; d <<= 1) {   // level 4d: lane l takes lane l + d's total
+                    uint32_t v[W];
+#pragma unroll
+                    for (uint32_t k = 0; k < W; ++k) v[k] = __shfl_down_sync(0xffffffffu, w[k], d);
+                    if ((ct & (2u * d - 1u)) == 0 && j0 + 4u * d < n) {
+                        Res a, o;
+                        memcpy(&a, w, sizeof(Res));
+                        memcpy(&o, v, sizeof(Res));
+                        B::combine(a, o);
+                        memcpy(w, &a, sizeof(Res));
+                    }
+                }
+                if ((ct & 31u) == 0 && j0 < n) memcpy(&x(j0), w, sizeof(Res));
+            } else {
+                if (j0 + 1 < n) B::combine(x(j0), x(j0 + 1));
+                if (j0 + 3 < n) B::combine(x(j0 + 2), x(j0 + 3));
+                if (j0 + 2 < n) B::combine(x(j0), x(j0 + 2));
+                for (uint32_t s = 4; s < 128 && s < n; s <<= 1) {
+                    __syncwarp();
+                    if (j0 % (2u * s) == 0 && j0 + s < n) B::combine(x(j0), x(j0 + s));
+                }
+            }
+            asm volatile("bar.sync 1, %0;" ::"n"(C) : "memory");
+            for (uint32_t s = 128; s < n; s <<= 1) {
+                for (uint32_t j = ct * 2u * s; j + s < n; j += C * 2u * s) B::combine(x(j), x(j + s));
+                asm volatile("bar.sync 1, %0;" ::"n"(C) : "memory");
+            }
+            // (a fold map's unit is a power of two: a shift, not a 64-bit division)
+            record::coop_copy(wp.fold_partials + ((rec.first - wp.fold_first) >> (__ffs(wp.syn_unit) - 1)) * L::R, out, L::R, ct, C);
+        } else {
+            uint8_t* dst = wp.ring + (size_t)t * wp.slot_stride;
+            const uint32_t bytes = rec.count * L::R;
+            const uint32_t nbs = (reinterpret_cast<uintptr_t>(dst) & 15) == 0 ? (bytes & ~15u) : 0u;
+            if (ct == 0) {
+                // one group per unit, empty when the unit's results are all copied by hand (fewer than 16 bytes, or an
+                // unaligned destination): the wait above counts groups, and must count units
+                if (nbs) bulk_store(dst, out, nbs);
+                else asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+            }
+            if (nbs < bytes) record::coop_copy(dst + nbs, out + nbs, bytes - nbs, ct, C);
         }
-        if (nbs < bytes) record::coop_copy(dst + nbs, out + nbs, bytes - nbs, ct, C);
         if (ct == 0) {
             bool lost = false;
             if constexpr (B::kCanFault) {
@@ -1517,6 +1624,28 @@ __global__ void __launch_bounds__(record::kThreads) dispatch_record_kernel(const
         }
     }
     if (ct == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+}
+
+// fold_tree_kernel: tree() over the n records x[k * stride], k < n, of a fold body.  CTA b folds tile b -- records
+// [b * kFoldTile, (b + 1) * kFoldTile), an aligned subtree of the whole tree -- in place, leaving its total at the tile's
+// first record; the host repeats with stride * kFoldTile over the tile totals, and the launch with a single tile copies
+// the result to dst.  The records are folded where they lie in global memory (L1 / L2 resident), so records up to 32 KB
+// need no shared-memory budget.
+template <class B>
+__global__ void __launch_bounds__(kThreads) fold_tree_kernel(uint8_t* x, uint64_t n, uint64_t stride, uint8_t* dst) {
+    using Res = typename B::Res;
+    constexpr uint32_t T = record::kFoldTile;
+    const uint64_t tiles = (n + T - 1) / T;
+    for (uint64_t b = blockIdx.x; b < tiles; b += gridDim.x) {
+        uint8_t* const base = x + b * T * stride;
+        const uint32_t c = (uint32_t)(n - b * T < T ? n - b * T : T);
+        for (uint32_t s = 1; s < c; s <<= 1) {
+            for (uint32_t j = threadIdx.x * 2u * s; j + s < c; j += kThreads * 2u * s)
+                B::combine(*reinterpret_cast<Res*>(base + j * stride), *reinterpret_cast<const Res*>(base + (j + s) * stride));
+            __syncthreads();
+        }
+        if (tiles == 1) record::coop_copy(dst, base, (uint32_t)sizeof(Res), threadIdx.x, kThreads);
+    }
 }
 
 // ================================================================================================

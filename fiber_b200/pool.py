@@ -307,21 +307,8 @@ class MapResult:
                 return self._result
             self._result = ResultArray(us, np.empty((0,) + us.result_dtype()[1], us.result_dtype()[0]), 0)
             return self._result
-        res = _abi.Result()
+        res = self._engine_wait(timeout)
         eng = self._engine
-        tmo = -1 if timeout is None else int(timeout * 1000)
-        rc = eng.lib.fbr_result_wait(eng.handle, self._seq, tmo, ctypes.byref(res))
-        if rc == _abi.FBR_ETIMEOUT:
-            raise TimeoutError("map %d not finished" % self._seq)
-        if rc == _abi.FBR_ETASK:
-            try:
-                self._raise_task_error(res)
-            except Exception as e:      # noqa: BLE001 -- remembered: later get() calls raise it without touching the engine
-                self._exc = e
-                raise
-        _abi.check(rc)
-        self._keepalive = None
-        self._pool.recv_tasks += self._n if self._n_items is None else self._n_items
         dtype, sub = self._spec.result_dtype()
         # exact, unbounded sum: the device folds the two halves of int64 results separately (nothing wraps)
         dsum = (int(res.sum_hi) * (1 << 32) + int(res.sum_lo)) if (self._flags & _abi.FBR_WANT_SUM) else None
@@ -357,6 +344,25 @@ class MapResult:
             return self._result
         self._result = ResultArray(self._spec, arr, dsum)
         return self._result
+
+    def _engine_wait(self, timeout):
+        """fbr_result_wait for a map of n > 0 tasks: its fbr_result_t, or the map's task error raised."""
+        res = _abi.Result()
+        eng = self._engine
+        tmo = -1 if timeout is None else int(timeout * 1000)
+        rc = eng.lib.fbr_result_wait(eng.handle, self._seq, tmo, ctypes.byref(res))
+        if rc == _abi.FBR_ETIMEOUT:
+            raise TimeoutError("map %d not finished" % self._seq)
+        if rc == _abi.FBR_ETASK:
+            try:
+                self._raise_task_error(res)
+            except Exception as e:      # noqa: BLE001 -- remembered: later get() calls raise it without touching the engine
+                self._exc = e
+                raise
+        _abi.check(rc)
+        self._keepalive = None
+        self._pool.recv_tasks += self._n if self._n_items is None else self._n_items
+        return res
 
     def _emit_result(self, res):
         """End offsets and values of a finished emit map: views of its pinned segments, or fetched from the device."""
@@ -490,6 +496,37 @@ class MapResult:
     def iget_unordered(self):
         # arrival order == ring order; ordered prefixes are a valid "unordered" stream
         return self._iter_ready()
+
+
+def fold_identity(spec):
+    """The identity() record of fold body ``spec`` as bytes (the result of a fold over no tasks)."""
+    lib = _abi.load()
+    nb = ctypes.c_uint32(0)
+    _abi.check(lib.fbr_body_fold_info(spec.func_id, None, ctypes.byref(nb)))
+    buf = ctypes.create_string_buffer(max(1, nb.value))
+    _abi.check(lib.fbr_body_fold_info(spec.func_id, buf, ctypes.byref(nb)))
+    return buf.raw[:nb.value]
+
+
+class FoldResult(MapResult):
+    """Handle of an asynchronous fold (``Pool.fold_async``): ``get()`` returns tree() over the map's results (FBR_FOLD in
+    include/fiber_b200.h), read like one task's result."""
+
+    def _wait(self, timeout=None):
+        if self._exc is not None:
+            raise self._exc
+        if self._result is None:
+            if self._n == 0:
+                raw = fold_identity(self._spec)
+            else:
+                res = self._engine_wait(timeout)
+                raw = ctypes.string_at(res.data, res.result_bytes)
+            self.raw = raw                  # the result record's bytes (process-isolated pools ship them)
+            self._result = (self._spec.unpack_result(raw),)
+        return self._result[0]
+
+    def _iter_ready(self):
+        raise TypeError("%s: a fold has one result, not one per task: use get()" % self._spec.name)
 
 
 class ApplyResult(MapResult):
@@ -821,6 +858,50 @@ class Pool:
 
     def map(self, func, iterable, chunksize=None):
         return self.map_async(func, iterable, chunksize).get()
+
+    # -- folds: a map reduced on the device with the body's combine() ------------------------------------------------
+    def _fold_spec(self, func):
+        spec = self._spec_of(func)
+        if not spec.flags & _abi.FBR_BODY_FOLD:
+            if not spec.flags & _abi.FBR_BODY_RECORD:
+                hint = "thread bodies do not fold; sum(pool.map(f, xs)) sums their results on the device"
+            else:
+                hint = "a record body folds when it defines identity() and combine() next to run()"
+            raise TypeError("%s cannot fold: it has no combine() (%s)" % (spec.name, hint))
+        return spec
+
+    def _fold(self, func, iterable, kind):
+        self._check_running()
+        spec = self._fold_spec(func)
+        if not hasattr(iterable, "__len__"):
+            iterable = list(iterable)
+        self.lazy_start_workers(func)
+        if self._proc is not None:
+            if kind == "starmap" and not isinstance(iterable, registry.Columns):
+                iterable = list(iterable)
+            return self._proc.submit_fold(spec, kind, iterable)
+        if len(iterable) == 0:                     # identity(): nothing to bind or submit
+            r = FoldResult(self, self._engine, spec, 0, 0, None)
+            r._flags = _abi.FBR_FOLD
+            return r
+        enc = spec.encode_map(iterable) if kind == "map" else spec.encode_starmap(iterable)
+        return self._submit(func, enc, _abi.FBR_MAP if kind == "map" else _abi.FBR_STARMAP, 0, cls=FoldResult,
+                            want_sum=False, extra_flags=_abi.FBR_FOLD, spec=spec)
+
+    def fold_async(self, func, iterable):
+        """``functools.reduce(combine, map(func, iterable))`` on the device, in the fixed order tree() of FBR_FOLD
+        (include/fiber_b200.h): a FoldResult.  There is no chunksize, since the order does not depend on one."""
+        return self._fold(func, iterable, "map")
+
+    def fold(self, func, iterable):
+        return self.fold_async(func, iterable).get()
+
+    def starfold_async(self, func, iterable):
+        """``fold_async`` over argument tuples, bound as ``starmap`` binds them."""
+        return self._fold(func, iterable, "starmap")
+
+    def starfold(self, func, iterable):
+        return self.starfold_async(func, iterable).get()
 
     def starmap_async(self, func, iterable, chunksize=None, callback=None, error_callback=None):
         self._check_running()

@@ -138,6 +138,9 @@ def gpu_worker_main(device, conn, results, sys_path, init=None):
         msg = conn.recv()
         if msg is None:
             break
+        if msg[0] == "fold":
+            _fold_totals_in_worker(pool, conn, segments, msg)
+            continue
         _, job, blk, body, kind, chunksize, payload, shm_name, off, attempt, module = msg
         try:
             if module is not None and body not in registry.body_names():
@@ -145,13 +148,18 @@ def gpu_worker_main(device, conn, results, sys_path, init=None):
             f = proxies.get(body) or proxies.setdefault(body, _proxy_for(body))
             items = range(*payload[1]) if payload[0] == "range" else pickle.loads(payload[1])
             pool._attempt = attempt
-            if kind == "starmap":
+            if kind in ("fold", "starfold"):             # the block's total, R bytes
+                res = pool.fold_async(f, items) if kind == "fold" else pool.starfold_async(f, items)
+                res.get()
+                raw = np.frombuffer(res.raw, np.uint8)
+            elif kind == "starmap":
                 res = pool.starmap(f, items, chunksize)
             elif kind == "apply":
                 res = pool.apply_async(f, items[0][0], items[0][1])._wait()
             else:
                 res = pool.map(f, items, chunksize)
-            raw = res.packed if res.packed is not None else np.ascontiguousarray(np.asarray(res)).view(np.uint8).reshape(-1)
+            if kind not in ("fold", "starfold"):
+                raw = res.packed if res.packed is not None else np.ascontiguousarray(np.asarray(res)).view(np.uint8).reshape(-1)
             seg = segments.get(shm_name)
             if seg is None:
                 segments.clear()                                   # one live segment per worker is enough
@@ -175,6 +183,34 @@ def gpu_worker_main(device, conn, results, sys_path, init=None):
     os._exit(0)
 
 
+def _fold_totals_in_worker(pool, conn, segments, msg):
+    """A fold map's last step, in the worker the master picked: the n_blocks totals after the result record in the map's
+    segment, folded in block order by fbr_fold_values into the result record (the segment's first R bytes)."""
+    from fiber_b200 import _abi, registry
+    _, job, n_blocks, body, shm_name, module = msg
+    try:
+        if module is not None and body not in registry.body_names():
+            registry.register_module(body, *module)
+        spec = registry.spec(body)
+        R = spec.result_bytes
+        seg = segments.get(shm_name) or SharedSegment(shm_name)
+        totals = np.array(seg.array[R:(1 + n_blocks) * R])
+        out = np.zeros(R, np.uint8)
+        eng = pool._engine
+        _abi.check(eng.lib.fbr_fold_values(eng.handle, spec.func_id, totals.ctypes.data, n_blocks, out.ctypes.data))
+        seg.array[:R] = out
+        conn.send(("folded", job))
+    except _abi.EngineError as e:
+        if e.status == _abi.FBR_ECUDA:
+            try:
+                conn.send(("dead", job, -1, str(e)))
+            finally:
+                os._exit(3)
+        conn.send(("error", job, -1, "EngineError", str(e)))
+    except (ValueError, TypeError, RuntimeError, KeyError, OSError) as e:
+        conn.send(("error", job, -1, type(e).__name__, str(e)))
+
+
 # ------------------------------------------------------------------------------------------------
 # master side
 # ------------------------------------------------------------------------------------------------
@@ -189,13 +225,15 @@ class _Worker:
 class _Job:
     def __init__(self, jid, body, kind, chunksize, n, result_bytes, bits, blocks, payload_of, module, out_dtype=None):
         self.id, self.body, self.kind, self.chunksize, self.n = jid, body, kind, chunksize, n
+        # fold maps: the segment holds the result record, then each block's total in block order
+        self.fold = kind in ("fold", "starfold")
         self.result_bytes, self.bits = result_bytes, bits
         self.out_dtype = out_dtype                    # emit bodies: the values' dtype (blocks put them in files of their own)
         self.ranges = [(lo, hi) for _, lo, hi, _ in blocks]
         self.blocks = collections.deque(blocks)       # (blk id, lo, hi, attempt)
         self.n_blocks, self.done_blocks = len(blocks), 0
         self.payload_of, self.module = payload_of, module
-        nbytes = ((n + 7) // 8) if bits else n * result_bytes
+        nbytes = ((n + 7) // 8) if bits else ((1 + len(blocks)) * result_bytes if self.fold else n * result_bytes)
         self.shm = SharedSegment("fbr_%d_%d_%d" % (os.getpid(), jid, int(time.time() * 1e6) & 0xFFFFFF), nbytes) if n else None
         self.nbytes = nbytes
         self.sum, self.error = 0, None
@@ -205,7 +243,9 @@ class _Job:
             if out_dtype is not None:
                 weakref.finalize(self, _unlink_values, self.shm.name, len(blocks))
 
-    def offset(self, lo):
+    def offset(self, lo, blk):
+        if self.fold:
+            return (1 + blk) * self.result_bytes
         return lo // 8 if self.bits else lo * self.result_bytes
 
 
@@ -251,6 +291,13 @@ class ProcessResult:
                 raise job.error
             dtype, sub = self._spec.result_dtype()
             total = job.sum if (self._spec.flags & 0x4) else None
+            if job.fold:
+                from .pool import fold_identity
+                raw = bytes(job.shm.array[:job.result_bytes]) if job.n else fold_identity(self._spec)
+                self._result = [self._spec.unpack_result(raw)]
+                if job.shm is not None:
+                    job.shm.release()
+                return self._result[0]
             if job.out_dtype is not None:
                 self._result = self._emit_result()
             elif job.n == 0:
@@ -284,6 +331,7 @@ class ProcessPool:
         self._cv = threading.Condition()
         self._next_job = 0
         self._closing = False
+        self._terminated = False     # terminate(): work still queued is abandoned (close() lets it finish)
         self._thread = None
         self.stats = {"workers_lost": 0, "workers_started": 0, "blocks_dispatched": 0, "blocks_redispatched": 0, "maps": 0}
 
@@ -314,13 +362,23 @@ class ProcessPool:
             time.sleep(0.01)
 
     # -- submission --------------------------------------------------------------------------------------
+    def fold_blocks(self, n):
+        """The task blocks [lo, hi) a map of n tasks is cut into, in block order (a fold map's result is tree() over their
+        totals in this order)."""
+        per = self._block_tasks or max(BLOCK_ALIGN, -(-n // (4 * self._n) // BLOCK_ALIGN) * BLOCK_ALIGN)
+        return [(lo, min(n, lo + per)) for lo in range(0, n, per)]
+
+    def submit_fold(self, spec, kind, items):
+        """A fold map (``kind`` "map" or "starmap"): each block runs ``Pool.fold`` in its worker and places its total;
+        once every block is in, one live worker folds the totals in block order."""
+        return self.submit(spec, None, "fold" if kind == "map" else "starfold", items, 0, single=True)
+
     def submit(self, spec, twin, kind, items, chunksize, single=False):
         """items: a ``range`` or a list/array of per-task items (tuples for starmap)."""
         from . import registry
         n = len(items)
         bits = twin is not None
-        per = self._block_tasks or max(BLOCK_ALIGN, -(-n // (4 * self._n) // BLOCK_ALIGN) * BLOCK_ALIGN)
-        blocks = [(i, lo, min(n, lo + per), 0) for i, lo in enumerate(range(0, n, per))]
+        blocks = [(i, lo, hi, 0) for i, (lo, hi) in enumerate(self.fold_blocks(n))]
         if isinstance(items, range):
             def payload_of(lo, hi, r=items):
                 sub = r[lo:hi]
@@ -408,7 +466,7 @@ class ProcessPool:
                     bid, lo, hi, attempt = job.blocks.popleft()
                     try:
                         w.conn.send(("block", job.id, bid, job.body, job.kind, job.chunksize, job.payload_of(lo, hi), job.shm.name,
-                                     job.offset(lo), attempt, job.module))
+                                     job.offset(lo, bid), attempt, job.module))
                     except (OSError, ValueError):
                         job.blocks.appendleft((bid, lo, hi, attempt))
                         w.block = None
@@ -458,7 +516,66 @@ class ProcessPool:
                     if w.block is not None and w.block[0] is job:
                         inflight -= 1
                     self._on_death(w, dead_reason)
+        if job.fold and job.n and job.error is None:
+            self._fold_totals(job)
         job.event.set()
+
+    def _fold_totals(self, job):
+        """A fold map whose blocks have all placed their totals: one live worker folds them in block order into the result
+        record.  This runs after close() too, like the blocks of queued maps; terminate() abandons it.  A worker that dies
+        meanwhile is replaced and the fold goes to the next live one, as a block would be re-queued: without error_handling
+        the first death fails the map, and MAX_ATTEMPTS deaths fail it in any case.  The map always ends folded or failed."""
+        deaths = 0
+        while job.error is None:
+            if self._terminated:
+                self._fail(job, RuntimeError("map %d: the pool was terminated before its block totals were folded" % job.id))
+                return
+            live = [w for w in self._workers if w.conn is not None and w.proc is not None and w.proc.is_alive()]
+            w = next((w for w in live if w.ready and w.block is None), None)
+            if w is None:
+                if not live and self._closing:                  # a closed pool replaces no worker
+                    self._fail(job, WorkerDied("map %d: no live worker is left to fold its block totals" % job.id))
+                    return
+                self._pump_idle()
+                time.sleep(0.01)
+                continue
+            dead_reason = None
+            try:
+                w.conn.send(("fold", job.id, job.n_blocks, job.body, job.shm.name, job.module))
+            except (OSError, ValueError):
+                dead_reason = "pipe closed"
+            while dead_reason is None:
+                ready = mpc.wait([w.conn, w.proc.sentinel], timeout=0.5)
+                msg = None
+                if w.conn in ready:
+                    try:
+                        msg = w.conn.recv()
+                    except (EOFError, OSError):
+                        dead_reason = "connection lost (exit code %s)" % w.proc.exitcode
+                elif w.proc.sentinel in ready and not w.proc.is_alive():
+                    dead_reason = "process exited with code %s" % w.proc.exitcode
+                if msg is not None and msg[0] == "ready":
+                    w.ready = True
+                elif msg is not None and msg[1] == job.id:
+                    if msg[0] == "folded":
+                        return
+                    if msg[0] == "error":
+                        exc = {"ValueError": ValueError, "TypeError": TypeError}.get(msg[3], RuntimeError)
+                        self._fail(job, exc(msg[4]))
+                        return
+                    if msg[0] == "dead":
+                        dead_reason = msg[3]
+            deaths += 1
+            self._on_death(w, dead_reason)                      # no block of its own: nothing is re-queued
+            if self._terminated:
+                continue
+            if not self._redispatch:
+                self._fail(job, WorkerDied("worker %d (CUDA device %d) died folding the block totals of map %d: %s; the pool was "
+                                           "created without error_handling, so the fold is not sent again"
+                                           % (w.index, w.device, job.id, dead_reason)))
+            elif deaths >= MAX_ATTEMPTS:
+                self._fail(job, WorkerDied("folding the block totals of map %d killed its worker %d times: %s"
+                                           % (job.id, deaths, dead_reason)))
 
     # -- shutdown ----------------------------------------------------------------------------------------
     def close(self):
@@ -467,6 +584,7 @@ class ProcessPool:
             self._cv.notify_all()
 
     def terminate(self):
+        self._terminated = True
         self.close()
         for w in self._workers:
             if w.conn is not None:

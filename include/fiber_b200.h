@@ -84,6 +84,10 @@ typedef enum fbr_result_kind {
                                      (fbr_body_emit_info) instead of a fixed record: result_bytes 8, result kind
                                      FBR_RES_OFFSETS.  Each map runs a count pass, a scan of the counts and an emit pass;
                                      never SUMMABLE, no bit-packed twin */
+#define FBR_BODY_FOLD 0x100u      /* record body with identity() and combine(): its maps may fold their results on the device
+                                     (FBR_FOLD, fbr_fold_values; fbr_body_fold_info).  Set exactly when the module
+                                     descriptor has `fold` and `identity`, with identity_bytes = result_bytes; never
+                                     with EMIT or SUMMABLE */
 
 typedef struct fbr_body_info {
     int32_t func_id;
@@ -136,6 +140,13 @@ typedef struct fbr_body_module {
        every other body */
     uint32_t item_streams;
     uint32_t more_item_bytes[3];
+    /* FBR_BODY_FOLD record bodies: tree() over n >= 1 device records at `values` (overwritten) into the record at `dst`
+       (device-accessible), launched on `cuda_stream` (fold_tree_kernel), and the body's identity() evaluated on the host,
+       identity_bytes (= result_bytes) bytes.  NULL, NULL, 0 (or left out of a hand-written descriptor) for every other
+       body; the fold maps themselves go through `launch` like any map (WaveParams::fold_partials set) */
+    void (*fold)(void* values, uint64_t n, void* dst, void* cuda_stream);
+    const void* identity;
+    uint32_t identity_bytes;
 } fbr_body_module_t;
 typedef const fbr_body_module_t* (*fbr_body_entry_fn)(void);
 int fbr_register_body(const char* name, const char* module_path, const char* entry, int* func_id);
@@ -151,6 +162,9 @@ int fbr_body_items_info(int func_id, uint32_t* item_bytes);
 int fbr_body_items_streams(int func_id, uint32_t* n_streams, uint32_t item_bytes[4]);
 /* Value size of a FBR_BODY_EMIT body (0 for other bodies). */
 int fbr_body_emit_info(int func_id, uint32_t* out_bytes);
+/* Identity record of a FBR_BODY_FOLD body: *bytes = result_bytes, and `identity` (if not NULL) gets that many bytes.
+ * Other bodies: *bytes = 0. */
+int fbr_body_fold_info(int func_id, void* identity, uint32_t* bytes);
 
 /* ---- pool lifecycle -------------------------------------------------------------------------
  * fbr_pool_create   <- ZPool.__init__ (fiber/pool.py:888-943) + worker start
@@ -206,6 +220,18 @@ int fbr_pool_worker_device(fbr_pool_t* pool, int worker, int* device_id);
                                    store small results straight into the pinned segment */
 #define FBR_RESILIENT 0x400u    /* ResilientZPool semantics (fiber/pool.py:1425-1688): a claim unit whose
                                    worker dies (FBR_TASK_FAULT) is re-dispatched until it completes */
+#define FBR_FOLD 0x4000u        /* fold the map's results on the device (FBR_BODY_FOLD bodies): fbr_result_t.data points
+                                   at ONE record of result_bytes, tree() over the totals of the map's non-empty blocks
+                                   in block order, each block's total tree() over its tasks' results in task order:
+                                       tree(x[0..c)): while c > 1: x[i] <- combine(x[2i], x[2i+1]) for every i with
+                                       2i+1 < c, an odd last element is carried to x[c/2]; c <- ceil(c/2)
+                                   and identity() for n_tasks = 0.  Claim units hold a power of two of tasks and start at
+                                   a multiple of it in their block, so the result depends on the block cut only (the
+                                   fold plan of fbr_plan_query), never on chunksize, ring_bytes, waves, FBR_SHUFFLE,
+                                   FBR_VIA_RING or re-dispatched units.  Refused with out, FBR_OUT_DEVICE, FBR_WANT_SUM or
+                                   FBR_NO_ZERO_COPY; FBR_RESULTS_ON_DEVICE changes nothing.  fbr_result_poll reports 0
+                                   tasks done until the whole map is, fbr_result_fetch refuses the map, and a worker
+                                   that dies under it fails it */
 
 typedef struct fbr_map_desc {
     int32_t func_id;
@@ -280,6 +306,13 @@ typedef struct fbr_plan {
 } fbr_plan_t;
 int fbr_plan_query(int func_id, uint64_t n_tasks, uint32_t chunksize, uint64_t ring_bytes, int n_workers,
                    int worker, int sm_count, fbr_plan_t* plan);
+/* chunksize of fbr_plan_query for the plan of a FBR_FOLD map, which takes no chunksize: the record unit rounded down to
+ * a power of two */
+#define FBR_PLAN_FOLD 0xffffffffu
+
+/* tree() (see FBR_FOLD) over n records of result_bytes each of FBR_BODY_FOLD body func_id, from host memory into `out`
+ * (host), on the pool's first live worker; blocks until done.  n = 0 gives identity(). */
+int fbr_fold_values(fbr_pool_t* pool, int func_id, const void* values, uint64_t n, void* out);
 
 /* ---- result collection ----------------------------------------------------------------------
  * fbr_result_wait    <- MapResult.get -> Inventory.get (fiber/pool.py:736-737, 666-679)

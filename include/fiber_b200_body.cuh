@@ -41,8 +41,23 @@
 // shared-memory stage and bulk-stores the unit's results from another, so a large record is never copied into
 // registers.  From Python: fiber_b200.device_body("polar_f64", source=..., entry="polar_entry",
 // args=[("x", "<f8"), ("y", "<f8")], result=[("r2", "<f8"), ("r", "<f8")]) -- the NumPy dtypes describe the
-// two structs byte for byte (INTEGRATION.md).  Record bodies cannot fold sums on the device and have no
-// bit-packed twin.
+// two structs byte for byte (INTEGRATION.md).  Record bodies have no bit-packed twin and no FBR_WANT_SUM; a record body
+// that defines identity() and combine() reduces a whole map to one Res on the device instead (a FOLD body, below).
+//
+// A FOLD record body defines, next to run():
+//
+//     __host__ __device__ static Res identity();                  // the result of a map of no tasks
+//     __device__ static void combine(Res& acc, const Res& x);     // acc <- acc (+) x; one thread; either operand may be
+//                                                                 // in shared or in global memory
+//
+// Res must also be default-constructible (the fold pass holds results in registers).  FBR_EXPORT_RECORD_BODY then sets
+// FBR_BODY_FOLD and exports fold_tree_kernel and identity() (evaluated on the host) with its size.
+// Any record form may fold (head record or range() index, items, broadcast block, group).  Pool.fold(f, xs) returns
+//     tree(x[0..c)): while c > 1: x[i] <- combine(x[2i], x[2i+1]) for every i with 2i+1 < c, an odd last element is
+//                    carried to x[c/2]; c <- ceil(c/2)
+// over each worker block's results in task order, then over the blocks' totals in block order (identity() for no tasks).
+// The order does not depend on chunksize, waves or scheduling, so a float combine gives the same bits on every run of a
+// pool of the same size.  Plain maps of a fold body run exactly as before.
 //
 // A record body may also read one array every task of a map shares (the pool initializer's initargs, or the same array
 // in every task tuple): it declares the array's element type and a shared-memory budget, and run() gets the block
@@ -268,15 +283,57 @@ template <class B>
 int occupancy_emit(int index_mode) {
     return std::min(occupancy_record<fbr::record::EmitPass<B, false>>(index_mode), occupancy_record<fbr::record::EmitPass<B, true>>(index_mode));
 }
+// fold bodies: FoldPass<B> for a fold map (wp.fold_partials set), else the plain kernels.  index_mode bit 1 asks for the
+// fold pass's occupancy, so plain maps keep their own
+template <class B>
+void launch_foldable(const void* wpv, int grid, void* sv) {
+    if (((const fbr::WaveParams*)wpv)->fold_partials != nullptr) launch_record<fbr::record::FoldPass<B>>(wpv, grid, sv);
+    else launch_record<B>(wpv, grid, sv);
+}
+template <class B>
+int occupancy_foldable(int index_mode) {
+    if (index_mode & 2) return occupancy_record<fbr::record::FoldPass<B>>(index_mode & 1);
+    return occupancy_record<B>(index_mode);
+}
+// tree() over n >= 1 device records (overwritten) into dst: fold_tree_kernel over tiles, then over the tile totals
+template <class B>
+void launch_fold(void* values, uint64_t n, void* dst, void* sv) {
+    constexpr uint64_t T = fbr::record::kFoldTile;
+    uint64_t stride = sizeof(typename B::Res);
+    for (;;) {
+        const uint64_t tiles = (n + T - 1) / T;
+        fbr::fold_tree_kernel<B><<<(unsigned)std::min<uint64_t>(tiles, 1u << 16), fbr::kThreads, 0, (cudaStream_t)sv>>>(
+            (uint8_t*)values, n, stride, tiles == 1 ? (uint8_t*)dst : nullptr);
+        if (tiles <= 1) return;
+        n = tiles;
+        stride *= T;
+    }
+}
+template <class B>
+const void* fold_identity() {
+    if constexpr (fbr::record::FoldOf<B>::kOn) {
+        static const typename B::Res id = B::identity();
+        return &id;
+    } else {
+        return nullptr;
+    }
+}
 template <class B>
 constexpr fbr_body_launch_fn record_launch() {
     if constexpr (fbr::record::EmitOf<B>::kOn) return launch_emit<B>;
+    else if constexpr (fbr::record::FoldOf<B>::kOn) return launch_foldable<B>;
     else return launch_record<B>;
 }
 template <class B>
 constexpr fbr_body_occupancy_fn record_occupancy() {
     if constexpr (fbr::record::EmitOf<B>::kOn) return occupancy_emit<B>;
+    else if constexpr (fbr::record::FoldOf<B>::kOn) return occupancy_foldable<B>;
     else return occupancy_record<B>;
+}
+template <class B>
+constexpr void (*record_fold())(void*, uint64_t, void*, void*) {
+    if constexpr (fbr::record::FoldOf<B>::kOn) return launch_fold<B>;
+    else return nullptr;
 }
 template <class B>
 constexpr bool record_body_ok() {
@@ -291,7 +348,8 @@ constexpr bool record_body_ok() {
 template <class B>
 constexpr uint32_t record_flags() {
     return FBR_BODY_RECORD | (fbr::record::BroadcastOf<B>::kOn ? (FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST) : 0u) |
-           (fbr::record::ItemsOf<B>::kOn ? FBR_BODY_ITEMS : 0u) | (fbr::record::EmitOf<B>::kOn ? FBR_BODY_EMIT : 0u);
+           (fbr::record::ItemsOf<B>::kOn ? FBR_BODY_ITEMS : 0u) | (fbr::record::EmitOf<B>::kOn ? FBR_BODY_EMIT : 0u) |
+           (fbr::record::FoldOf<B>::kOn ? FBR_BODY_FOLD : 0u);
 }
 // the descriptor's group_threads: kGroup of a group body, 0 for a one-thread body
 template <class B>
@@ -306,7 +364,8 @@ constexpr uint32_t record_group() {
 // index instantiation would read no arguments).  unit_tasks is the number of tasks whose records fill one shared-memory
 // stage of dispatch_record_kernel.  A body with a Shared type also gets FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST and
 // its element size and staging budget; a body with kGroup gets group_threads = kGroup; a body with an Item type (or an
-// Items = fbr::ItemTypes<...> list) gets FBR_BODY_ITEMS, its item streams and their item sizes.
+// Items = fbr::ItemTypes<...> list) gets FBR_BODY_ITEMS, its item streams and their item sizes; a body with combine() gets
+// FBR_BODY_FOLD, its fold entry (fold_tree_kernel) and its identity().
 #define FBR_EXPORT_RECORD_BODY(Body, body_name, entry, body_flags)                                                \
     static_assert(fbr_body_export::record_body_ok<Body>(), "record body");                                       \
     static_assert((((body_flags) & FBR_BODY_INDEX_ARG) != 0) == Body::kIndexArg,                                 \
@@ -323,7 +382,9 @@ constexpr uint32_t record_group() {
                                             fbr::record::ItemsOf<Body>::kElem, fbr::record::EmitOf<Body>::kElem, \
                                             fbr::record::ItemsOf<Body>::kStreams,                                \
                                             {fbr::record::ItemsOf<Body>::elem(1), fbr::record::ItemsOf<Body>::elem(2), \
-                                             fbr::record::ItemsOf<Body>::elem(3)}};                              \
+                                             fbr::record::ItemsOf<Body>::elem(3)},                               \
+                                            fbr_body_export::record_fold<Body>(), fbr_body_export::fold_identity<Body>(), \
+                                            fbr::record::FoldOf<Body>::kOn ? fbr::record::Layout<Body>::R : 0u};  \
         return &m;                                                                                               \
     }
 
