@@ -22,6 +22,7 @@ FBR_BODY_INDEX_ARG, FBR_BODY_NEEDS_SHARED, FBR_BODY_SUMMABLE, FBR_BODY_INDEX_ONL
     FBR_BODY_ITEMS = 0x1, 0x2, 0x4, 0x8, 0x10, 0x20, 0x40
 FBR_BODY_EMIT = 0x80
 FBR_BODY_FOLD = 0x100
+FBR_BODY_SCAN = 0x200
 FBR_BODY_MODULE_ABI = 4
 MAX_ITEM_STREAMS = 4        # item streams of one items body (fbr_map_submit_items_n)
 # pool flags
@@ -31,6 +32,7 @@ FBR_MAP, FBR_STARMAP, FBR_APPLY = 0x0, 0x1, 0x2
 FBR_ARGS_DEVICE, FBR_OUT_DEVICE, FBR_WANT_SUM, FBR_SHUFFLE, FBR_FULL_WINDOW, FBR_SHARED_HANDLE, FBR_RESILIENT, \
     FBR_RESULTS_ON_DEVICE, FBR_VIA_RING, FBR_NO_ZERO_COPY = 0x10, 0x20, 0x40, 0x80, 0x100, 0x200, 0x400, 0x800, 0x1000, 0x2000
 FBR_FOLD = 0x4000
+FBR_SCAN = 0x8000
 FBR_PLAN_FOLD = 0xFFFFFFFF   # fbr_plan_query's chunksize for the plan of a fold map
 # fbr_task_error
 FBR_TASK_OK, FBR_TASK_OVERFLOW, FBR_TASK_BADARG, FBR_TASK_FAULT = range(4)
@@ -41,6 +43,7 @@ SYMBOLS = [
     "fbr_abi_version", "fbr_last_error", "fbr_device_count",
     "fbr_body_count", "fbr_body_info", "fbr_body_lookup", "fbr_register_body", "fbr_body_shared_info",
     "fbr_body_items_info", "fbr_body_emit_info", "fbr_body_items_streams", "fbr_body_fold_info", "fbr_fold_values",
+    "fbr_scan_values",
     "fbr_pool_create", "fbr_pool_close", "fbr_pool_terminate", "fbr_pool_join", "fbr_pool_destroy",
     "fbr_pool_n_workers", "fbr_pool_worker_device",
     "fbr_map_submit", "fbr_map_submit_items", "fbr_map_submit_items_n", "fbr_shared_put", "fbr_shared_drop", "fbr_plan_query",
@@ -157,6 +160,7 @@ def load():
         "fbr_body_items_streams": (i32, [i32, P(u32), P(u32)]),
         "fbr_body_fold_info": (i32, [i32, vp, P(u32)]),
         "fbr_fold_values": (i32, [vp, i32, vp, u64, vp]),
+        "fbr_scan_values": (i32, [vp, i32, vp, u32, vp, u64]),
         "fbr_pool_create": (i32, [i32, P(i32), u64, u32, P(vp)]),
         "fbr_pool_close": (i32, [vp]),
         "fbr_pool_terminate": (i32, [vp]),

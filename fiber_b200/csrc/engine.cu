@@ -175,6 +175,7 @@ struct BodyEntry {
     uint32_t out_bytes = 0;                                   // FBR_BODY_EMIT record bodies
     void (*fold)(void*, uint64_t, void*, void*) = nullptr;    // FBR_BODY_FOLD record bodies: tree() over device records ...
     std::vector<uint8_t> identity;                            // ... and identity(), result_bytes bytes
+    int (*scan)(void*, uint64_t, int, const void*, uint32_t, void*) = nullptr;   // FBR_BODY_SCAN: prefix folds, wraps
 };
 
 static std::mutex g_body_mu;
@@ -302,6 +303,7 @@ struct PartCtx {                          // constants of one worker's block of 
                                           // unit at its final index (no ring, no task records, no gather launch)
     bool fold = false;                    // FBR_FOLD: each unit writes its tree to d_fold, no result leaves the device
     uint8_t* fold_total = nullptr;        // FBR_FOLD: the block's total, in the map's pinned segment
+    bool scan = false;                    // FBR_SCAN: the block's window becomes its prefix folds after its last round
     const uint8_t* d_shared = nullptr;
     uint8_t* window_base = nullptr;       // device output of a FULL_WINDOW part
     const uint8_t* args_full = nullptr;   // device-resident arguments of the whole map (args_dev / resilient)
@@ -382,6 +384,10 @@ struct SeqState {
     void* values = nullptr;                // emit pass: pinned values segment (host-resident results) ...
     uint64_t n_values = 0;                 // ... and the map's number of values
     bool folded = false;                   // FBR_FOLD: the result record (out) holds tree() over the block totals
+    bool scanned = false;                  // FBR_SCAN: every block after the first is wrapped with its cross-block pieces
+    std::vector<uint8_t> scan_pieces;      // FBR_SCAN, several blocks: every block's pieces, folded before any block is wrapped
+    std::vector<uint64_t> scan_piece_at;   // ... block b's are records scan_piece_at[b] .. scan_piece_at[b + 1] - 1
+    std::vector<cudaEvent_t> scan_done;    // ... and block b's wrap (and D2H copy) once queued on its worker's s_fold
 };
 
 struct SharedBlock {
@@ -705,7 +711,7 @@ static uint32_t pick_unit(const BodyEntry& b, uint32_t chunksize, uint64_t n_tas
 
 // the chunksize a map's units are picked for: a fold map's units ignore it (FBR_PLAN_FOLD)
 static uint32_t map_chunksize(const fbr_map_desc_t& d) {
-    if (d.flags & FBR_FOLD) return FBR_PLAN_FOLD;
+    if (d.flags & (FBR_FOLD | FBR_SCAN)) return FBR_PLAN_FOLD;   // a scan map's block cut is the fold plan's
     return d.chunksize ? d.chunksize : 32u;
 }
 
@@ -1065,7 +1071,14 @@ static int finish_round(fbr_pool* p, SeqState& st, SeqPart& part, bool copy_wind
     // Every block finishes on s_out, behind its copy-outs, even one without any: finishing on the compute stream puts a
     // DMA hop between back-to-back kernels of pipelined maps, which costs them what a blocking map() gains.
     CK(cudaStreamWaitEvent(w.s_out, w.ev_comp[last_rw], 0));
-    if (copy_window && cx.full_window && !cx.out_dev && !cx.keep_on_device && !cx.zero_copy && !cx.fold && part.count) {
+    if (copy_window && cx.scan && part.count) {   // the last round: the block's own prefix folds, in place in its window
+        const cudaError_t e = (cudaError_t)body_of(st.func_id)->scan(cx.window_base, part.count, 1, nullptr, 0, (void*)w.s_out);
+        if (e != cudaSuccess) return fail(FBR_ECUDA, "scan of body %s on worker %d: %s", body_of(st.func_id)->name.c_str(),
+                                          part.worker, cudaGetErrorString(e));
+    }
+    // a scan block after the first keeps its window on the device: scan_finish wraps it there, then copies it out once
+    const bool scan_later = cx.scan && part.first != 0;
+    if (copy_window && cx.full_window && !cx.out_dev && !cx.keep_on_device && !cx.zero_copy && !cx.fold && !scan_later && part.count) {
         CK(cudaMemcpyAsync((uint8_t*)st.out + part.first * cx.R, cx.window_base, part.count * cx.R, cudaMemcpyDeviceToHost, w.s_out));
         STAT_ADD(p, d2h_bytes, part.count * cx.R);
     }
@@ -1099,6 +1112,7 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
     cx.args_dev = (d.flags & FBR_ARGS_DEVICE) != 0;
     cx.out_dev = (d.flags & FBR_OUT_DEVICE) != 0;
     cx.fold = (d.flags & FBR_FOLD) != 0;
+    cx.scan = (d.flags & FBR_SCAN) != 0;
     cx.keep_on_device = (d.flags & FBR_RESULTS_ON_DEVICE) != 0 && !cx.fold;
     {
         // Output resident on worker 0, computed by another worker: kernels storing over NVLink stay below what a
@@ -1118,7 +1132,8 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
                        !(d.flags & (FBR_FULL_WINDOW | FBR_SHUFFLE | FBR_VIA_RING | FBR_NO_ZERO_COPY)) && st.out != nullptr;
     }
     cx.full_window = (cx.out_dev && !cx.peer_out) || cx.resilient || cx.keep_on_device || (d.flags & FBR_FULL_WINDOW) || cx.zero_copy ||
-                     cx.fold;   // a fold block has no output window: nothing is staged or copied out
+                     cx.fold ||   // a fold block has no output window: nothing is staged or copied out
+                     cx.scan;     // a scan block's results are rewritten in place once all of them are there
     cx.host_args = d.arg_stride != 0 && !cx.args_dev && !cx.resilient;
     {
         // device-resident arguments on worker 0, consumed by another worker: stream them through the staging halves,
@@ -1488,9 +1503,9 @@ static void on_worker_death(fbr_pool* p, int wi, cudaError_t err) {
         if (!touched) continue;
         // device-resident arguments / outputs of a map live on worker 0
         const bool on_w0 = (st.flags & (FBR_ARGS_DEVICE | FBR_OUT_DEVICE)) != 0;
-        // an emit pass's blocks carry the offsets of the workers that counted them, and a fold map's order depends on its
-        // block cut: both are failed, not re-cut
-        if (!(st.flags & FBR_RESILIENT) || live.empty() || (on_w0 && p->workers[0].dead) || st.emit_pass || (st.flags & FBR_FOLD)) {
+        // an emit pass's blocks carry the offsets of the workers that counted them, and a fold or scan map's order depends
+        // on its block cut: both are failed, not re-cut
+        if (!(st.flags & FBR_RESILIENT) || live.empty() || (on_w0 && p->workers[0].dead) || st.emit_pass || (st.flags & (FBR_FOLD | FBR_SCAN))) {
             st.dead_worker = wi;
             st.dead_error = (int)err;
             continue;
@@ -1538,6 +1553,11 @@ static void free_emit_block(fbr_pool* p, int worker, EmitBlock& e) {
 }
 
 static void free_seq(fbr_pool* p, SeqState& st) {
+    // a scan map's wraps run on s_fold, its windows are freed on s_in: a wrap still in flight finishes first
+    for (cudaEvent_t ev : st.scan_done)
+        if (ev) { cudaEventSynchronize(ev); cudaEventDestroy(ev); }
+    cudaGetLastError();
+    st.scan_done.clear();
     for (auto& part : st.graveyard)        // device-side resources died with the worker's context
         if (part.h_lost) cudaFreeHost(part.h_lost);
     st.graveyard.clear();
@@ -1735,6 +1755,15 @@ static std::string descriptor_error(const fbr_body_module_t* m, const char* modu
     } else if (fold ? m->identity_bytes != m->result_bytes : m->identity_bytes != 0) {
         why = fold ? "the identity record must be result_bytes long (identity_bytes)" : "describes an identity size but lacks FBR_BODY_FOLD";
     }
+    // `scan` follows identity_bytes: it is read only from a descriptor that sets FBR_BODY_SCAN, so a fold descriptor that
+    // ends before it stays valid
+    const bool scan = (m->flags & FBR_BODY_SCAN) != 0;
+    if (why) {
+    } else if (scan && !fold) {
+        why = "FBR_BODY_SCAN needs FBR_BODY_FOLD (a scan is a running fold)";
+    } else if (scan && m->scan == nullptr) {
+        why = "sets FBR_BODY_SCAN but its descriptor lacks the scan entry";
+    }
     if (why) return strf("module %s: body '%s' %s", module_path, name, why);
     const uint32_t group = m->group_threads;
     if (group > 1 && (group > 32 || (group & (group - 1)) != 0))
@@ -1808,6 +1837,7 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
         b.fold = m->fold;
         b.identity.assign((const uint8_t*)m->identity, (const uint8_t*)m->identity + m->result_bytes);
     }
+    if (m->flags & FBR_BODY_SCAN) b.scan = m->scan;
     b.launch = m->launch; b.occupancy = m->occupancy;
     b.module = h;
     g_bodies.push_back(b);
@@ -2268,6 +2298,17 @@ static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_ite
     if ((d->flags & FBR_RESULTS_ON_DEVICE) && ((d->flags & FBR_OUT_DEVICE) || d->out))
         return fail(FBR_EINVAL, "FBR_RESULTS_ON_DEVICE owns its output buffer: do not pass out / FBR_OUT_DEVICE");
     if ((d->flags & FBR_RESILIENT) && (d->flags & FBR_SHUFFLE)) return fail(FBR_EINVAL, "FBR_RESILIENT cannot be combined with FBR_SHUFFLE");
+    // (before the generic FBR_WANT_SUM check: a scan body is never summable, and the scan map says why)
+    if (d->flags & FBR_SCAN) {
+        if (!(body.flags & FBR_BODY_SCAN))
+            return fail(FBR_EINVAL, "body %s exports no scan entry: its maps cannot return prefix folds (FBR_SCAN needs FBR_BODY_SCAN)", body.name.c_str());
+        if (d->flags & FBR_FOLD) return fail(FBR_EINVAL, "FBR_SCAN returns every prefix of the fold: it cannot be combined with FBR_FOLD");
+        if (d->out || (d->flags & FBR_OUT_DEVICE))
+            return fail(FBR_EINVAL, "a scan map (FBR_SCAN) of body %s owns its result window: no out or FBR_OUT_DEVICE", body.name.c_str());
+        if (d->flags & FBR_WANT_SUM) return fail(FBR_EINVAL, "a scan map (FBR_SCAN) has no sum of its results (FBR_WANT_SUM)");
+        if (d->flags & FBR_NO_ZERO_COPY)
+            return fail(FBR_EINVAL, "a scan map (FBR_SCAN) always stages its results on the device: FBR_NO_ZERO_COPY does not apply");
+    }
     if ((d->flags & FBR_WANT_SUM) && !(body.flags & FBR_BODY_SUMMABLE))
         return fail(FBR_EINVAL, "body %s results cannot be summed", body.name.c_str());
     if (d->flags & FBR_FOLD) {
@@ -2452,6 +2493,146 @@ static int fold_finish(fbr_pool* p, SeqState& st) {
     return rc;
 }
 
+// Wraps n records of scan body `body` with the m host records `pieces`, right-nested (the body's scan entry without its
+// prefix step), on worker wi's s_fold; blocks until done.  `values` is host memory (copied to worker wi and back), or, with
+// on_device, worker wi's own device memory, rewritten in place.  The caller holds the pool lock; a worker whose context
+// died on the way is retired and the wrap fails with FBR_ECUDA, as in fold_host_records.
+static int wrap_records(fbr_pool* p, int wi, const BodyEntry& body, const void* pieces, uint32_t m, void* values, uint64_t n,
+                        bool on_device) {
+    const uint64_t R = body.result_bytes;
+    if (n == 0 || m == 0) return FBR_OK;
+    Worker& w = p->workers[wi];
+    if (w.dead) return fail(FBR_ECUDA, "worker %d died before its block of a scan map was wrapped", wi);
+    uint8_t* d = nullptr;   // the pieces, then (host values) the n records
+    const uint64_t bytes = m * R + (on_device ? 0 : n * R);
+    cudaError_t e = cudaSetDevice(w.device);
+    if (e == cudaSuccess) e = cudaMallocAsync((void**)&d, bytes, w.s_fold);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d, pieces, m * R, cudaMemcpyHostToDevice, w.s_fold);
+    uint8_t* const v = on_device ? (uint8_t*)values : d + m * R;
+    if (e == cudaSuccess && !on_device) e = cudaMemcpyAsync(v, values, n * R, cudaMemcpyHostToDevice, w.s_fold);
+    if (e == cudaSuccess) e = (cudaError_t)body.scan(v, n, 0, d, m, (void*)w.s_fold);
+    if (e == cudaSuccess && !on_device) e = cudaMemcpyAsync(values, v, n * R, cudaMemcpyDeviceToHost, w.s_fold);
+    if (d) cudaFreeAsync(d, w.s_fold);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(w.s_fold);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        cudaError_t why = e;
+        if (worker_context_dead(w, &why)) on_worker_death(p, wi, why);
+        return fail(FBR_ECUDA, "wrapping %llu records of body %s on worker %d: %s", (unsigned long long)n, body.name.c_str(), wi,
+                    cudaGetErrorString(e));
+    }
+    p->stats.h2d_bytes += m * R + (on_device ? 0 : n * R);
+    p->stats.d2h_bytes += on_device ? 0 : n * R;
+    return FBR_OK;
+}
+
+static int first_live_worker(fbr_pool* p) {
+    for (size_t i = 0; i < p->workers.size(); ++i)
+        if (!p->workers[i].dead) return (int)i;
+    return -1;
+}
+
+// FBR_SCAN, once every block is done: each block's window holds its own prefix folds (its last record is its total t_k),
+// and every block but the first is still on its worker's device.  Block b > 0 is wrapped with the pieces G_1 .. G_m of
+// t_0 .. t_{b-1} -- tree() over the aligned power-of-two ranges of block totals given by the set bits of b, largest first
+// -- which gives tree(t_0, ..., t_{b-1}, p_i) (the same identity as within a block, over b + 1 elements).  Like fold_finish
+// it starts at completion, so no worker's stream waits on another device.
+//
+// The caller holds the pool lock.  The first call reads every total (R bytes per block) and folds every block's pieces
+// (a few records) before any block is touched, then queues each block's wrap on its own worker's s_fold: the m pieces go
+// up, the window is wrapped in place, and host results take their one D2H copy into the pinned segment.  Nothing bulk is
+// waited for here: each queued block records st.scan_done[b], which fbr_result_wait waits for outside the lock.  A block is
+// queued once (st.scan_queued), so a call that failed part-way resumes at the first block it had not queued.  *done tells
+// whether every wrap has finished.
+static int scan_finish(fbr_pool* p, SeqState& st, bool* done) {
+    *done = st.scanned;
+    if (st.scanned) return FBR_OK;
+    const BodyEntry& body = *body_of(st.func_id);
+    const uint64_t R = body.result_bytes;
+    const bool on_device = (st.flags & FBR_RESULTS_ON_DEVICE) != 0;
+    std::vector<SeqPart*> blocks;
+    for (auto& part : st.parts) blocks.push_back(&part);
+    std::sort(blocks.begin(), blocks.end(), [](const SeqPart* a, const SeqPart* b) { return a->first < b->first; });
+    const size_t nb = blocks.size();
+    if (nb > 1 && st.scan_piece_at.empty()) {
+        std::vector<uint8_t> totals(nb * R);
+        for (size_t k = 0; k < nb; ++k) {
+            const SeqPart& part = *blocks[k];
+            Worker& w = p->workers[part.worker];
+            if (w.dead) return fail(FBR_ECUDA, "worker %d died before its block of a scan map was wrapped", part.worker);
+            cudaError_t e = cudaSetDevice(w.device);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(&totals[k * R], part.cx.window_base + (part.count - 1) * R, R, cudaMemcpyDeviceToHost, w.s_fold);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(w.s_fold);
+            if (e != cudaSuccess) {
+                cudaGetLastError();
+                cudaError_t why = e;
+                if (worker_context_dead(w, &why)) on_worker_death(p, part.worker, why);
+                return fail(FBR_ECUDA, "reading the total of a scan block on worker %d: %s", part.worker, cudaGetErrorString(e));
+            }
+        }
+        std::vector<uint8_t> pieces;
+        std::vector<uint64_t> at(nb + 1, 0);      // block b's pieces are records at[b] .. at[b + 1] - 1 of `pieces`
+        for (size_t b = 1; b < nb; ++b) {
+            at[b] = pieces.size() / R;
+            for (int k = 63; k >= 0; --k) {
+                if (!((b >> k) & 1)) continue;
+                const uint64_t lo = (b >> (k + 1)) << (k + 1);
+                pieces.resize(pieces.size() + R);
+                const int rc = fold_host_records(p, body, &totals[lo * R], 1ull << k, &pieces[pieces.size() - R]);
+                if (rc != FBR_OK) return rc;
+            }
+        }
+        at[nb] = pieces.size() / R;
+        st.scan_pieces.swap(pieces);
+        st.scan_piece_at.swap(at);
+        st.scan_done.assign(nb, nullptr);
+    }
+    for (size_t b = 1; b < nb; ++b) {
+        if (st.scan_done[b]) continue;            // queued by an earlier call
+        SeqPart& part = *blocks[b];
+        Worker& w = p->workers[part.worker];
+        if (w.dead) return fail(FBR_ECUDA, "worker %d died before its block of a scan map was wrapped", part.worker);
+        const uint32_t m = (uint32_t)(st.scan_piece_at[b + 1] - st.scan_piece_at[b]);
+        uint8_t* d = nullptr;
+        cudaEvent_t ev = nullptr;
+        cudaError_t e = cudaSetDevice(w.device);
+        if (e == cudaSuccess) e = cudaMallocAsync((void**)&d, m * R, w.s_fold);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(d, &st.scan_pieces[st.scan_piece_at[b] * R], m * R, cudaMemcpyHostToDevice, w.s_fold);
+        if (e == cudaSuccess) e = (cudaError_t)body.scan(part.cx.window_base, part.count, 0, d, m, (void*)w.s_fold);
+        if (e == cudaSuccess && !on_device)
+            e = cudaMemcpyAsync((uint8_t*)st.out + part.first * R, part.cx.window_base, part.count * R, cudaMemcpyDeviceToHost, w.s_fold);
+        if (d) cudaFreeAsync(d, w.s_fold);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventRecord(ev, w.s_fold);
+        if (e != cudaSuccess) {
+            if (ev) cudaEventDestroy(ev);
+            cudaGetLastError();
+            cudaError_t why = e;
+            if (worker_context_dead(w, &why)) on_worker_death(p, part.worker, why);
+            return fail(FBR_ECUDA, "wrapping block %zu of a scan map of body %s on worker %d: %s", b, body.name.c_str(), part.worker,
+                        cudaGetErrorString(e));
+        }
+        st.scan_done[b] = ev;
+        p->stats.h2d_bytes += m * R;
+        if (!on_device) p->stats.d2h_bytes += part.count * R;
+    }
+    for (size_t b = 1; b < nb; ++b) {
+        const Worker& w = p->workers[blocks[b]->worker];
+        cudaError_t q = w.dead ? cudaErrorUnknown : cudaSetDevice(w.device);
+        if (q == cudaSuccess) q = cudaEventQuery(st.scan_done[b]);
+        if (q == cudaErrorNotReady) { cudaGetLastError(); return FBR_OK; }
+        if (q != cudaSuccess) {
+            cudaGetLastError();
+            cudaError_t why = q;
+            if (worker_context_dead(p->workers[blocks[b]->worker], &why)) on_worker_death(p, blocks[b]->worker, why);
+            return fail(FBR_ECUDA, "wrapping block %zu of a scan map on worker %d: %s", b, blocks[b]->worker, cudaGetErrorString(q));
+        }
+    }
+    st.scanned = true;
+    *done = true;
+    return FBR_OK;
+}
+
 static void harvest(fbr_pool* p, SeqState& st) {
     if (st.finished) return;
     st.sum = 0;
@@ -2533,6 +2714,13 @@ static int result_wait_locked_out(fbr_pool_t* p, uint64_t seq, int timeout_ms, f
             if (it == p->seqs.end()) return fail(FBR_ENOENT, "unknown seq %llu", (unsigned long long)seq);
             if (it->second->dead_worker >= 0) return dead_map_error(p, *it->second);
             for (auto& part : it->second->parts) evs.push_back({part.worker, p->workers[part.worker].device, part.done});
+            // FBR_SCAN: the wraps of blocks after the first, once queued (scan_done[b] belongs to the b-th block by start)
+            std::vector<const SeqPart*> by_first;
+            for (auto& part : it->second->parts) by_first.push_back(&part);
+            std::sort(by_first.begin(), by_first.end(), [](const SeqPart* a, const SeqPart* b) { return a->first < b->first; });
+            for (size_t b = 1; b < it->second->scan_done.size() && b < by_first.size(); ++b)
+                if (it->second->scan_done[b])
+                    evs.push_back({by_first[b]->worker, p->workers[by_first[b]->worker].device, it->second->scan_done[b]});
         }
         // block outside the pool lock so other threads can keep submitting
         bool again = false;
@@ -2592,6 +2780,12 @@ static int result_wait_locked_out(fbr_pool_t* p, uint64_t seq, int timeout_ms, f
         if ((st.flags & FBR_FOLD) && !st.err_code) {
             const int rc = fold_finish(p, st);
             if (rc != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc;
+        }
+        if ((st.flags & FBR_SCAN) && !st.err_code) {
+            bool scanned = false;
+            const int rc = scan_finish(p, st, &scanned);
+            if (rc != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc;
+            if (!scanned) continue;               // wait for the queued wraps outside the lock
         }
         memset(res, 0, sizeof *res);
         res->seq = seq;
@@ -2678,6 +2872,23 @@ int fbr_result_poll(fbr_pool_t* p, uint64_t seq, uint64_t* n_done) {
             if (rc != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc;
         }
     }
+    if (st.flags & FBR_SCAN) {   // blocks after the first are final once every block is done and wrapped
+        bool all = done >= st.n_tasks;
+        for (size_t pi = 0; pi < st.parts.size() && all; ++pi) {
+            const SeqPart& part = st.parts[pi];
+            const Worker& w = p->workers[part.worker];
+            all = !w.dead && cudaSetDevice(w.device) == cudaSuccess && cudaEventQuery(part.done) == cudaSuccess;
+        }
+        cudaGetLastError();
+        if (!all) {
+            done = 0;
+        } else if (harvest(p, st), !st.err_code) {   // a failed map raises its task error instead
+            bool scanned = false;
+            const int rc = scan_finish(p, st, &scanned);
+            if (rc != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc;
+            if (!scanned) done = 0;
+        }
+    }
     *n_done = done;
     return FBR_OK;
 }
@@ -2743,6 +2954,23 @@ int fbr_result_fetch(fbr_pool_t* p, uint64_t seq, uint64_t first, uint64_t count
     if (!(st.flags & FBR_RESULTS_ON_DEVICE)) return fail(FBR_EINVAL, "seq %llu does not keep its results on the device", (unsigned long long)seq);
     if (first + count > st.n_tasks) return fail(FBR_EINVAL, "range out of bounds");
     const uint64_t R = st.result_bytes;
+    if ((st.flags & FBR_SCAN) && !st.scanned) {   // blocks after the first hold their own prefixes until every block is done
+        if (st.dead_worker >= 0) return dead_map_error(p, st);
+        for (auto& part : st.parts) {
+            CK(cudaSetDevice(p->workers[part.worker].device));
+            CK(cudaEventSynchronize(part.done));
+        }
+        harvest(p, st);
+        if (!st.err_code) {
+            bool scanned = false;
+            const int rc = scan_finish(p, st, &scanned);
+            if (rc != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc;
+            for (size_t b = 1; !scanned && b < st.scan_done.size(); ++b)   // a fetch reads the wrapped window
+                if (st.scan_done[b]) CK(cudaEventSynchronize(st.scan_done[b]));
+            const int rc2 = scanned ? FBR_OK : scan_finish(p, st, &scanned);
+            if (rc2 != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc2;
+        }
+    }
     for (auto& part : st.parts) {
         const uint64_t lo = std::max(first, part.first), hi = std::min(first + count, part.first + part.count);
         if (lo >= hi) continue;
@@ -2782,6 +3010,17 @@ int fbr_fold_values(fbr_pool_t* p, int func_id, const void* values, uint64_t n, 
     if (!(bp->flags & FBR_BODY_FOLD)) return fail(FBR_EINVAL, "body %s has no combine(): it cannot fold", bp->name.c_str());
     std::lock_guard<std::mutex> g(p->mu);
     return fold_host_records(p, *bp, values, n, out);
+}
+
+int fbr_scan_values(fbr_pool_t* p, int func_id, const void* pieces, uint32_t n_pieces, void* values, uint64_t n) {
+    if (!p || (n_pieces && !pieces) || (n && !values)) return fail(FBR_EINVAL, "NULL argument");
+    const BodyEntry* bp = body_of(func_id);
+    if (!bp) return fail(FBR_EINVAL, "bad func_id %d", func_id);
+    if (!(bp->flags & FBR_BODY_SCAN)) return fail(FBR_EINVAL, "body %s exports no scan entry (FBR_BODY_SCAN)", bp->name.c_str());
+    std::lock_guard<std::mutex> g(p->mu);
+    const int wi = first_live_worker(p);
+    if (wi < 0) return fail(FBR_ECUDA, "every worker of this pool has died");
+    return wrap_records(p, wi, *bp, pieces, n_pieces, values, n, false);
 }
 
 int fbr_host_alloc(fbr_pool_t* p, uint64_t bytes, void** ptr) {

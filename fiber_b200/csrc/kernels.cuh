@@ -1649,6 +1649,103 @@ __global__ void __launch_bounds__(kThreads) fold_tree_kernel(uint8_t* x, uint64_
 }
 
 // ================================================================================================
+// Prefix folds of a fold body (FBR_SCAN maps, fbr_scan_values).  y[i] = tree(x[0..i]) is computed without a running
+// carry, whose bracketing would depend on scheduling: with F_1 .. F_k the aligned power-of-two pieces of [0, i) given by
+// the set bits of i, largest first -- each the tree of a complete aligned subtree, so the same bits as tree()'s node --
+//     y[i] = F_1 (+) (F_2 (+) ( ... (+) (F_k (+) x[i])))            (a (+) b = combine(acc = a, b))
+// evaluated innermost first, popcount(i) combines per element.  scan_level_kernel builds one level of the complete
+// subtrees from the level below it (level k holds the n >> k subtrees of 2^k records), scan_wrap_kernel wraps each element.
+// Records of at most kScanRegBytes are combined in registers; larger ones in global memory, through one scratch record
+// per thread, so no record is ever copied to the stack.
+// ================================================================================================
+constexpr uint32_t kScanRegBytes = 32;
+constexpr int kScanMaxLevels = 64;
+struct ScanLevels {
+    const uint8_t* at[kScanMaxLevels];   // at[k]: level k (at[0] unused: level 0 is x itself)
+};
+
+namespace scan_detail {
+// dst <- src, one record of R (a multiple of 4) bytes, by one thread
+__device__ __forceinline__ void copy_record(uint8_t* dst, const uint8_t* src, uint32_t R) {
+#pragma unroll 1
+    for (uint32_t k = 0; k < R; k += 4) *reinterpret_cast<uint32_t*>(dst + k) = *reinterpret_cast<const uint32_t*>(src + k);
+}
+}  // namespace scan_detail
+
+// scan_level_kernel: dst[j] = src[2j] (+) src[2j + 1] for j < n
+template <class B>
+__global__ void __launch_bounds__(kThreads) scan_level_kernel(const uint8_t* src, uint8_t* dst, uint64_t n) {
+    using Res = typename B::Res;
+    constexpr uint32_t R = sizeof(Res);
+    for (uint64_t j = blockIdx.x * (uint64_t)kThreads + threadIdx.x; j < n; j += (uint64_t)gridDim.x * kThreads) {
+        const Res* s = reinterpret_cast<const Res*>(src + 2 * j * R);
+        Res* d = reinterpret_cast<Res*>(dst + j * R);
+        if constexpr (R <= kScanRegBytes) {
+            Res a = s[0];
+            B::combine(a, s[1]);
+            *d = a;
+        } else {
+            scan_detail::copy_record(dst + j * R, src + 2 * j * R, R);
+            B::combine(*d, s[1]);
+        }
+    }
+}
+
+// scan_wrap_kernel: record i of x (n records, rewritten in place) becomes y[i] when `prefix` is set (lv holds levels 1 ..
+// 63 - clz(n)), then is wrapped with the n_pieces records G_1 .. G_m at `pieces`, right-nested:
+// G_1 (+) (G_2 (+) ( ... (+) (G_m (+) y[i]))).  An odd i starts from level 1's node i >> 1, which is x[i - 1] (+) x[i] by
+// the same combine, so no thread reads another thread's element.  `tmp` holds one scratch record per thread of the grid
+// when R > kScanRegBytes.
+template <class B>
+__global__ void __launch_bounds__(kThreads) scan_wrap_kernel(uint8_t* x, uint64_t n, int prefix, const ScanLevels lv,
+                                                             const uint8_t* pieces, uint32_t n_pieces, uint8_t* tmp) {
+    using Res = typename B::Res;
+    constexpr uint32_t R = sizeof(Res);
+    const uint64_t tid = blockIdx.x * (uint64_t)kThreads + threadIdx.x;
+    for (uint64_t i = tid; i < n; i += (uint64_t)gridDim.x * kThreads) {
+        uint8_t* const xi = x + i * R;
+        const uint8_t* cur = xi;                   // where the element's value is so far
+        uint64_t bits = prefix ? i : 0;            // set bits still to wrap
+        if (bits & 1) {
+            cur = lv.at[1] + (i >> 1) * R;
+            bits &= ~1ull;
+        }
+        if constexpr (R <= kScanRegBytes) {
+            Res a = *reinterpret_cast<const Res*>(cur);
+            for (int k = 1; bits; ++k) {
+                if (!((bits >> k) & 1)) continue;
+                bits &= ~(1ull << k);
+                Res b = *reinterpret_cast<const Res*>(lv.at[k] + ((i >> k) - 1) * R);
+                B::combine(b, a);
+                a = b;
+            }
+            for (uint32_t m = n_pieces; m-- > 0;) {
+                Res b = *reinterpret_cast<const Res*>(pieces + (uint64_t)m * R);
+                B::combine(b, a);
+                a = b;
+            }
+            *reinterpret_cast<Res*>(xi) = a;
+        } else {
+            uint8_t* const t = tmp + tid * R;
+            // each step writes F (+) cur to whichever of xi and t does not hold cur
+            auto wrap = [&](const uint8_t* f) {
+                uint8_t* const dst = cur == xi ? t : xi;
+                scan_detail::copy_record(dst, f, R);
+                B::combine(*reinterpret_cast<Res*>(dst), *reinterpret_cast<const Res*>(cur));
+                cur = dst;
+            };
+            for (int k = 1; bits; ++k) {
+                if (!((bits >> k) & 1)) continue;
+                bits &= ~(1ull << k);
+                wrap(lv.at[k] + ((i >> k) - 1) * R);
+            }
+            for (uint32_t m = n_pieces; m-- > 0;) wrap(pieces + (uint64_t)m * R);
+            if (cur != xi) scan_detail::copy_record(xi, cur, R);
+        }
+    }
+}
+
+// ================================================================================================
 // scan_counts_kernel: the emit pass's offsets from the count pass's counts -- offs[i] = counts[0] + ... + counts[i-1] for
 // i = 0 .. n, and *total = offs[n] (mapped pinned memory: the host reads it once the kernel is done).  A single-pass
 // exclusive scan with decoupled look-back: CTAs claim tiles of kScanTile counts by ticket, so tile t only ever waits for

@@ -903,6 +903,46 @@ class Pool:
     def starfold(self, func, iterable):
         return self.starfold_async(func, iterable).get()
 
+    # -- accumulates: every prefix of a fold, on the device ------------------------------------------------------------
+    def _accumulate(self, func, iterable, kind):
+        self._check_running()
+        spec = self._fold_spec(func)
+        if not spec.flags & _abi.FBR_BODY_SCAN:
+            raise TypeError("%s cannot accumulate: its module exports no scan entry (rebuild it with "
+                            "FBR_EXPORT_RECORD_BODY)" % spec.name)
+        if not hasattr(iterable, "__len__"):
+            iterable = list(iterable)
+        self.lazy_start_workers(func)
+        if self._proc is not None:
+            if kind == "starmap" and not isinstance(iterable, registry.Columns):
+                iterable = list(iterable)
+            r = self._proc.submit_accumulate(spec, kind, iterable)
+            self.sent_tasks += len(iterable)
+            return r
+        if len(iterable) == 0:                     # no prefixes: nothing to bind or submit
+            r = MapResult(self, self._engine, spec, 0, 0, None)
+            r._flags = _abi.FBR_SCAN
+            return r
+        enc = spec.encode_map(iterable) if kind == "map" else spec.encode_starmap(iterable)
+        return self._submit(func, enc, _abi.FBR_MAP if kind == "map" else _abi.FBR_STARMAP, 0, want_sum=False,
+                            extra_flags=_abi.FBR_SCAN, spec=spec)
+
+    def accumulate_async(self, func, iterable):
+        """``itertools.accumulate(map(func, iterable), combine)`` on the device: a MapResult whose record i is the fold of
+        results 0 .. i in the order of FBR_SCAN (include/fiber_b200.h) -- on one worker ``fold(func, iterable[:i + 1])``
+        bit for bit, and the last record is always ``fold(func, iterable)``.  There is no chunksize, as for ``fold``."""
+        return self._accumulate(func, iterable, "map")
+
+    def accumulate(self, func, iterable):
+        return self.accumulate_async(func, iterable).get()
+
+    def staraccumulate_async(self, func, iterable):
+        """``accumulate_async`` over argument tuples, bound as ``starmap`` binds them."""
+        return self._accumulate(func, iterable, "starmap")
+
+    def staraccumulate(self, func, iterable):
+        return self.staraccumulate_async(func, iterable).get()
+
     def starmap_async(self, func, iterable, chunksize=None, callback=None, error_callback=None):
         self._check_running()
         if chunksize is None:

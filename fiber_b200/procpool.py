@@ -141,6 +141,9 @@ def gpu_worker_main(device, conn, results, sys_path, init=None):
         if msg[0] == "fold":
             _fold_totals_in_worker(pool, conn, segments, msg)
             continue
+        if msg[0] == "scan":
+            _scan_blocks_in_worker(pool, conn, segments, msg)
+            continue
         _, job, blk, body, kind, chunksize, payload, shm_name, off, attempt, module = msg
         try:
             if module is not None and body not in registry.body_names():
@@ -152,6 +155,8 @@ def gpu_worker_main(device, conn, results, sys_path, init=None):
                 res = pool.fold_async(f, items) if kind == "fold" else pool.starfold_async(f, items)
                 res.get()
                 raw = np.frombuffer(res.raw, np.uint8)
+            elif kind in ("accumulate", "staraccumulate"):   # the block's own prefix folds, placed like a map's results
+                res = pool.accumulate(f, items) if kind == "accumulate" else pool.staraccumulate(f, items)
             elif kind == "starmap":
                 res = pool.starmap(f, items, chunksize)
             elif kind == "apply":
@@ -181,6 +186,55 @@ def gpu_worker_main(device, conn, results, sys_path, init=None):
         except (OverflowError, ValueError, TypeError, RuntimeError, KeyError, OSError) as e:   # OSError: the segment of a failed map is gone
             conn.send(("error", job, blk, type(e).__name__, str(e)))
     os._exit(0)
+
+
+def _scan_pieces(fold, totals, b):
+    """The pieces G_1 .. G_m of block b (largest first): fold(lo, count) over the aligned power-of-two ranges of the block
+    totals before it given by the set bits of b."""
+    return [fold((b >> (k + 1)) << (k + 1), 1 << k) for k in range(b.bit_length() - 1, -1, -1) if (b >> k) & 1]
+
+
+def _scan_blocks_in_worker(pool, conn, segments, msg):
+    """An accumulate map's last step, in the worker the master picked: each listed block b > 0 of the map's segment (its own
+    prefix folds) is wrapped with the pieces of the block totals before it (fbr_fold_values), right-nested
+    (fbr_scan_values).  The totals come from the master, read before any block was wrapped, so a step sent again after a
+    death wraps the blocks still listed exactly as the first attempt would have.  Each block is wrapped in a private copy,
+    placed, and reported ("scanned"), so the master never lists a placed block again."""
+    from fiber_b200 import _abi, registry
+    _, job, ranges, todo, totals, body, shm_name, module = msg
+    try:
+        if module is not None and body not in registry.body_names():
+            registry.register_module(body, *module)
+        spec = registry.spec(body)
+        R = spec.result_bytes
+        seg = segments.get(shm_name) or SharedSegment(shm_name)
+        eng = pool._engine
+        tot = np.frombuffer(totals, np.uint8)
+
+        def fold(lo, count):
+            out = np.zeros(R, np.uint8)
+            src = np.ascontiguousarray(tot[lo * R:(lo + count) * R])
+            _abi.check(eng.lib.fbr_fold_values(eng.handle, spec.func_id, src.ctypes.data, count, out.ctypes.data))
+            return out
+
+        for b in todo:
+            lo, hi = ranges[b]
+            pieces = np.concatenate(_scan_pieces(fold, tot, b))
+            recs = np.array(seg.array[lo * R:hi * R])
+            _abi.check(eng.lib.fbr_scan_values(eng.handle, spec.func_id, pieces.ctypes.data, len(pieces) // R,
+                                               recs.ctypes.data, hi - lo))
+            seg.array[lo * R:hi * R] = recs
+            conn.send(("scanned", job, b))
+        conn.send(("folded", job))
+    except _abi.EngineError as e:
+        if e.status == _abi.FBR_ECUDA:
+            try:
+                conn.send(("dead", job, -1, str(e)))
+            finally:
+                os._exit(3)
+        conn.send(("error", job, -1, "EngineError", str(e)))
+    except (ValueError, TypeError, RuntimeError, KeyError, OSError) as e:
+        conn.send(("error", job, -1, type(e).__name__, str(e)))
 
 
 def _fold_totals_in_worker(pool, conn, segments, msg):
@@ -227,6 +281,10 @@ class _Job:
         self.id, self.body, self.kind, self.chunksize, self.n = jid, body, kind, chunksize, n
         # fold maps: the segment holds the result record, then each block's total in block order
         self.fold = kind in ("fold", "starfold")
+        # accumulate maps: each block places its own prefix folds like a map; blocks after the first are wrapped at the end
+        self.scan = kind in ("accumulate", "staraccumulate")
+        self.scan_wrapped = set()                     # blocks (b > 0) already wrapped and placed
+        self.scan_totals = None                       # every block's total, read once before the first wrap
         self.result_bytes, self.bits = result_bytes, bits
         self.out_dtype = out_dtype                    # emit bodies: the values' dtype (blocks put them in files of their own)
         self.ranges = [(lo, hi) for _, lo, hi, _ in blocks]
@@ -373,6 +431,12 @@ class ProcessPool:
         once every block is in, one live worker folds the totals in block order."""
         return self.submit(spec, None, "fold" if kind == "map" else "starfold", items, 0, single=True)
 
+    def submit_accumulate(self, spec, kind, items):
+        """An accumulate map (``kind`` "map" or "starmap"): each block runs ``Pool.accumulate`` in its worker and places its
+        own prefix folds; once every block is in, one live worker wraps blocks 1, 2, ... with the pieces of the block totals
+        before them, so record i of block b is tree(t_0, ..., t_{b-1}, p_i) over the blocks of ``fold_blocks``."""
+        return self.submit(spec, None, "accumulate" if kind == "map" else "staraccumulate", items, 0)
+
     def submit(self, spec, twin, kind, items, chunksize, single=False):
         """items: a ``range`` or a list/array of per-task items (tuples for starmap)."""
         from . import registry
@@ -516,14 +580,14 @@ class ProcessPool:
                     if w.block is not None and w.block[0] is job:
                         inflight -= 1
                     self._on_death(w, dead_reason)
-        if job.fold and job.n and job.error is None:
+        if (job.fold or (job.scan and job.n_blocks > 1)) and job.n and job.error is None:
             self._fold_totals(job)
         job.event.set()
 
     def _fold_totals(self, job):
         """A fold map whose blocks have all placed their totals: one live worker folds them in block order into the result
-        record.  This runs after close() too, like the blocks of queued maps; terminate() abandons it.  A worker that dies
-        meanwhile is replaced and the fold goes to the next live one, as a block would be re-queued: without error_handling
+        record; an accumulate map's wraps every block after the first (_scan_blocks_in_worker).  This runs after close()
+        too, like the blocks of queued maps; terminate() abandons it.  A worker that dies meanwhile is replaced and the fold goes to the next live one, as a block would be re-queued: without error_handling
         the first death fails the map, and MAX_ATTEMPTS deaths fail it in any case.  The map always ends folded or failed."""
         deaths = 0
         while job.error is None:
@@ -541,7 +605,14 @@ class ProcessPool:
                 continue
             dead_reason = None
             try:
-                w.conn.send(("fold", job.id, job.n_blocks, job.body, job.shm.name, job.module))
+                if job.scan:
+                    R = job.result_bytes
+                    if job.scan_totals is None:
+                        job.scan_totals = b"".join(bytes(job.shm.array[(hi - 1) * R:hi * R]) for _, hi in job.ranges)
+                    todo = [b for b in range(1, job.n_blocks) if b not in job.scan_wrapped]
+                    w.conn.send(("scan", job.id, job.ranges, todo, job.scan_totals, job.body, job.shm.name, job.module))
+                else:
+                    w.conn.send(("fold", job.id, job.n_blocks, job.body, job.shm.name, job.module))
             except (OSError, ValueError):
                 dead_reason = "pipe closed"
             while dead_reason is None:
@@ -557,6 +628,9 @@ class ProcessPool:
                 if msg is not None and msg[0] == "ready":
                     w.ready = True
                 elif msg is not None and msg[1] == job.id:
+                    if msg[0] == "scanned":
+                        job.scan_wrapped.add(msg[2])
+                        continue
                     if msg[0] == "folded":
                         return
                     if msg[0] == "error":

@@ -88,6 +88,10 @@ typedef enum fbr_result_kind {
                                      (FBR_FOLD, fbr_fold_values; fbr_body_fold_info).  Set exactly when the module
                                      descriptor has `fold` and `identity`, with identity_bytes = result_bytes; never
                                      with EMIT or SUMMABLE */
+#define FBR_BODY_SCAN 0x200u      /* FBR_BODY_FOLD body whose descriptor exports `scan`: its maps may return every prefix of
+                                     the fold (FBR_SCAN, fbr_scan_values).  Set exactly when `scan` is exported, and only
+                                     with FBR_BODY_FOLD; `scan` is read only from descriptors that set it, so a fold
+                                     descriptor that ends at identity_bytes stays a valid fold body */
 
 typedef struct fbr_body_info {
     int32_t func_id;
@@ -147,6 +151,12 @@ typedef struct fbr_body_module {
     void (*fold)(void* values, uint64_t n, void* dst, void* cuda_stream);
     const void* identity;
     uint32_t identity_bytes;
+    /* FBR_BODY_SCAN bodies: the n device records at `values` (overwritten) become their prefix folds when `prefix` is
+       set (record i <- tree(values[0..i]), see FBR_SCAN), then each is wrapped with the n_pieces device records at
+       `pieces`, right-nested: pieces[0] (+) (pieces[1] (+) ( ... (+) (pieces[m-1] (+) record))).  Queued on `cuda_stream`
+       (scan_level_kernel, scan_wrap_kernel, and stream-ordered scratch of fewer than n records); returns the launch's
+       cudaError_t.  Left out of (or NULL in) a descriptor without FBR_BODY_SCAN */
+    int (*scan)(void* values, uint64_t n, int prefix, const void* pieces, uint32_t n_pieces, void* cuda_stream);
 } fbr_body_module_t;
 typedef const fbr_body_module_t* (*fbr_body_entry_fn)(void);
 int fbr_register_body(const char* name, const char* module_path, const char* entry, int* func_id);
@@ -232,6 +242,23 @@ int fbr_pool_worker_device(fbr_pool_t* pool, int worker, int* device_id);
                                    FBR_NO_ZERO_COPY; FBR_RESULTS_ON_DEVICE changes nothing.  fbr_result_poll reports 0
                                    tasks done until the whole map is, fbr_result_fetch refuses the map, and a worker
                                    that dies under it fails it */
+#define FBR_SCAN 0x8000u        /* every prefix of the fold (FBR_BODY_SCAN bodies): fbr_result_t.data holds n_tasks
+                                   records, record i the fold of results 0 .. i under the fold plan's block cut.  Task i of
+                                   the b-th non-empty block gets tree(t_0, ..., t_{b-1}, p_i), t_k block k's total and p_i
+                                   tree() over block b's results from its first task to i; on one worker that is
+                                   tree(x[0..i]), bit for bit the FBR_FOLD result of the first i + 1 tasks, and the last
+                                   record is always the FBR_FOLD result.  Record 0 is the first result itself, never
+                                   combine(identity(), x0).  Evaluated without a running carry, as
+                                       y[i] = F_1 (+) (F_2 (+) ( ... (+) (F_k (+) x[i])))
+                                   with F_1 .. F_k the aligned power-of-two pieces of [0, i) given by the set bits of i,
+                                   largest first, each the tree() of a complete aligned subtree (across blocks the same
+                                   form over the block totals, with p_i in place of x[i]).  Independent of chunksize,
+                                   unit size, ring_bytes, waves, FBR_SHUFFLE, FBR_VIA_RING and re-dispatched units.
+                                   Refused with FBR_FOLD, out, FBR_OUT_DEVICE, FBR_WANT_SUM or FBR_NO_ZERO_COPY; allowed
+                                   with FBR_RESULTS_ON_DEVICE (fbr_result_fetch), FBR_RESILIENT and FBR_ARGS_DEVICE.
+                                   Blocks after the first are wrapped once every block is done (from fbr_result_wait,
+                                   fbr_result_poll or fbr_result_fetch), so fbr_result_poll reports 0 tasks done until
+                                   the whole map is, and a worker that dies under it fails it */
 
 typedef struct fbr_map_desc {
     int32_t func_id;
@@ -313,6 +340,12 @@ int fbr_plan_query(int func_id, uint64_t n_tasks, uint32_t chunksize, uint64_t r
 /* tree() (see FBR_FOLD) over n records of result_bytes each of FBR_BODY_FOLD body func_id, from host memory into `out`
  * (host), on the pool's first live worker; blocks until done.  n = 0 gives identity(). */
 int fbr_fold_values(fbr_pool_t* pool, int func_id, const void* values, uint64_t n, void* out);
+/* Wraps the n host records at `values` (result_bytes each, rewritten in place) of FBR_BODY_SCAN body func_id with the
+ * n_pieces host records at `pieces`, right-nested: pieces[0] (+) (pieces[1] (+) ( ... (+) (pieces[n_pieces-1] (+) v))),
+ * on the pool's first live worker; blocks until done.  With pieces G_1 .. G_m the tree() of the aligned power-of-two
+ * ranges of block totals t_0 .. t_{b-1} given by the set bits of b (largest first, fbr_fold_values), this turns block b's
+ * own prefix folds into the FBR_SCAN records of a map cut into blocks elsewhere (process-isolated pools). */
+int fbr_scan_values(fbr_pool_t* pool, int func_id, const void* pieces, uint32_t n_pieces, void* values, uint64_t n);
 
 /* ---- result collection ----------------------------------------------------------------------
  * fbr_result_wait    <- MapResult.get -> Inventory.get (fiber/pool.py:736-737, 666-679)

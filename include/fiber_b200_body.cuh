@@ -59,6 +59,13 @@
 // The order does not depend on chunksize, waves or scheduling, so a float combine gives the same bits on every run of a
 // pool of the same size.  Plain maps of a fold body run exactly as before.
 //
+// A fold body also gets its running fold with no more code (FBR_BODY_SCAN): Pool.accumulate(f, xs) returns n records,
+// record i the fold of results 0 .. i under the same block cut.  On one worker y[i] = tree(x[0..i]), which is
+// Pool.fold(f, xs[:i+1]) bit for bit; on several, task i of block b gets tree(t_0, ..., t_{b-1}, p_i), t_k block k's
+// total and p_i tree() over block b's results up to i, so y[n-1] is Pool.fold(f, xs).  y[0] is the first result itself.
+// It is computed without a running carry: with F_1 .. F_k the aligned power-of-two pieces of [0, i) given by the set bits
+// of i, largest first (each a complete aligned subtree of tree()), y[i] = F_1 (+) (F_2 (+) ( ... (+) (F_k (+) x[i]))).
+//
 // A record body may also read one array every task of a map shares (the pool initializer's initargs, or the same array
 // in every task tuple): it declares the array's element type and a shared-memory budget, and run() gets the block
 // after the result:
@@ -318,6 +325,52 @@ const void* fold_identity() {
         return nullptr;
     }
 }
+// prefix folds of n device records (in place) of a fold body, then wrapped with n_pieces device records, right-nested
+// (scan_level_kernel per level of complete subtrees, then scan_wrap_kernel); returns a cudaError_t.  The levels (fewer
+// than n records) and, for records over kScanRegBytes, one scratch record per thread are allocated on the stream.
+template <class B>
+int launch_scan(void* values, uint64_t n, int prefix, const void* pieces, uint32_t n_pieces, void* sv) {
+    constexpr uint64_t R = sizeof(typename B::Res);
+    const cudaStream_t s = (cudaStream_t)sv;
+    if (n == 0) return (int)cudaSuccess;
+    // this module's own last error: a launch of its other entries has already been reported through the engine's checks
+    (void)cudaGetLastError();
+    uint64_t off[fbr::kScanMaxLevels] = {}, level_records = 0;
+    int levels = 0;   // levels 1 .. levels hold n >> k complete subtrees each
+    if (prefix)
+        for (uint64_t c = n >> 1; c; c >>= 1) {
+            off[++levels] = level_records;
+            level_records += c;
+        }
+    uint64_t grid = std::min<uint64_t>((n + fbr::kThreads - 1) / fbr::kThreads, 4096);
+    if (R > fbr::kScanRegBytes)   // scratch records: at most 64 MiB of them
+        grid = std::min<uint64_t>(grid, std::max<uint64_t>(1, (64ull << 20) / (R * fbr::kThreads)));
+    const uint64_t tmp_bytes = R > fbr::kScanRegBytes ? grid * fbr::kThreads * R : 0;
+    uint8_t* buf = nullptr;
+    cudaError_t e = cudaSuccess;
+    if (level_records * R + tmp_bytes) e = cudaMallocAsync((void**)&buf, level_records * R + tmp_bytes, s);
+    if (e != cudaSuccess) {
+        (void)cudaGetLastError();
+        return (int)e;
+    }
+    fbr::ScanLevels lv{};
+    const uint8_t* src = (const uint8_t*)values;
+    for (int k = 1; k <= levels; ++k) {
+        uint8_t* dst = buf + off[k] * R;
+        const uint64_t c = n >> k;
+        fbr::scan_level_kernel<B><<<(unsigned)std::min<uint64_t>((c + fbr::kThreads - 1) / fbr::kThreads, 4096), fbr::kThreads, 0, s>>>(
+            src, dst, c);
+        lv.at[k] = src = dst;
+        if ((e = cudaGetLastError()) != cudaSuccess) break;
+    }
+    if (e == cudaSuccess) {
+        fbr::scan_wrap_kernel<B><<<(unsigned)grid, fbr::kThreads, 0, s>>>((uint8_t*)values, n, prefix, lv, (const uint8_t*)pieces,
+                                                                          n_pieces, buf ? buf + level_records * R : nullptr);
+        e = cudaGetLastError();
+    }
+    if (buf) cudaFreeAsync(buf, s);
+    return (int)e;
+}
 template <class B>
 constexpr fbr_body_launch_fn record_launch() {
     if constexpr (fbr::record::EmitOf<B>::kOn) return launch_emit<B>;
@@ -336,6 +389,11 @@ constexpr void (*record_fold())(void*, uint64_t, void*, void*) {
     else return nullptr;
 }
 template <class B>
+constexpr int (*record_scan())(void*, uint64_t, int, const void*, uint32_t, void*) {
+    if constexpr (fbr::record::FoldOf<B>::kOn) return launch_scan<B>;
+    else return nullptr;
+}
+template <class B>
 constexpr bool record_body_ok() {
     static_assert(std::is_trivially_copyable<typename B::Arg>::value && std::is_trivially_copyable<typename B::Res>::value,
                   "record bodies: Arg and Res are trivially copyable");
@@ -349,7 +407,7 @@ template <class B>
 constexpr uint32_t record_flags() {
     return FBR_BODY_RECORD | (fbr::record::BroadcastOf<B>::kOn ? (FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST) : 0u) |
            (fbr::record::ItemsOf<B>::kOn ? FBR_BODY_ITEMS : 0u) | (fbr::record::EmitOf<B>::kOn ? FBR_BODY_EMIT : 0u) |
-           (fbr::record::FoldOf<B>::kOn ? FBR_BODY_FOLD : 0u);
+           (fbr::record::FoldOf<B>::kOn ? (FBR_BODY_FOLD | FBR_BODY_SCAN) : 0u);
 }
 // the descriptor's group_threads: kGroup of a group body, 0 for a one-thread body
 template <class B>
@@ -365,7 +423,8 @@ constexpr uint32_t record_group() {
 // stage of dispatch_record_kernel.  A body with a Shared type also gets FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST and
 // its element size and staging budget; a body with kGroup gets group_threads = kGroup; a body with an Item type (or an
 // Items = fbr::ItemTypes<...> list) gets FBR_BODY_ITEMS, its item streams and their item sizes; a body with combine() gets
-// FBR_BODY_FOLD, its fold entry (fold_tree_kernel) and its identity().
+// FBR_BODY_FOLD | FBR_BODY_SCAN, its fold entry (fold_tree_kernel), its identity() and its scan entry (scan_level_kernel,
+// scan_wrap_kernel).
 #define FBR_EXPORT_RECORD_BODY(Body, body_name, entry, body_flags)                                                \
     static_assert(fbr_body_export::record_body_ok<Body>(), "record body");                                       \
     static_assert((((body_flags) & FBR_BODY_INDEX_ARG) != 0) == Body::kIndexArg,                                 \
@@ -384,7 +443,8 @@ constexpr uint32_t record_group() {
                                             {fbr::record::ItemsOf<Body>::elem(1), fbr::record::ItemsOf<Body>::elem(2), \
                                              fbr::record::ItemsOf<Body>::elem(3)},                               \
                                             fbr_body_export::record_fold<Body>(), fbr_body_export::fold_identity<Body>(), \
-                                            fbr::record::FoldOf<Body>::kOn ? fbr::record::Layout<Body>::R : 0u};  \
+                                            fbr::record::FoldOf<Body>::kOn ? fbr::record::Layout<Body>::R : 0u,   \
+                                            fbr_body_export::record_scan<Body>()};                               \
         return &m;                                                                                               \
     }
 
