@@ -247,8 +247,8 @@ struct Worker {
     int sm_count = 0;
     cudaStream_t s_in = nullptr, s_comp = nullptr, s_out = nullptr;
     cudaStream_t s_gath = nullptr;         // higher-priority stream for gathers that overlap the next dispatch
-    cudaStream_t s_fold = nullptr;         // fbr_fold_values and the cross-block fold of fold maps: waited for under the pool lock,
-                                           // so it never queues behind the maps on the other streams
+    cudaStream_t s_fold = nullptr;         // fold_host_records and the wraps of queue_wrap: nothing there queues behind the maps
+                                           // on the other streams, so a wait for it under the pool lock is short
     bool prev_wave_overlap = false;        // the previous wave used only its half of the ring
     cudaStream_t s_push = nullptr;         // a stream of the ROOT worker's device: its copy engine pushes this worker's argument waves
     cudaStream_t s_push2 = nullptr;        // (waves alternate between the two, like the copy-outs)
@@ -383,10 +383,10 @@ struct SeqState {
     bool emit_pass = false;                // the emit pass of an emit map: its blocks carry the offsets their workers counted
     void* values = nullptr;                // emit pass: pinned values segment (host-resident results) ...
     uint64_t n_values = 0;                 // ... and the map's number of values
-    bool folded = false;                   // FBR_FOLD: the result record (out) holds tree() over the block totals
-    bool scanned = false;                  // FBR_SCAN: every block after the first is wrapped with its cross-block pieces
-    std::vector<uint8_t> scan_pieces;      // FBR_SCAN, several blocks: every block's pieces, folded before any block is wrapped
-    std::vector<uint64_t> scan_piece_at;   // ... block b's are records scan_piece_at[b] .. scan_piece_at[b + 1] - 1
+    bool completed = false;                // complete_map is done: the map is harvested, a fold map's result record (out) holds
+                                           // tree() over the block totals, and a scan map's blocks after the first are wrapped
+    std::vector<uint8_t> scan_totals;      // FBR_SCAN, several blocks: every block's total in block order, read before any
+                                           // block is wrapped (the wrap rewrites the record that holds it)
     std::vector<cudaEvent_t> scan_done;    // ... and block b's wrap (and D2H copy) once queued on its worker's s_fold
 };
 
@@ -1454,6 +1454,18 @@ static bool worker_context_dead(Worker& w, cudaError_t* why) {
     return true;
 }
 
+static void on_worker_death(fbr_pool* p, int wi, cudaError_t err);
+
+// After a failed CUDA call on worker wi: clears the error and, if the worker's context died, retires the worker
+// (on_worker_death).  True if it did.
+static bool retire_if_dead(fbr_pool* p, int wi) {
+    cudaGetLastError();
+    cudaError_t why = cudaErrorUnknown;
+    if (!worker_context_dead(p->workers[wi], &why)) return false;
+    on_worker_death(p, wi, why);
+    return true;
+}
+
 // contiguous, claim-unit aligned sub-blocks of tasks [first, first + count) over `workers`
 static void cut_blocks(fbr_pool* p, const BodyEntry& body, const fbr_map_desc_t& d, uint64_t first, uint64_t count,
                        const std::vector<int>& workers, uint32_t attempt, std::vector<SeqPart>& out) {
@@ -1473,6 +1485,14 @@ static void cut_blocks(fbr_pool* p, const BodyEntry& body, const fbr_map_desc_t&
         part.attempt = attempt;
         out.push_back(std::move(part));
     }
+}
+
+// a map's blocks in task order
+static std::vector<SeqPart*> parts_in_order(SeqState& st) {
+    std::vector<SeqPart*> v;
+    for (auto& part : st.parts) v.push_back(&part);
+    std::sort(v.begin(), v.end(), [](const SeqPart* a, const SeqPart* b) { return a->first < b->first; });
+    return v;
 }
 
 static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& body);
@@ -1525,9 +1545,7 @@ static void on_worker_death(fbr_pool* p, int wi, cudaError_t err) {
             const int pw = part.worker;
             if (p->workers[pw].dead) continue;            // re-cut by a nested call below
             if (submit_part(p, st, part, body) != FBR_OK) {
-                cudaError_t why = cudaSuccess;
-                if (worker_context_dead(p->workers[pw], &why)) {
-                    on_worker_death(p, pw, why);          // a survivor turned out dead as well: cut again (st.parts changes)
+                if (retire_if_dead(p, pw)) {              // a survivor turned out dead as well: cut again (st.parts changes)
                     i = (size_t)-1;                       // restart: submit whatever is still unsubmitted
                     if (st.dead_worker >= 0) break;
                 } else {
@@ -2099,9 +2117,7 @@ static int emit_scan(fbr_pool_t* p, uint64_t cseq, bool host_offs, std::vector<S
     std::lock_guard<std::mutex> g(p->mu);
     auto it = p->seqs.find(cseq);
     if (it == p->seqs.end()) return fail(FBR_ENOENT, "count pass of an emit map was released");
-    std::vector<const SeqPart*> parts;
-    for (auto& part : it->second->parts) parts.push_back(&part);
-    std::sort(parts.begin(), parts.end(), [](const SeqPart* a, const SeqPart* b) { return a->first < b->first; });
+    const std::vector<SeqPart*> parts = parts_in_order(*it->second);
     // one total per block, written by its scan into pinned memory (mapped into every device's address space)
     int rc = pinned_acquire(p, sizeof(uint64_t) * std::max<size_t>(1, parts.size()), (void**)totals);
     if (rc != FBR_OK) return rc;
@@ -2346,10 +2362,7 @@ static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_ite
         // host allocations fail with the sticky error too once a context of this process has died: tell the two apart
         auto died_meanwhile = [&]() {
             bool any = false;
-            for (int wi : live) {
-                cudaError_t why = cudaSuccess;
-                if (worker_context_dead(p->workers[wi], &why)) { on_worker_death(p, wi, why); any = true; }
-            }
+            for (int wi : live) any |= retire_if_dead(p, wi);
             return any;
         };
         if (need_segment && live.size() == 1) {
@@ -2436,17 +2449,21 @@ static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_ite
             return FBR_OK;
         }
         const std::string msg = g_err;
-        cudaError_t why = cudaSuccess;
-        const bool died = worker_context_dead(p->workers[failed_worker], &why);
-        if (died) on_worker_death(p, failed_worker, why);   // before free_seq: its parts on that worker are skipped
+        const bool died = retire_if_dead(p, failed_worker);   // before free_seq: its parts on that worker are skipped
         free_seq(p, *st);
         if (!died) { g_err = msg; return rc; }
     }
     return fail(FBR_ECUDA, "submission kept failing while workers died");
 }
 
+static int first_live_worker(fbr_pool* p) {
+    for (size_t i = 0; i < p->workers.size(); ++i)
+        if (!p->workers[i].dead) return (int)i;
+    return -1;
+}
+
 // tree() over n host records of fold body `body` into `out` (host), on the pool's first live worker; blocks until done.
-// The caller holds the pool lock: the work goes to the worker's own s_fold, where nothing else waits, so the wait is one
+// The caller holds the pool lock: the work goes to the worker's own s_fold, where no map's waves queue, so the wait is one
 // small launch long.  A worker whose context died on the way is retired (on_worker_death), and the fold fails with FBR_ECUDA.
 static int fold_host_records(fbr_pool* p, const BodyEntry& body, const void* values, uint64_t n, void* out) {
     const uint64_t R = body.result_bytes;
@@ -2454,9 +2471,7 @@ static int fold_host_records(fbr_pool* p, const BodyEntry& body, const void* val
         memmove(out, n ? values : body.identity.data(), R);
         return FBR_OK;
     }
-    int wi = -1;
-    for (size_t i = 0; i < p->workers.size() && wi < 0; ++i)
-        if (!p->workers[i].dead) wi = (int)i;
+    const int wi = first_live_worker(p);
     if (wi < 0) return fail(FBR_ECUDA, "every worker of this pool has died");
     Worker& w = p->workers[wi];
     uint8_t* d = nullptr;   // the n records, then the result
@@ -2471,9 +2486,7 @@ static int fold_host_records(fbr_pool* p, const BodyEntry& body, const void* val
     if (d) cudaFreeAsync(d, w.s_fold);
     if (e == cudaSuccess) e = cudaStreamSynchronize(w.s_fold);
     if (e != cudaSuccess) {
-        cudaGetLastError();
-        cudaError_t why = e;
-        if (worker_context_dead(w, &why)) on_worker_death(p, wi, why);
+        retire_if_dead(p, wi);
         return fail(FBR_ECUDA, "folding %llu records of body %s on worker %d: %s", (unsigned long long)n, body.name.c_str(), wi,
                     cudaGetErrorString(e));
     }
@@ -2482,79 +2495,46 @@ static int fold_host_records(fbr_pool* p, const BodyEntry& body, const void* val
     return FBR_OK;
 }
 
-// FBR_FOLD, once every block is done: the map's result record (out) is tree() over the block totals that follow it.  It
-// runs at completion rather than behind a cross-device event on worker 0, so a fold map never makes one worker's stream
-// wait for another's, and a dead worker fails the map before any other device depends on it
-static int fold_finish(fbr_pool* p, SeqState& st) {
-    if (st.folded) return FBR_OK;
-    const BodyEntry& body = *body_of(st.func_id);
-    const int rc = fold_host_records(p, body, (const uint8_t*)st.out + body.result_bytes, st.parts.size(), st.out);
-    st.folded = rc == FBR_OK;
-    return rc;
-}
-
-// Wraps n records of scan body `body` with the m host records `pieces`, right-nested (the body's scan entry without its
-// prefix step), on worker wi's s_fold; blocks until done.  `values` is host memory (copied to worker wi and back), or, with
-// on_device, worker wi's own device memory, rewritten in place.  The caller holds the pool lock; a worker whose context
-// died on the way is retired and the wrap fails with FBR_ECUDA, as in fold_host_records.
-static int wrap_records(fbr_pool* p, int wi, const BodyEntry& body, const void* pieces, uint32_t m, void* values, uint64_t n,
-                        bool on_device) {
+// Queues on worker w's s_fold the wrap of the n records at `values` (w's device memory, rewritten in place) with the m host
+// records `pieces`, right-nested: the body's scan entry without its prefix step.  With `host`, the wrapped records are then
+// copied there; with `done`, an event is created there and recorded behind it all.  Nothing is waited for, but an upload
+// from pageable memory is staged before it returns, so pageable `pieces` may be freed then.
+static cudaError_t queue_wrap(Worker& w, const BodyEntry& body, const void* pieces, uint32_t m, uint8_t* values, uint64_t n,
+                              void* host, cudaEvent_t* done) {
     const uint64_t R = body.result_bytes;
-    if (n == 0 || m == 0) return FBR_OK;
-    Worker& w = p->workers[wi];
-    if (w.dead) return fail(FBR_ECUDA, "worker %d died before its block of a scan map was wrapped", wi);
-    uint8_t* d = nullptr;   // the pieces, then (host values) the n records
-    const uint64_t bytes = m * R + (on_device ? 0 : n * R);
+    uint8_t* d = nullptr;
     cudaError_t e = cudaSetDevice(w.device);
-    if (e == cudaSuccess) e = cudaMallocAsync((void**)&d, bytes, w.s_fold);
+    if (e == cudaSuccess) e = cudaMallocAsync((void**)&d, m * R, w.s_fold);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d, pieces, m * R, cudaMemcpyHostToDevice, w.s_fold);
-    uint8_t* const v = on_device ? (uint8_t*)values : d + m * R;
-    if (e == cudaSuccess && !on_device) e = cudaMemcpyAsync(v, values, n * R, cudaMemcpyHostToDevice, w.s_fold);
-    if (e == cudaSuccess) e = (cudaError_t)body.scan(v, n, 0, d, m, (void*)w.s_fold);
-    if (e == cudaSuccess && !on_device) e = cudaMemcpyAsync(values, v, n * R, cudaMemcpyDeviceToHost, w.s_fold);
+    if (e == cudaSuccess) e = (cudaError_t)body.scan(values, n, 0, d, m, (void*)w.s_fold);
+    if (e == cudaSuccess && host) e = cudaMemcpyAsync(host, values, n * R, cudaMemcpyDeviceToHost, w.s_fold);
     if (d) cudaFreeAsync(d, w.s_fold);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(w.s_fold);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        cudaError_t why = e;
-        if (worker_context_dead(w, &why)) on_worker_death(p, wi, why);
-        return fail(FBR_ECUDA, "wrapping %llu records of body %s on worker %d: %s", (unsigned long long)n, body.name.c_str(), wi,
-                    cudaGetErrorString(e));
-    }
-    p->stats.h2d_bytes += m * R + (on_device ? 0 : n * R);
-    p->stats.d2h_bytes += on_device ? 0 : n * R;
-    return FBR_OK;
-}
-
-static int first_live_worker(fbr_pool* p) {
-    for (size_t i = 0; i < p->workers.size(); ++i)
-        if (!p->workers[i].dead) return (int)i;
-    return -1;
+    cudaEvent_t ev = nullptr;
+    if (e == cudaSuccess && done) e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+    if (e == cudaSuccess && done) e = cudaEventRecord(ev, w.s_fold);
+    if (e == cudaSuccess && done) *done = ev;
+    else if (ev) cudaEventDestroy(ev);
+    return e;
 }
 
 // FBR_SCAN, once every block is done: each block's window holds its own prefix folds (its last record is its total t_k),
 // and every block but the first is still on its worker's device.  Block b > 0 is wrapped with the pieces G_1 .. G_m of
 // t_0 .. t_{b-1} -- tree() over the aligned power-of-two ranges of block totals given by the set bits of b, largest first
-// -- which gives tree(t_0, ..., t_{b-1}, p_i) (the same identity as within a block, over b + 1 elements).  Like fold_finish
-// it starts at completion, so no worker's stream waits on another device.
+// -- which gives tree(t_0, ..., t_{b-1}, p_i) (the same identity as within a block, over b + 1 elements).
 //
-// The caller holds the pool lock.  The first call reads every total (R bytes per block) and folds every block's pieces
-// (a few records) before any block is touched, then queues each block's wrap on its own worker's s_fold: the m pieces go
-// up, the window is wrapped in place, and host results take their one D2H copy into the pinned segment.  Nothing bulk is
-// waited for here: each queued block records st.scan_done[b], which fbr_result_wait waits for outside the lock.  A block is
-// queued once (st.scan_queued), so a call that failed part-way resumes at the first block it had not queued.  *done tells
-// whether every wrap has finished.
-static int scan_finish(fbr_pool* p, SeqState& st, bool* done) {
-    *done = st.scanned;
-    if (st.scanned) return FBR_OK;
+// The caller holds the pool lock.  The first call reads every block's total into st.scan_totals (R bytes per block)
+// before any block is wrapped: a wrap rewrites the record that holds its block's total.  Then, block by block, the pieces
+// are folded from those totals and the wrap is queued on the block's own worker's s_fold (queue_wrap), host results with
+// their one D2H copy into the pinned segment, behind the event st.scan_done[b].  A call that failed part-way resumes at the
+// first block without one and folds the same pieces from the kept totals.  With `block` the wraps are waited for here;
+// otherwise *ready tells whether they have all finished (fbr_result_wait waits for them outside the lock).
+static int scan_finish(fbr_pool* p, SeqState& st, bool block, bool* ready) {
     const BodyEntry& body = *body_of(st.func_id);
     const uint64_t R = body.result_bytes;
     const bool on_device = (st.flags & FBR_RESULTS_ON_DEVICE) != 0;
-    std::vector<SeqPart*> blocks;
-    for (auto& part : st.parts) blocks.push_back(&part);
-    std::sort(blocks.begin(), blocks.end(), [](const SeqPart* a, const SeqPart* b) { return a->first < b->first; });
+    const std::vector<SeqPart*> blocks = parts_in_order(st);
     const size_t nb = blocks.size();
-    if (nb > 1 && st.scan_piece_at.empty()) {
+    if (nb > 1 && st.scan_totals.empty()) {
         std::vector<uint8_t> totals(nb * R);
         for (size_t k = 0; k < nb; ++k) {
             const SeqPart& part = *blocks[k];
@@ -2564,27 +2544,11 @@ static int scan_finish(fbr_pool* p, SeqState& st, bool* done) {
             if (e == cudaSuccess) e = cudaMemcpyAsync(&totals[k * R], part.cx.window_base + (part.count - 1) * R, R, cudaMemcpyDeviceToHost, w.s_fold);
             if (e == cudaSuccess) e = cudaStreamSynchronize(w.s_fold);
             if (e != cudaSuccess) {
-                cudaGetLastError();
-                cudaError_t why = e;
-                if (worker_context_dead(w, &why)) on_worker_death(p, part.worker, why);
+                retire_if_dead(p, part.worker);
                 return fail(FBR_ECUDA, "reading the total of a scan block on worker %d: %s", part.worker, cudaGetErrorString(e));
             }
         }
-        std::vector<uint8_t> pieces;
-        std::vector<uint64_t> at(nb + 1, 0);      // block b's pieces are records at[b] .. at[b + 1] - 1 of `pieces`
-        for (size_t b = 1; b < nb; ++b) {
-            at[b] = pieces.size() / R;
-            for (int k = 63; k >= 0; --k) {
-                if (!((b >> k) & 1)) continue;
-                const uint64_t lo = (b >> (k + 1)) << (k + 1);
-                pieces.resize(pieces.size() + R);
-                const int rc = fold_host_records(p, body, &totals[lo * R], 1ull << k, &pieces[pieces.size() - R]);
-                if (rc != FBR_OK) return rc;
-            }
-        }
-        at[nb] = pieces.size() / R;
-        st.scan_pieces.swap(pieces);
-        st.scan_piece_at.swap(at);
+        st.scan_totals.swap(totals);
         st.scan_done.assign(nb, nullptr);
     }
     for (size_t b = 1; b < nb; ++b) {
@@ -2592,44 +2556,36 @@ static int scan_finish(fbr_pool* p, SeqState& st, bool* done) {
         SeqPart& part = *blocks[b];
         Worker& w = p->workers[part.worker];
         if (w.dead) return fail(FBR_ECUDA, "worker %d died before its block of a scan map was wrapped", part.worker);
-        const uint32_t m = (uint32_t)(st.scan_piece_at[b + 1] - st.scan_piece_at[b]);
-        uint8_t* d = nullptr;
-        cudaEvent_t ev = nullptr;
-        cudaError_t e = cudaSetDevice(w.device);
-        if (e == cudaSuccess) e = cudaMallocAsync((void**)&d, m * R, w.s_fold);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d, &st.scan_pieces[st.scan_piece_at[b] * R], m * R, cudaMemcpyHostToDevice, w.s_fold);
-        if (e == cudaSuccess) e = (cudaError_t)body.scan(part.cx.window_base, part.count, 0, d, m, (void*)w.s_fold);
-        if (e == cudaSuccess && !on_device)
-            e = cudaMemcpyAsync((uint8_t*)st.out + part.first * R, part.cx.window_base, part.count * R, cudaMemcpyDeviceToHost, w.s_fold);
-        if (d) cudaFreeAsync(d, w.s_fold);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventRecord(ev, w.s_fold);
+        std::vector<uint8_t> pieces;
+        for (int k = 63; k >= 0; --k) {
+            if (!((b >> k) & 1)) continue;
+            const uint64_t lo = (b >> (k + 1)) << (k + 1);
+            pieces.resize(pieces.size() + R);
+            const int rc = fold_host_records(p, body, &st.scan_totals[lo * R], 1ull << k, &pieces[pieces.size() - R]);
+            if (rc != FBR_OK) return rc;
+        }
+        const uint32_t m = (uint32_t)(pieces.size() / R);
+        uint8_t* const host = on_device ? nullptr : (uint8_t*)st.out + part.first * R;
+        const cudaError_t e = queue_wrap(w, body, pieces.data(), m, part.cx.window_base, part.count, host, &st.scan_done[b]);
         if (e != cudaSuccess) {
-            if (ev) cudaEventDestroy(ev);
-            cudaGetLastError();
-            cudaError_t why = e;
-            if (worker_context_dead(w, &why)) on_worker_death(p, part.worker, why);
+            retire_if_dead(p, part.worker);
             return fail(FBR_ECUDA, "wrapping block %zu of a scan map of body %s on worker %d: %s", b, body.name.c_str(), part.worker,
                         cudaGetErrorString(e));
         }
-        st.scan_done[b] = ev;
         p->stats.h2d_bytes += m * R;
-        if (!on_device) p->stats.d2h_bytes += part.count * R;
+        if (host) p->stats.d2h_bytes += part.count * R;
     }
     for (size_t b = 1; b < nb; ++b) {
-        const Worker& w = p->workers[blocks[b]->worker];
-        cudaError_t q = w.dead ? cudaErrorUnknown : cudaSetDevice(w.device);
-        if (q == cudaSuccess) q = cudaEventQuery(st.scan_done[b]);
-        if (q == cudaErrorNotReady) { cudaGetLastError(); return FBR_OK; }
+        const int wi = blocks[b]->worker;
+        cudaError_t q = p->workers[wi].dead ? cudaErrorUnknown : cudaSetDevice(p->workers[wi].device);
+        if (q == cudaSuccess) q = block ? cudaEventSynchronize(st.scan_done[b]) : cudaEventQuery(st.scan_done[b]);
+        if (q == cudaErrorNotReady) { cudaGetLastError(); *ready = false; return FBR_OK; }
         if (q != cudaSuccess) {
-            cudaGetLastError();
-            cudaError_t why = q;
-            if (worker_context_dead(p->workers[blocks[b]->worker], &why)) on_worker_death(p, blocks[b]->worker, why);
-            return fail(FBR_ECUDA, "wrapping block %zu of a scan map on worker %d: %s", b, blocks[b]->worker, cudaGetErrorString(q));
+            retire_if_dead(p, wi);
+            return fail(FBR_ECUDA, "wrapping block %zu of a scan map on worker %d: %s", b, wi, cudaGetErrorString(q));
         }
     }
-    st.scanned = true;
-    *done = true;
+    *ready = true;
     return FBR_OK;
 }
 
@@ -2676,6 +2632,25 @@ static int dead_map_error(fbr_pool* p, const SeqState& st) {
                                            : "the pool was created without error_handling, so its blocks are not re-dispatched");
 }
 
+// The completion step, once every part of the map is done: harvests the map and, unless a task failed (fbr_result_wait
+// raises its error), gives a fold map its result record, tree() over the block totals that follow it in out, or wraps a
+// scan map's blocks after the first (scan_finish).  Both run here rather than behind cross-device events, so no worker's
+// stream waits on another device, and a dead worker fails the map before any other device depends on it.  *ready tells
+// whether the map's results are final: without `block`, a scan map's queued wraps may still be running.  The caller holds
+// the pool lock.
+static int complete_map(fbr_pool* p, SeqState& st, bool block, bool* ready) {
+    harvest(p, st);
+    *ready = true;
+    if (st.completed || st.err_code) return FBR_OK;
+    const BodyEntry& body = *body_of(st.func_id);
+    int rc = FBR_OK;
+    if (st.flags & FBR_FOLD) rc = fold_host_records(p, body, (const uint8_t*)st.out + body.result_bytes, st.parts.size(), st.out);
+    else if (st.flags & FBR_SCAN) rc = scan_finish(p, st, block, ready);
+    if (rc != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc;
+    st.completed = *ready;
+    return FBR_OK;
+}
+
 static int result_wait_locked_out(fbr_pool_t* p, uint64_t seq, int timeout_ms, fbr_result_t* res);
 
 // A waiter blocks on CUDA events OUTSIDE the pool lock; a concurrent fbr_result_release must not destroy them under it.
@@ -2712,15 +2687,13 @@ static int result_wait_locked_out(fbr_pool_t* p, uint64_t seq, int timeout_ms, f
             std::lock_guard<std::mutex> g(p->mu);
             auto it = p->seqs.find(seq);
             if (it == p->seqs.end()) return fail(FBR_ENOENT, "unknown seq %llu", (unsigned long long)seq);
-            if (it->second->dead_worker >= 0) return dead_map_error(p, *it->second);
-            for (auto& part : it->second->parts) evs.push_back({part.worker, p->workers[part.worker].device, part.done});
+            SeqState& st = *it->second;
+            if (st.dead_worker >= 0) return dead_map_error(p, st);
+            for (auto& part : st.parts) evs.push_back({part.worker, p->workers[part.worker].device, part.done});
             // FBR_SCAN: the wraps of blocks after the first, once queued (scan_done[b] belongs to the b-th block by start)
-            std::vector<const SeqPart*> by_first;
-            for (auto& part : it->second->parts) by_first.push_back(&part);
-            std::sort(by_first.begin(), by_first.end(), [](const SeqPart* a, const SeqPart* b) { return a->first < b->first; });
-            for (size_t b = 1; b < it->second->scan_done.size() && b < by_first.size(); ++b)
-                if (it->second->scan_done[b])
-                    evs.push_back({by_first[b]->worker, p->workers[by_first[b]->worker].device, it->second->scan_done[b]});
+            const std::vector<SeqPart*> blocks = parts_in_order(st);
+            for (size_t b = 1; b < st.scan_done.size() && b < blocks.size(); ++b)
+                if (st.scan_done[b]) evs.push_back({blocks[b]->worker, p->workers[blocks[b]->worker].device, st.scan_done[b]});
         }
         // block outside the pool lock so other threads can keep submitting
         bool again = false;
@@ -2740,12 +2713,9 @@ static int result_wait_locked_out(fbr_pool_t* p, uint64_t seq, int timeout_ms, f
             }
             if (q != cudaSuccess) {
                 // watchdog: is it the worker (sticky context error) or just this call?
-                cudaGetLastError();
                 std::lock_guard<std::mutex> g(p->mu);
-                cudaError_t why = q;
-                if (!worker_context_dead(p->workers[e.worker], &why))
+                if (!retire_if_dead(p, e.worker))
                     return fail(FBR_ECUDA, "waiting for seq %llu on worker %d: %s", (unsigned long long)seq, e.worker, cudaGetErrorString(q));
-                on_worker_death(p, e.worker, why);
                 again = true;       // the map's parts changed (re-dispatched) or it is marked dead
                 break;
             }
@@ -2767,26 +2737,17 @@ static int result_wait_locked_out(fbr_pool_t* p, uint64_t seq, int timeout_ms, f
             int rc = q == cudaSuccess ? resilient_advance(p, st, part) : FBR_ECUDA;
             if (rc < 0) {
                 const std::string msg = g_err;
-                cudaError_t why = q;
-                if (!worker_context_dead(w, &why)) { g_err = msg; return rc; }
-                on_worker_death(p, part.worker, why);     // st.parts is a different vector now
-                more = 1;
+                if (!retire_if_dead(p, part.worker)) { g_err = msg; return rc; }
+                more = 1;                                 // st.parts is a different vector now
                 break;
             }
             more |= rc;
         }
         if (more) continue;
-        harvest(p, st);
-        if ((st.flags & FBR_FOLD) && !st.err_code) {
-            const int rc = fold_finish(p, st);
-            if (rc != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc;
-        }
-        if ((st.flags & FBR_SCAN) && !st.err_code) {
-            bool scanned = false;
-            const int rc = scan_finish(p, st, &scanned);
-            if (rc != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc;
-            if (!scanned) continue;               // wait for the queued wraps outside the lock
-        }
+        bool ready = false;
+        const int rc = complete_map(p, st, false, &ready);
+        if (rc != FBR_OK) return rc;
+        if (!ready) continue;                     // wait for the queued wraps outside the lock
         memset(res, 0, sizeof *res);
         res->seq = seq;
         res->n_tasks = st.n_tasks;
@@ -2826,10 +2787,7 @@ int fbr_result_poll(fbr_pool_t* p, uint64_t seq, uint64_t* n_done) {
         if (q == cudaSuccess) q = cudaEventQuery(part.done);
         if (q != cudaSuccess && q != cudaErrorNotReady) {
             // watchdog (same as fbr_result_wait): a dead worker's blocks move to the survivors
-            cudaGetLastError();
-            cudaError_t why = q;
-            if (!worker_context_dead(w, &why)) return fail(FBR_ECUDA, "polling seq %llu on worker %d: %s", (unsigned long long)seq, part.worker, cudaGetErrorString(q));
-            on_worker_death(p, part.worker, why);
+            if (!retire_if_dead(p, part.worker)) return fail(FBR_ECUDA, "polling seq %llu on worker %d: %s", (unsigned long long)seq, part.worker, cudaGetErrorString(q));
             if (st.dead_worker >= 0) return dead_map_error(p, st);
             break;                                        // progress so far stands; the next poll sees the new parts
         }
@@ -2842,17 +2800,16 @@ int fbr_result_poll(fbr_pool_t* p, uint64_t seq, uint64_t* n_done) {
                 int rc = resilient_advance(p, st, part);
                 if (rc < 0) {
                     const std::string msg = g_err;
-                    cudaError_t why = cudaSuccess;
-                    if (!worker_context_dead(w, &why)) { g_err = msg; return rc; }
-                    on_worker_death(p, part.worker, why);
+                    if (!retire_if_dead(p, part.worker)) { g_err = msg; return rc; }
                     if (st.dead_worker >= 0) return dead_map_error(p, st);
                 }
             }
             break;
         }
         uint64_t part_done = 0;
-        if (part.cx.full_window && !part.cx.out_dev && !part.cx.keep_on_device) {
-            // the window reaches the host in one copy at the end: nothing is final before that
+        if (part.cx.full_window && (part.cx.scan || (!part.cx.out_dev && !part.cx.keep_on_device))) {
+            // the window reaches the host in one copy at the end, or (a scan block, results on the device too) its prefix
+            // folds are written in place behind its last wave: nothing is final before that
             if (part_finished) { done += part.count; continue; }
             break;
         }
@@ -2864,30 +2821,13 @@ int fbr_result_poll(fbr_pool_t* p, uint64_t seq, uint64_t* n_done) {
         done += part_done;
         if (part_done < part.count) break;
     }
-    if (st.flags & FBR_FOLD) {   // the one result record is there once every block is: 0 tasks done until then
-        if (done < st.n_tasks) {
-            done = 0;
-        } else {
-            const int rc = fold_finish(p, st);
-            if (rc != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc;
+    if (st.flags & (FBR_FOLD | FBR_SCAN)) {   // results are final once the map is complete: 0 tasks done until then
+        bool ready = false;
+        if (done >= st.n_tasks) {                 // every part is done: fold and scan blocks count only then (above)
+            const int rc = complete_map(p, st, false, &ready);
+            if (rc != FBR_OK) return rc;
         }
-    }
-    if (st.flags & FBR_SCAN) {   // blocks after the first are final once every block is done and wrapped
-        bool all = done >= st.n_tasks;
-        for (size_t pi = 0; pi < st.parts.size() && all; ++pi) {
-            const SeqPart& part = st.parts[pi];
-            const Worker& w = p->workers[part.worker];
-            all = !w.dead && cudaSetDevice(w.device) == cudaSuccess && cudaEventQuery(part.done) == cudaSuccess;
-        }
-        cudaGetLastError();
-        if (!all) {
-            done = 0;
-        } else if (harvest(p, st), !st.err_code) {   // a failed map raises its task error instead
-            bool scanned = false;
-            const int rc = scan_finish(p, st, &scanned);
-            if (rc != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc;
-            if (!scanned) done = 0;
-        }
+        if (!ready) done = 0;
     }
     *n_done = done;
     return FBR_OK;
@@ -2954,22 +2894,15 @@ int fbr_result_fetch(fbr_pool_t* p, uint64_t seq, uint64_t first, uint64_t count
     if (!(st.flags & FBR_RESULTS_ON_DEVICE)) return fail(FBR_EINVAL, "seq %llu does not keep its results on the device", (unsigned long long)seq);
     if (first + count > st.n_tasks) return fail(FBR_EINVAL, "range out of bounds");
     const uint64_t R = st.result_bytes;
-    if ((st.flags & FBR_SCAN) && !st.scanned) {   // blocks after the first hold their own prefixes until every block is done
+    if ((st.flags & FBR_SCAN) && !st.completed) {   // blocks after the first hold their own prefixes until the map completes
         if (st.dead_worker >= 0) return dead_map_error(p, st);
         for (auto& part : st.parts) {
             CK(cudaSetDevice(p->workers[part.worker].device));
             CK(cudaEventSynchronize(part.done));
         }
-        harvest(p, st);
-        if (!st.err_code) {
-            bool scanned = false;
-            const int rc = scan_finish(p, st, &scanned);
-            if (rc != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc;
-            for (size_t b = 1; !scanned && b < st.scan_done.size(); ++b)   // a fetch reads the wrapped window
-                if (st.scan_done[b]) CK(cudaEventSynchronize(st.scan_done[b]));
-            const int rc2 = scanned ? FBR_OK : scan_finish(p, st, &scanned);
-            if (rc2 != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc2;
-        }
+        bool ready = false;
+        const int rc = complete_map(p, st, true, &ready);   // a fetch reads the wrapped windows
+        if (rc != FBR_OK) return rc;
     }
     for (auto& part : st.parts) {
         const uint64_t lo = std::max(first, part.first), hi = std::min(first + count, part.first + part.count);
@@ -3020,7 +2953,24 @@ int fbr_scan_values(fbr_pool_t* p, int func_id, const void* pieces, uint32_t n_p
     std::lock_guard<std::mutex> g(p->mu);
     const int wi = first_live_worker(p);
     if (wi < 0) return fail(FBR_ECUDA, "every worker of this pool has died");
-    return wrap_records(p, wi, *bp, pieces, n_pieces, values, n, false);
+    const uint64_t R = bp->result_bytes;
+    if (n == 0 || n_pieces == 0) return FBR_OK;
+    Worker& w = p->workers[wi];
+    uint8_t* d = nullptr;   // the n records, wrapped in place
+    cudaError_t e = cudaSetDevice(w.device);
+    if (e == cudaSuccess) e = cudaMallocAsync((void**)&d, n * R, w.s_fold);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d, values, n * R, cudaMemcpyHostToDevice, w.s_fold);
+    if (e == cudaSuccess) e = queue_wrap(w, *bp, pieces, n_pieces, d, n, values, nullptr);
+    if (d) cudaFreeAsync(d, w.s_fold);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(w.s_fold);
+    if (e != cudaSuccess) {
+        retire_if_dead(p, wi);
+        return fail(FBR_ECUDA, "wrapping %llu records of body %s on worker %d: %s", (unsigned long long)n, bp->name.c_str(), wi,
+                    cudaGetErrorString(e));
+    }
+    p->stats.h2d_bytes += (n_pieces + n) * R;
+    p->stats.d2h_bytes += n * R;
+    return FBR_OK;
 }
 
 int fbr_host_alloc(fbr_pool_t* p, uint64_t bytes, void** ptr) {
