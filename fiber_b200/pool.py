@@ -281,18 +281,56 @@ class EmitResultArray(ResultArray):
                         % self._spec.name)
 
 
+def host_result(spec, kind, data, n=0, total=None, values=None):
+    """What a finished map whose results are in host memory returns, in either isolation.  ``kind`` is "plain", "bits"
+    (one bit per bool result), "emit" (variable-length results) or "fold"; ``spec`` is the body the caller mapped; ``n``
+    the number of results the caller sees.  ``data`` holds the result records as uint8 (the bit-packed bytes, the end
+    offsets of an emit map, a fold's one record), or is None for a map over no tasks; ``values`` are an emit map's
+    values; ``total`` is the device-side sum, or None."""
+    if kind == "fold":
+        return spec.unpack_result(fold_identity(spec) if data is None else bytes(data))
+    if kind == "emit":
+        if data is None:
+            return EmitResultArray(spec, np.empty(0, np.uint64), np.empty(0, spec.out_dtype))
+        return EmitResultArray(spec, data.view(np.uint64), values)
+    if kind == "bits" and data is not None:
+        return ResultArray(spec, None, total, n=n, bits=data)
+    dtype, sub = spec.result_dtype()
+    if data is None:
+        return ResultArray(spec, np.empty((0,) + sub, dtype), 0)
+    return ResultArray(spec, data.view(dtype).reshape((n,) + sub), total)
+
+
+def _raise_task_error(name, code, task, emit_count=None):
+    """Raise the exception of a map's first failed task (``err_code`` / ``err_task`` of its fbr_result_t) for body
+    ``name``; ``emit_count(task)`` gives the number of values an emit body's task was counted to push."""
+    if code == _abi.FBR_TASK_EMIT:
+        raise RuntimeError("%s: task %d emitted another number of values than the %d its count pass gave"
+                           % (name, task, emit_count(task)))
+    if code == _abi.FBR_TASK_OVERFLOW:
+        raise OverflowError("%s: result of task %d does not fit int64 (Python ints are unbounded; "
+                            "the device body refuses to wrap)" % (name, task))
+    if code == _abi.FBR_TASK_BADARG:
+        raise ValueError("%s: bad argument in task %d" % (name, task))
+    raise RuntimeError("%s: task %d failed with device error code %d" % (name, task, code))
+
+
 class MapResult:
     """Handle of an asynchronous map (fiber/pool.py:731-743)."""
 
-    def __init__(self, pool, engine, spec, seq, n, keepalive):
+    def __init__(self, pool, engine, spec, seq, n, keepalive, flags=0, user_spec=None, n_items=None):
+        """``flags``: the map's FBR_* flags.  A bit-packed map runs ``spec``, the bit-packed twin of the bool body
+        ``user_spec`` the caller mapped, over ``n`` = ceil(n_items / 8) byte tasks."""
         self._pool, self._engine, self._spec, self._seq, self._n = pool, engine, spec, seq, n
         self._keepalive = keepalive   # argument buffers must outlive the asynchronous H2D copies
+        self._flags = flags
+        self._user_spec = user_spec or spec
+        self._n_items = n if n_items is None else n_items      # the items the caller mapped
+        self._kind = "fold" if flags & _abi.FBR_FOLD else "bits" if user_spec is not None else \
+            "emit" if spec.flags & _abi.FBR_BODY_EMIT else "plain"
         self._result = None
         self._exc = None              # a task error is raised again by every later get()
         self._segment = _Segment(engine, seq) if n else None   # owns the seq from submission on
-        self._yielded = False
-        self._n_items = None          # bit-packed maps: number of range() indices (n = ceil(n_items / 8) byte tasks)
-        self._user_spec = spec
 
     # -- internal ----------------------------------------------------------------------------
     def _wait(self, timeout=None):
@@ -301,49 +339,49 @@ class MapResult:
         if self._exc is not None:
             raise self._exc
         if self._n == 0:
-            us = self._user_spec
-            if getattr(us, "out_dtype", None) is not None:
-                self._result = EmitResultArray(us, np.empty(0, np.uint64), np.empty(0, us.out_dtype))
-                return self._result
-            self._result = ResultArray(us, np.empty((0,) + us.result_dtype()[1], us.result_dtype()[0]), 0)
+            self._result = host_result(self._user_spec, self._kind, None)
             return self._result
         res = self._engine_wait(timeout)
-        eng = self._engine
-        dtype, sub = self._spec.result_dtype()
         # exact, unbounded sum: the device folds the two halves of int64 results separately (nothing wraps)
         dsum = (int(res.sum_hi) * (1 << 32) + int(res.sum_lo)) if (self._flags & _abi.FBR_WANT_SUM) else None
         self.n_waves = res.n_waves
-        if getattr(self._spec, "out_dtype", None) is not None:
-            self._result = self._emit_result(res)
-            return self._result
-        if self._flags & _abi.FBR_RESULTS_ON_DEVICE:
-            seg = self._segment                              # owns the seq (device buffer) until GC
-            rb, seq = res.result_bytes, self._seq
-
-            def fetch(lo, hi, seg=seg):
-                block = _PinnedBlock(eng, max(1, (hi - lo) * rb))
-                if hi > lo:
-                    _abi.check(eng.lib.fbr_result_fetch(eng.handle, seq, lo, hi - lo, ctypes.c_void_p(block.ptr)))
-                return np.asarray(block)[: (hi - lo) * rb].view(dtype).reshape((hi - lo,) + sub)
-            self._result = ResultArray(self._spec, None, dsum, n=int(res.n_tasks), fetch=fetch)
-            return self._result
-        seg = self._segment.bind(res.data, res.n_tasks * res.result_bytes)
-        arr = np.asarray(seg).view(dtype).reshape((res.n_tasks,) + sub)
-        if self._n_items is not None:
-            # bit-packed map (pi_inside_bits8): `arr` holds ceil(n/8) bytes.  The body evaluated all 8
-            # indices of the last byte; the ones past the end of the range are dropped here, from the
-            # byte and from the folded count.
-            n, extra = self._n_items, (-self._n_items) % 8
-            if extra:
-                last = int(arr[-1])
-                keep = last & (0xFF >> extra)
+        if self._kind == "fold":
+            self.raw = ctypes.string_at(res.data, res.result_bytes)     # process-isolated pools ship these bytes
+            self._result = host_result(self._spec, "fold", self.raw)
+        elif self._flags & _abi.FBR_RESULTS_ON_DEVICE:
+            self._result = self._device_result(res, dsum)
+        else:
+            data = np.asarray(self._segment.bind(res.data, res.n_tasks * res.result_bytes))
+            values = self._values_view() if self._kind == "emit" else None
+            if self._kind == "bits" and self._n_items % 8:
+                # `data` holds ceil(n/8) bytes.  The body evaluated all 8 indices of the last byte; the ones past the
+                # end of the range are dropped here, from the byte and from the folded count.
+                last = int(data[-1])
+                keep = last & (0xFF >> (-self._n_items) % 8)
                 if dsum is not None:
                     dsum -= bin(last ^ keep).count("1")
-                arr[-1] = keep
-            self._result = ResultArray(self._user_spec, None, dsum, n=n, bits=arr)
-            return self._result
-        self._result = ResultArray(self._spec, arr, dsum)
+                data[-1] = keep
+            self._result = host_result(self._user_spec, self._kind, data, self._n_items, dsum, values)
         return self._result
+
+    def _device_result(self, res, dsum):
+        """A finished map whose results stay in HBM: ranges of its results (and an emit map's values) are fetched on demand."""
+        eng, seq, seg = self._engine, self._seq, self._segment       # the segment owns the seq (device buffer) until GC
+
+        def fetcher(call, itemsize, dtype, sub=()):
+            def fetch(lo, hi, seg=seg):
+                block = _PinnedBlock(eng, max(1, (hi - lo) * itemsize))
+                if hi > lo:
+                    _abi.check(call(eng.handle, seq, lo, hi - lo, ctypes.c_void_p(block.ptr)))
+                return np.asarray(block)[: (hi - lo) * itemsize].view(dtype).reshape((hi - lo,) + sub)
+            return fetch
+        n = int(res.n_tasks)
+        if self._kind == "emit":
+            od = self._spec.out_dtype
+            return EmitResultArray(self._spec, None, None, n=n, fetch=fetcher(eng.lib.fbr_result_fetch, 8, np.uint64),
+                                   fetch_values=fetcher(eng.lib.fbr_result_fetch_values, od.itemsize, od))
+        dtype, sub = self._spec.result_dtype()
+        return ResultArray(self._spec, None, dsum, n=n, fetch=fetcher(eng.lib.fbr_result_fetch, res.result_bytes, dtype, sub))
 
     def _engine_wait(self, timeout):
         """fbr_result_wait for a map of n > 0 tasks: its fbr_result_t, or the map's task error raised."""
@@ -355,33 +393,14 @@ class MapResult:
             raise TimeoutError("map %d not finished" % self._seq)
         if rc == _abi.FBR_ETASK:
             try:
-                self._raise_task_error(res)
+                _raise_task_error(self._user_spec.name, res.err_code, res.err_task, lambda task: self._emit_count(res, task))
             except Exception as e:      # noqa: BLE001 -- remembered: later get() calls raise it without touching the engine
                 self._exc = e
                 raise
         _abi.check(rc)
         self._keepalive = None
-        self._pool.recv_tasks += self._n if self._n_items is None else self._n_items
+        self._pool.recv_tasks += self._n_items
         return res
-
-    def _emit_result(self, res):
-        """End offsets and values of a finished emit map: views of its pinned segments, or fetched from the device."""
-        eng, seq, seg, n, od = self._engine, self._seq, self._segment, int(res.n_tasks), self._spec.out_dtype
-        if self._flags & _abi.FBR_RESULTS_ON_DEVICE:
-            def fetch(lo, hi):
-                block = _PinnedBlock(eng, max(1, (hi - lo) * 8))
-                if hi > lo:
-                    _abi.check(eng.lib.fbr_result_fetch(eng.handle, seq, lo, hi - lo, ctypes.c_void_p(block.ptr)))
-                return np.asarray(block)[: (hi - lo) * 8].view(np.uint64)
-
-            def fetch_values(lo, hi, seg=seg):
-                block = _PinnedBlock(eng, max(1, (hi - lo) * od.itemsize))
-                if hi > lo:
-                    _abi.check(eng.lib.fbr_result_fetch_values(eng.handle, seq, lo, hi - lo, ctypes.c_void_p(block.ptr)))
-                return np.asarray(block)[: (hi - lo) * od.itemsize].view(od)
-            return EmitResultArray(self._spec, None, None, n=n, fetch=fetch, fetch_values=fetch_values)
-        ends = np.asarray(seg.bind(res.data, n * 8)).view(np.uint64)
-        return EmitResultArray(self._spec, ends, self._values_view())
 
     def _values_view(self):
         eng, ptr, nv = self._engine, ctypes.c_void_p(), ctypes.c_uint64(0)
@@ -400,19 +419,6 @@ class MapResult:
             ctypes.memmove(ends.ctypes.data, res.data + lo * 8, ends.nbytes)
         return int(ends[-1]) - (int(ends[0]) if task > 0 else 0)
 
-    def _raise_task_error(self, res):
-        code, task = res.err_code, res.err_task
-        name = getattr(self, "_user_spec", self._spec).name     # the body the caller mapped (not its bit-packed twin)
-        if code == _abi.FBR_TASK_EMIT:
-            raise RuntimeError("%s: task %d emitted another number of values than the %d its count pass gave"
-                               % (name, task, self._emit_count(res, task)))
-        if code == _abi.FBR_TASK_OVERFLOW:
-            raise OverflowError("%s: result of task %d does not fit int64 (Python ints are unbounded; "
-                                "the device body refuses to wrap)" % (name, task))
-        if code == _abi.FBR_TASK_BADARG:
-            raise ValueError("%s: bad argument in task %d" % (name, task))
-        raise RuntimeError("%s: task %d failed with device error code %d" % (name, task, code))
-
     # -- reference surface -------------------------------------------------------------------
     def get(self, timeout=None):
         return self._wait(timeout)
@@ -424,71 +430,33 @@ class MapResult:
         if self._flags & _abi.FBR_RESULTS_ON_DEVICE:
             yield from self._wait()
             return
-        eng = self._engine
-        if getattr(self._spec, "out_dtype", None) is not None:
-            # an emit map: the values of a finished wave are final in the values segment, its end offsets in the result one
-            done, emitted = ctypes.c_uint64(0), 0
-            values = None
-            while emitted < self._n:
-                _abi.check(eng.lib.fbr_result_poll(eng.handle, self._seq, ctypes.byref(done)))
-                if done.value >= self._n:
-                    break
-                if done.value > emitted:
-                    values = self._values_view() if values is None else values
-                    ends = self._peek(max(0, emitted - 1), done.value, np.dtype(np.uint64), ())
-                    if emitted == 0:
-                        ends = np.concatenate([np.zeros(1, np.uint64), ends])
-                    for k in range(len(ends) - 1):
-                        yield _emit_value(self._spec, values[int(ends[k]):int(ends[k + 1])])
-                    emitted = done.value
-                else:
-                    time.sleep(0.0002)
-            res = self._wait()
-            if emitted < self._n:
-                yield from res[emitted:]
-            return
-        if self._n_items is not None:
-            # bit-packed map: progress is counted in result bytes (8 tasks each); every byte of a finished
-            # wave is a full byte, the (masked) last byte of the map only comes from _wait()
-            done, emitted = ctypes.c_uint64(0), 0
-            while emitted < self._n:
-                _abi.check(eng.lib.fbr_result_poll(eng.handle, self._seq, ctypes.byref(done)))
-                if done.value >= self._n:
-                    break
-                if done.value > emitted:
-                    part = self._peek(emitted, done.value, np.dtype(np.uint8), ())
-                    yield from np.unpackbits(part, bitorder="little").view(np.bool_).tolist()
-                    emitted = done.value
-                else:
-                    time.sleep(0.0002)
-            res = self._wait()
-            if emitted * 8 < self._n_items:
-                yield from res[emitted * 8:]
-            return
-        done = ctypes.c_uint64(0)
-        emitted = 0
-        dtype, sub = self._spec.result_dtype()
+        eng, values = self._engine, None
+        done, emitted, items = ctypes.c_uint64(0), 0, 0
         # peek at the segment: results land in it wave by wave
         while emitted < self._n:
             _abi.check(eng.lib.fbr_result_poll(eng.handle, self._seq, ctypes.byref(done)))
             if done.value >= self._n:
                 break
             if done.value > emitted:
-                # an ordered prefix is final but the map is not: hand it out from the live segment
-                part = self._peek(emitted, done.value, dtype, sub)
-                yield from self._spec.rows_to_list(part)
+                # an ordered prefix is final but the map is not: hand it out from the live segment (an emit map's values
+                # of a finished wave are final in its values segment)
+                values = self._values_view() if self._kind == "emit" and values is None else values
+                part = self._live_prefix(done.value, values)[items:]
+                yield from part
+                items += len(part)
                 emitted = done.value
             else:
                 time.sleep(0.0002)
-        res = self._wait()
-        if emitted < self._n:
-            yield from self._spec.rows_to_list(res.array[emitted:])
+        yield from self._wait()[items:]
 
-    def _peek(self, lo, hi, dtype, sub):
-        base = self._pool._segment_ptr(self._seq)
-        rb = self._spec.result_bytes
-        buf = (ctypes.c_char * ((hi - lo) * rb)).from_address(base + lo * rb)
-        return np.frombuffer(buf, dtype=dtype).reshape((hi - lo,) + sub).copy()
+    def _live_prefix(self, rows, values):
+        """The results of the first ``rows`` result rows of the live segment, read as the finished map reads them.  A
+        bit-packed map's row is a byte of 8 results: every byte of a finished wave is a full byte, the (masked) last byte
+        of the map only comes from _wait()."""
+        eng, ptr = self._engine, ctypes.c_void_p()
+        _abi.check(eng.lib.fbr_result_data(eng.handle, self._seq, ctypes.byref(ptr)))   # the engine-owned pinned segment
+        data = np.asarray(_View(self._segment, ptr.value, rows * self._spec.result_bytes))
+        return host_result(self._user_spec, self._kind, data, 8 * rows if self._kind == "bits" else rows, None, values)
 
     def iget_ordered(self):
         return self._iter_ready()
@@ -511,19 +479,6 @@ def fold_identity(spec):
 class FoldResult(MapResult):
     """Handle of an asynchronous fold (``Pool.fold_async``): ``get()`` returns tree() over the map's results (FBR_FOLD in
     include/fiber_b200.h), read like one task's result."""
-
-    def _wait(self, timeout=None):
-        if self._exc is not None:
-            raise self._exc
-        if self._result is None:
-            if self._n == 0:
-                raw = fold_identity(self._spec)
-            else:
-                res = self._engine_wait(timeout)
-                raw = ctypes.string_at(res.data, res.result_bytes)
-            self.raw = raw                  # the result record's bytes (process-isolated pools ship them)
-            self._result = (self._spec.unpack_result(raw),)
-        return self._result[0]
 
     def _iter_ready(self):
         raise TypeError("%s: a fold has one result, not one per task: use get()" % self._spec.name)
@@ -583,10 +538,8 @@ class ExpressResult:
             raise TimeoutError("apply %d not finished" % self._ticket)
         if rc == _abi.FBR_ETASK:
             self._done = True
-            res = _abi.Result()
-            res.err_code, res.err_task = err.value, 0
             try:
-                MapResult._raise_task_error(self, res)
+                _raise_task_error(self._spec.name, err.value, 0)
             except Exception as e:      # noqa: BLE001 -- remembered so that a second get() raises again
                 self._exc = e
                 raise
@@ -753,7 +706,7 @@ class Pool:
             eng.lib.fbr_shared_drop(eng.handle, old)
         return h.value
 
-    def _submit(self, func, enc, kind, chunksize, cls=MapResult, want_sum=True, extra_flags=0, spec=None):
+    def _submit(self, func, enc, kind, chunksize, cls=MapResult, want_sum=True, extra_flags=0, spec=None, user_spec=None):
         spec = spec or registry.spec(registry.body_name_of(func))
         eng = self._engine
         d = _abi.MapDesc()
@@ -799,68 +752,72 @@ class Pool:
             _abi.check(eng.lib.fbr_map_submit_items_n(eng.handle, ctypes.byref(d), streams, len(streams), ctypes.byref(seq)))
         elif enc.n:
             _abi.check(eng.lib.fbr_map_submit(eng.handle, ctypes.byref(d), ctypes.byref(seq)))
-        self.sent_tasks += enc.n
-        r = cls(self, eng, spec, seq.value, enc.n, keep)
-        r._flags = flags
-        return r
-
-    def _segment_ptr(self, seq):
-        # results are written into the engine-owned pinned segment wave by wave
-        eng = self._engine
-        ptr = ctypes.c_void_p()
-        _abi.check(eng.lib.fbr_result_data(eng.handle, seq, ctypes.byref(ptr)))
-        return ptr.value
+        n_items = enc.n if user_spec is None else enc.n_items
+        self.sent_tasks += n_items
+        return cls(self, eng, spec, seq.value, enc.n, keep, flags, user_spec, n_items)
 
     @staticmethod
     def _spec_of(func):
         return registry.spec(registry.body_name_of(func))
 
-    def map_async(self, func, iterable, chunksize=None, callback=None, error_callback=None, _streaming=False):
-        if error_callback:
-            raise NotImplementedError
+    def _start(self, func, iterable, *, star, mode, chunksize=None, streaming=False):
+        """The one submission path of maps (``mode`` "map"), folds and accumulates of ``func`` over ``iterable``, whose
+        items are argument tuples with ``star``: a MapResult, or a FoldResult for a fold."""
         self._check_running()
         if chunksize is None:
-            chunksize = DEFAULT_CHUNKSIZE
+            chunksize = DEFAULT_CHUNKSIZE if mode == "map" else 0     # a fold's order does not depend on a chunksize
+        spec = self._spec_of(func) if mode == "map" else self._fold_spec(func, scan=mode == "accumulate")
         if not hasattr(iterable, "__len__"):
             iterable = list(iterable)
-        spec = self._spec_of(func)
         self.lazy_start_workers(func)
         if self._proc is not None:
-            return self._submit_proc(spec, "map", iterable, chunksize)
-        enc = spec.encode_map(iterable)
+            return self._submit_proc(spec, ("star" if star else "") + mode, iterable, chunksize)
         # imap wants ordered prefixes as they complete: results are staged and copied out wave by wave instead of being
         # stored straight into the pinned segment by one kernel (zero copy, final only when the whole block is)
-        extra = _abi.FBR_NO_ZERO_COPY if _streaming else 0
-        if self._results_bits and spec.name in registry.BITS_TWIN:
-            return self._submit_bits(func, spec, enc, _abi.FBR_MAP, chunksize, extra)
-        return self._submit(func, enc, _abi.FBR_MAP, chunksize, extra_flags=extra)
+        cls, want_sum, flags = {"map": (MapResult, True, _abi.FBR_NO_ZERO_COPY if streaming else 0),
+                                "fold": (FoldResult, False, _abi.FBR_FOLD),
+                                "accumulate": (MapResult, False, _abi.FBR_SCAN)}[mode]
+        if mode != "map" and len(iterable) == 0:          # identity() / no prefixes: nothing to bind or submit
+            return cls(self, self._engine, spec, 0, 0, None, flags)
+        enc = spec.encode_starmap(iterable) if star else spec.encode_map(iterable)
+        kind = _abi.FBR_STARMAP if star else _abi.FBR_MAP
+        if mode == "map" and self._results_bits and spec.name in registry.BITS_TWIN:
+            # A bool needs one bit: the twin body evaluates 8 consecutive items (range() indices or argument
+            # records) per result byte, so the ring, the ordered output and the D2H copy move n/8 bytes.
+            twin = registry.spec(registry.BITS_TWIN[spec.name])
+            return self._submit(func, twin.from_encoded(enc), kind, max(1, chunksize // 8), extra_flags=flags, spec=twin,
+                                user_spec=spec)
+        return self._submit(func, enc, kind, chunksize, cls=cls, want_sum=want_sum, extra_flags=flags, spec=spec)
 
-    def _submit_proc(self, spec, kind, items, chunksize, single=False):
-        """Process-isolated workers: the map is cut into blocks that worker processes pull (procpool.py)."""
-        if not isinstance(items, (range, list, np.ndarray, registry.Ragged, registry.Columns)):
+    def _submit_proc(self, spec, kind, items, chunksize):
+        """Process-isolated workers: the map is cut into blocks that worker processes pull (procpool.py).  ``kind`` is the
+        block kind: "map", "apply", "fold" or "accumulate", with "star" in front for argument tuples."""
+        if (kind.startswith("star") and not isinstance(items, registry.Columns)) or \
+                not isinstance(items, (range, list, np.ndarray, registry.Ragged, registry.Columns)):
             items = list(items)         # a Ragged (or Columns) stays one: its blocks are slices with rebased offsets
         if kind == "map" and len(items):
             spec.encode_map(items[:1] if not isinstance(items, range) else items)      # argument validation up front
-        twin = registry.BITS_TWIN.get(spec.name) if (self._results_bits and kind != "apply") else None
-        r = self._proc.submit(spec, twin, kind, items, chunksize, single)
+        twin = registry.BITS_TWIN.get(spec.name) if self._results_bits and kind in ("map", "starmap") else None
+        r = self._proc.submit(spec, twin, kind, items, chunksize, single=kind in ("apply", "fold", "starfold"))
         self.sent_tasks += len(items)
         return r
 
-    def _submit_bits(self, func, spec, enc, kind, chunksize, extra_flags=0):
-        """A bool needs one bit: the twin body evaluates 8 consecutive items (range() indices or argument
-        records) per result byte, so the ring, the ordered output and the D2H copy move n/8 bytes."""
-        twin = registry.spec(registry.BITS_TWIN[spec.name])
-        n_items = enc.n
-        r = self._submit(func, twin.from_encoded(enc), kind, max(1, chunksize // 8), spec=twin, extra_flags=extra_flags)
-        r._n_items, r._user_spec = n_items, spec
-        self.sent_tasks += n_items - r._n
-        return r
+    def map_async(self, func, iterable, chunksize=None, callback=None, error_callback=None, _streaming=False):
+        if error_callback:
+            raise NotImplementedError
+        return self._start(func, iterable, star=False, mode="map", chunksize=chunksize, streaming=_streaming)
 
     def map(self, func, iterable, chunksize=None):
         return self.map_async(func, iterable, chunksize).get()
 
+    def starmap_async(self, func, iterable, chunksize=None, callback=None, error_callback=None):
+        return self._start(func, iterable, star=True, mode="map", chunksize=chunksize)
+
+    def starmap(self, func, iterable, chunksize=None):
+        return self.starmap_async(func, iterable, chunksize).get()
+
     # -- folds: a map reduced on the device with the body's combine() ------------------------------------------------
-    def _fold_spec(self, func):
+    def _fold_spec(self, func, scan=False):
         spec = self._spec_of(func)
         if not spec.flags & _abi.FBR_BODY_FOLD:
             if not spec.flags & _abi.FBR_BODY_RECORD:
@@ -868,105 +825,49 @@ class Pool:
             else:
                 hint = "a record body folds when it defines identity() and combine() next to run()"
             raise TypeError("%s cannot fold: it has no combine() (%s)" % (spec.name, hint))
+        if scan and not spec.flags & _abi.FBR_BODY_SCAN:
+            raise TypeError("%s cannot accumulate: its module exports no scan entry (rebuild it with "
+                            "FBR_EXPORT_RECORD_BODY)" % spec.name)
         return spec
-
-    def _fold(self, func, iterable, kind):
-        self._check_running()
-        spec = self._fold_spec(func)
-        if not hasattr(iterable, "__len__"):
-            iterable = list(iterable)
-        self.lazy_start_workers(func)
-        if self._proc is not None:
-            if kind == "starmap" and not isinstance(iterable, registry.Columns):
-                iterable = list(iterable)
-            return self._proc.submit_fold(spec, kind, iterable)
-        if len(iterable) == 0:                     # identity(): nothing to bind or submit
-            r = FoldResult(self, self._engine, spec, 0, 0, None)
-            r._flags = _abi.FBR_FOLD
-            return r
-        enc = spec.encode_map(iterable) if kind == "map" else spec.encode_starmap(iterable)
-        return self._submit(func, enc, _abi.FBR_MAP if kind == "map" else _abi.FBR_STARMAP, 0, cls=FoldResult,
-                            want_sum=False, extra_flags=_abi.FBR_FOLD, spec=spec)
 
     def fold_async(self, func, iterable):
         """``functools.reduce(combine, map(func, iterable))`` on the device, in the fixed order tree() of FBR_FOLD
         (include/fiber_b200.h): a FoldResult.  There is no chunksize, since the order does not depend on one."""
-        return self._fold(func, iterable, "map")
+        return self._start(func, iterable, star=False, mode="fold")
 
     def fold(self, func, iterable):
         return self.fold_async(func, iterable).get()
 
     def starfold_async(self, func, iterable):
         """``fold_async`` over argument tuples, bound as ``starmap`` binds them."""
-        return self._fold(func, iterable, "starmap")
+        return self._start(func, iterable, star=True, mode="fold")
 
     def starfold(self, func, iterable):
         return self.starfold_async(func, iterable).get()
 
     # -- accumulates: every prefix of a fold, on the device ------------------------------------------------------------
-    def _accumulate(self, func, iterable, kind):
-        self._check_running()
-        spec = self._fold_spec(func)
-        if not spec.flags & _abi.FBR_BODY_SCAN:
-            raise TypeError("%s cannot accumulate: its module exports no scan entry (rebuild it with "
-                            "FBR_EXPORT_RECORD_BODY)" % spec.name)
-        if not hasattr(iterable, "__len__"):
-            iterable = list(iterable)
-        self.lazy_start_workers(func)
-        if self._proc is not None:
-            if kind == "starmap" and not isinstance(iterable, registry.Columns):
-                iterable = list(iterable)
-            r = self._proc.submit_accumulate(spec, kind, iterable)
-            self.sent_tasks += len(iterable)
-            return r
-        if len(iterable) == 0:                     # no prefixes: nothing to bind or submit
-            r = MapResult(self, self._engine, spec, 0, 0, None)
-            r._flags = _abi.FBR_SCAN
-            return r
-        enc = spec.encode_map(iterable) if kind == "map" else spec.encode_starmap(iterable)
-        return self._submit(func, enc, _abi.FBR_MAP if kind == "map" else _abi.FBR_STARMAP, 0, want_sum=False,
-                            extra_flags=_abi.FBR_SCAN, spec=spec)
-
     def accumulate_async(self, func, iterable):
         """``itertools.accumulate(map(func, iterable), combine)`` on the device: a MapResult whose record i is the fold of
         results 0 .. i in the order of FBR_SCAN (include/fiber_b200.h) -- on one worker ``fold(func, iterable[:i + 1])``
         bit for bit, and the last record is always ``fold(func, iterable)``.  There is no chunksize, as for ``fold``."""
-        return self._accumulate(func, iterable, "map")
+        return self._start(func, iterable, star=False, mode="accumulate")
 
     def accumulate(self, func, iterable):
         return self.accumulate_async(func, iterable).get()
 
     def staraccumulate_async(self, func, iterable):
         """``accumulate_async`` over argument tuples, bound as ``starmap`` binds them."""
-        return self._accumulate(func, iterable, "starmap")
+        return self._start(func, iterable, star=True, mode="accumulate")
 
     def staraccumulate(self, func, iterable):
         return self.staraccumulate_async(func, iterable).get()
-
-    def starmap_async(self, func, iterable, chunksize=None, callback=None, error_callback=None):
-        self._check_running()
-        if chunksize is None:
-            chunksize = DEFAULT_CHUNKSIZE
-        if not hasattr(iterable, "__len__"):
-            iterable = list(iterable)
-        spec = self._spec_of(func)
-        self.lazy_start_workers(func)
-        if self._proc is not None:
-            return self._submit_proc(spec, "starmap", iterable if isinstance(iterable, registry.Columns) else list(iterable), chunksize)
-        enc = spec.encode_starmap(iterable)
-        if self._results_bits and spec.name in registry.BITS_TWIN:
-            return self._submit_bits(func, spec, enc, _abi.FBR_STARMAP, chunksize)
-        return self._submit(func, enc, _abi.FBR_STARMAP, chunksize)
-
-    def starmap(self, func, iterable, chunksize=None):
-        return self.starmap_async(func, iterable, chunksize).get()
 
     def apply_async(self, func, args=(), kwds={}, callback=None, error_callback=None):
         self._check_running()
         spec = self._spec_of(func)
         self.lazy_start_workers(func)
         if self._proc is not None:
-            return self._submit_proc(spec, "apply", [(tuple(args), dict(kwds))], 1, single=True)
+            return self._submit_proc(spec, "apply", [(tuple(args), dict(kwds))], 1)
         if self._use_express and spec.name in _Express.BODIES:
             # one task whose record fits the doorbell lane: no kernel launch / copy on the round trip
             rec = spec.pack_apply(args, kwds)
@@ -988,8 +889,7 @@ class Pool:
         return iter(r.get()) if self._proc is not None else r.iget_ordered()
 
     def imap_unordered(self, func, iterable, chunksize=1):
-        r = self.map_async(func, iterable, chunksize, _streaming=True)
-        return iter(r.get()) if self._proc is not None else r.iget_unordered()
+        return self.imap(func, iterable, chunksize)     # arrival order == ring order: ordered prefixes are a valid "unordered" stream
 
     # -- shutdown (fiber/pool.py:1332-1403) -----------------------------------------------------------
     def close(self):

@@ -17,6 +17,7 @@ replaced by a fresh process.  Everything a worker computes still runs through th
 fallback here either.
 """
 import collections
+import contextlib
 import mmap
 import multiprocessing as mp
 import multiprocessing.connection as mpc
@@ -28,6 +29,8 @@ import time
 import weakref
 
 import numpy as np
+
+from . import _abi
 
 BLOCK_ALIGN = 32768          # tasks: a multiple of every claim unit and of 8 (bit-packed bytes stay whole)
 MAX_ATTEMPTS = 6
@@ -116,6 +119,40 @@ def _initializer_for(body):
     return registry.device_initializer(body)(initializer)
 
 
+def _register(body, module):
+    """Register device body ``body`` from ``module`` (``registry.module_of`` in the master) if this process lacks it."""
+    from . import registry
+    if module is not None and body not in registry.body_names():
+        registry.register_module(body, *module)
+
+
+def _attach(segments, name):
+    """This worker's mapping of the map segment ``name``: one live segment per worker is enough."""
+    seg = segments.get(name)
+    if seg is None:
+        segments.clear()
+        seg = segments[name] = SharedSegment(name)
+    return seg
+
+
+@contextlib.contextmanager
+def _reporting(conn, job, blk):
+    """One step of map ``job`` (block ``blk``, -1 for a map's last step) in a worker: a failure is sent to the master as
+    "error", except a lost CUDA context, which is sent as "dead" and ends the process."""
+    try:
+        yield
+    except _abi.EngineError as e:
+        if e.status == _abi.FBR_ECUDA:
+            # the CUDA context of this process is gone for good: report and die, the master re-queues the work
+            try:
+                conn.send(("dead", job, blk, str(e)))
+            finally:
+                os._exit(3)
+        conn.send(("error", job, blk, "EngineError", str(e)))
+    except (OverflowError, ValueError, TypeError, RuntimeError, KeyError, OSError) as e:   # OSError: the segment of a failed map is gone
+        conn.send(("error", job, blk, type(e).__name__, str(e)))
+
+
 def gpu_worker_main(device, conn, results, sys_path, init=None):
     """Worker process: one engine on one GPU, blocks in, ordered result bytes out (into shared memory).  ``init``:
     (body, initargs, module) of the pool's initializer, or None."""
@@ -123,12 +160,11 @@ def gpu_worker_main(device, conn, results, sys_path, init=None):
         if p not in sys.path:
             sys.path.insert(0, p)
     import fiber_b200
-    from fiber_b200 import _abi, registry
+    from fiber_b200 import registry
     kw = {}
     if init is not None:
         body, initargs, module = init
-        if module is not None and body not in registry.body_names():
-            registry.register_module(body, *module)
+        _register(body, module)
         kw = {"initializer": _initializer_for(body), "initargs": initargs}
     pool = fiber_b200.Pool(1, devices=[device], express=False, results=results, **kw)
     pool.start_workers()
@@ -145,47 +181,38 @@ def gpu_worker_main(device, conn, results, sys_path, init=None):
             _scan_blocks_in_worker(pool, conn, segments, msg)
             continue
         _, job, blk, body, kind, chunksize, payload, shm_name, off, attempt, module = msg
-        try:
-            if module is not None and body not in registry.body_names():
-                registry.register_module(body, *module)
+        with _reporting(conn, job, blk):
+            _register(body, module)
+            spec = registry.spec(body)
             f = proxies.get(body) or proxies.setdefault(body, _proxy_for(body))
             items = range(*payload[1]) if payload[0] == "range" else pickle.loads(payload[1])
             pool._attempt = attempt
-            if kind in ("fold", "starfold"):             # the block's total, R bytes
-                res = pool.fold_async(f, items) if kind == "fold" else pool.starfold_async(f, items)
-                res.get()
-                raw = np.frombuffer(res.raw, np.uint8)
-            elif kind in ("accumulate", "staraccumulate"):   # the block's own prefix folds, placed like a map's results
-                res = pool.accumulate(f, items) if kind == "accumulate" else pool.staraccumulate(f, items)
-            elif kind == "starmap":
-                res = pool.starmap(f, items, chunksize)
-            elif kind == "apply":
-                res = pool.apply_async(f, items[0][0], items[0][1])._wait()
+            # the block runs as the same kind of map of a thread-isolated pool: an accumulate block gives its own prefix folds
+            mode = kind.removeprefix("star")
+            if mode == "apply":
+                handle = pool.apply_async(f, items[0][0], items[0][1])
             else:
-                res = pool.map(f, items, chunksize)
-            if kind not in ("fold", "starfold"):
+                handle = pool._start(f, items, star=mode != kind, mode=mode, chunksize=chunksize)
+            res = handle._wait()
+            if mode == "fold":                                     # the block's total, R bytes
+                raw = np.frombuffer(handle.raw, np.uint8)
+            else:
                 raw = res.packed if res.packed is not None else np.ascontiguousarray(np.asarray(res)).view(np.uint8).reshape(-1)
-            seg = segments.get(shm_name)
-            if seg is None:
-                segments.clear()                                   # one live segment per worker is enough
-                seg = segments.setdefault(shm_name, SharedSegment(shm_name))
-            seg.array[off:off + raw.nbytes] = raw                  # placement by index (fiber/pool.py:672), block-wise
-            if getattr(registry.spec(body), "out_dtype", None) is not None:
+            _attach(segments, shm_name).array[off:off + raw.nbytes] = raw      # placement by index (fiber/pool.py:672), block-wise
+            if spec.flags & _abi.FBR_BODY_EMIT:
                 put_values(values_name(shm_name, blk), res.ragged.values)   # an emit body: the block's values beside it
-            total = res.sum() if (registry.spec(body).flags & _abi.FBR_BODY_SUMMABLE) else None
+            total = res.sum() if (spec.flags & _abi.FBR_BODY_SUMMABLE) else None
             del res, raw
             conn.send(("done", job, blk, total))
-        except _abi.EngineError as e:
-            if e.status == _abi.FBR_ECUDA:
-                # the CUDA context of this process is gone for good: report and die, the master re-queues the block
-                try:
-                    conn.send(("dead", job, blk, str(e)))
-                finally:
-                    os._exit(3)
-            conn.send(("error", job, blk, "EngineError", str(e)))
-        except (OverflowError, ValueError, TypeError, RuntimeError, KeyError, OSError) as e:   # OSError: the segment of a failed map is gone
-            conn.send(("error", job, blk, type(e).__name__, str(e)))
     os._exit(0)
+
+
+def _fold_values(pool, spec, records, count):
+    """tree() over ``count`` result records of body ``spec`` (uint8, back to back) in their order, by fbr_fold_values."""
+    out = np.zeros(spec.result_bytes, np.uint8)
+    src = np.ascontiguousarray(records)
+    _abi.check(pool._engine.lib.fbr_fold_values(pool._engine.handle, spec.func_id, src.ctypes.data, count, out.ctypes.data))
+    return out
 
 
 def _scan_pieces(fold, totals, b):
@@ -200,22 +227,18 @@ def _scan_blocks_in_worker(pool, conn, segments, msg):
     (fbr_scan_values).  The totals come from the master, read before any block was wrapped, so a step sent again after a
     death wraps the blocks still listed exactly as the first attempt would have.  Each block is wrapped in a private copy,
     placed, and reported ("scanned"), so the master never lists a placed block again."""
-    from fiber_b200 import _abi, registry
+    from fiber_b200 import registry
     _, job, ranges, todo, totals, body, shm_name, module = msg
-    try:
-        if module is not None and body not in registry.body_names():
-            registry.register_module(body, *module)
+    with _reporting(conn, job, -1):
+        _register(body, module)
         spec = registry.spec(body)
         R = spec.result_bytes
-        seg = segments.get(shm_name) or SharedSegment(shm_name)
+        seg = _attach(segments, shm_name)
         eng = pool._engine
         tot = np.frombuffer(totals, np.uint8)
 
-        def fold(lo, count):
-            out = np.zeros(R, np.uint8)
-            src = np.ascontiguousarray(tot[lo * R:(lo + count) * R])
-            _abi.check(eng.lib.fbr_fold_values(eng.handle, spec.func_id, src.ctypes.data, count, out.ctypes.data))
-            return out
+        def fold(k, count):
+            return _fold_values(pool, spec, tot[k * R:(k + count) * R], count)
 
         for b in todo:
             lo, hi = ranges[b]
@@ -226,43 +249,20 @@ def _scan_blocks_in_worker(pool, conn, segments, msg):
             seg.array[lo * R:hi * R] = recs
             conn.send(("scanned", job, b))
         conn.send(("folded", job))
-    except _abi.EngineError as e:
-        if e.status == _abi.FBR_ECUDA:
-            try:
-                conn.send(("dead", job, -1, str(e)))
-            finally:
-                os._exit(3)
-        conn.send(("error", job, -1, "EngineError", str(e)))
-    except (ValueError, TypeError, RuntimeError, KeyError, OSError) as e:
-        conn.send(("error", job, -1, type(e).__name__, str(e)))
 
 
 def _fold_totals_in_worker(pool, conn, segments, msg):
     """A fold map's last step, in the worker the master picked: the n_blocks totals after the result record in the map's
     segment, folded in block order by fbr_fold_values into the result record (the segment's first R bytes)."""
-    from fiber_b200 import _abi, registry
+    from fiber_b200 import registry
     _, job, n_blocks, body, shm_name, module = msg
-    try:
-        if module is not None and body not in registry.body_names():
-            registry.register_module(body, *module)
+    with _reporting(conn, job, -1):
+        _register(body, module)
         spec = registry.spec(body)
         R = spec.result_bytes
-        seg = segments.get(shm_name) or SharedSegment(shm_name)
-        totals = np.array(seg.array[R:(1 + n_blocks) * R])
-        out = np.zeros(R, np.uint8)
-        eng = pool._engine
-        _abi.check(eng.lib.fbr_fold_values(eng.handle, spec.func_id, totals.ctypes.data, n_blocks, out.ctypes.data))
-        seg.array[:R] = out
+        seg = _attach(segments, shm_name)
+        seg.array[:R] = _fold_values(pool, spec, seg.array[R:(1 + n_blocks) * R], n_blocks)
         conn.send(("folded", job))
-    except _abi.EngineError as e:
-        if e.status == _abi.FBR_ECUDA:
-            try:
-                conn.send(("dead", job, -1, str(e)))
-            finally:
-                os._exit(3)
-        conn.send(("error", job, -1, "EngineError", str(e)))
-    except (ValueError, TypeError, RuntimeError, KeyError, OSError) as e:
-        conn.send(("error", job, -1, type(e).__name__, str(e)))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -311,6 +311,25 @@ def _release_shm(shm):
     shm.release()                   # unlink the name; the mapping lives as long as NumPy views of it do
 
 
+# the exceptions a worker's "error" message names that the master raises as they are; any other becomes RuntimeError
+_ERRORS = {"OverflowError": OverflowError, "ValueError": ValueError, "TypeError": TypeError}
+
+
+def _receive(w, ready, when=""):
+    """What worker ``w`` has to say, given the objects ``mpc.wait`` found ``ready``: (message, None); (message or None,
+    reason) when the worker is dead -- it reported its CUDA context lost, its pipe broke or its process exited; or
+    (None, None) when it has nothing to say.  ``when`` is put after "connection lost" in the reason."""
+    if w.conn in ready:
+        try:
+            msg = w.conn.recv()
+        except (EOFError, OSError):
+            return None, "connection lost%s (exit code %s)" % (when, w.proc.exitcode)
+        return msg, (msg[3] if msg[0] == "dead" else None)
+    if w.proc is not None and w.proc.sentinel in ready and not w.proc.is_alive():
+        return None, "process exited with code %s" % w.proc.exitcode
+    return None, None
+
+
 class ProcessResult:
     """Handle of an asynchronous map on the process pool (``MapResult``, fiber/pool.py:731-743)."""
 
@@ -318,13 +337,10 @@ class ProcessResult:
         self._pool, self._job, self._spec, self._single = pool, job, spec, single
         self._result = None
 
-    def _emit_result(self):
+    def _emit_parts(self):
         """An emit map: the blocks' end offsets rebased by the values of the blocks before them, and their values
         concatenated in block order."""
-        from .pool import EmitResultArray
         job = self._job
-        if job.n == 0:
-            return EmitResultArray(self._spec, np.empty(0, np.uint64), np.empty(0, job.out_dtype))
         ends = job.shm.array[:job.nbytes].view(np.uint64).copy()
         parts, base = [], 0
         for b, (lo, hi) in enumerate(job.ranges):
@@ -337,37 +353,29 @@ class ProcessResult:
             ends[lo:hi] += np.uint64(base)
             base += k
         _unlink_values(job.shm.name, len(job.ranges))
-        return EmitResultArray(self._spec, ends, np.concatenate(parts))
+        return ends, np.concatenate(parts)
 
     def get(self, timeout=None):
-        from .pool import ResultArray
+        from .pool import host_result
         if self._result is None:
             job = self._job
             if not job.event.wait(timeout):
                 raise TimeoutError("map %d not finished" % job.id)
             if job.error is not None:
                 raise job.error
-            dtype, sub = self._spec.result_dtype()
-            total = job.sum if (self._spec.flags & 0x4) else None
-            if job.fold:
-                from .pool import fold_identity
-                raw = bytes(job.shm.array[:job.result_bytes]) if job.n else fold_identity(self._spec)
-                self._result = [self._spec.unpack_result(raw)]
-                if job.shm is not None:
-                    job.shm.release()
-                return self._result[0]
-            if job.out_dtype is not None:
-                self._result = self._emit_result()
-            elif job.n == 0:
-                self._result = ResultArray(self._spec, np.empty((0,) + sub, dtype), 0)
-            elif job.bits:
-                self._result = ResultArray(self._spec, None, total, n=job.n, bits=job.shm.array[:job.nbytes])
-            else:
-                arr = job.shm.array[:job.nbytes].view(dtype).reshape((job.n,) + sub)
-                self._result = ResultArray(self._spec, arr, total)
+            kind = "fold" if job.fold else "emit" if job.out_dtype is not None else "bits" if job.bits else "plain"
+            data = values = None
+            if kind == "emit" and job.n:
+                data, values = self._emit_parts()
+            elif job.n:
+                data = job.shm.array[:job.result_bytes if job.fold else job.nbytes]
+            total = job.sum if (self._spec.flags & _abi.FBR_BODY_SUMMABLE) else None
+            result = host_result(self._spec, kind, data, job.n, total, values)
             if job.shm is not None:
-                self._result._shm = job.shm      # the mapping lives as long as the result; workers are done with the name
+                if not job.fold:
+                    result._shm = job.shm    # the mapping lives as long as the result; workers are done with the name
                 job.shm.release()
+            self._result = (result,) if job.fold else result
         return self._result[0] if self._single else self._result
 
 
@@ -498,15 +506,13 @@ class ProcessPool:
     def _pump_idle(self):
         """No map in flight: take "ready" notes from fresh workers, replace workers that died while idle."""
         waitables = [w.conn for w in self._workers if w.conn is not None]
-        for c in mpc.wait(waitables, timeout=0) if waitables else []:
-            for w in self._workers:
-                if w.conn is c:
-                    try:
-                        msg = c.recv()
-                        if msg and msg[0] == "ready":
-                            w.ready = True
-                    except (EOFError, OSError):
-                        self._on_death(w, "connection lost while idle (exit code %s)" % w.proc.exitcode)
+        ready = mpc.wait(waitables, timeout=0) if waitables else []
+        for w in self._workers:
+            msg, dead_reason = _receive(w, ready, " while idle")
+            if msg is not None and msg[0] == "ready":
+                w.ready = True
+            if dead_reason is not None:
+                self._on_death(w, dead_reason)
 
     def _run(self):
         while True:
@@ -544,38 +550,24 @@ class ProcessPool:
             for w in self._workers:
                 if w.conn is None:
                     continue
-                dead_reason = None
-                if w.conn in ready:
-                    try:
-                        msg = w.conn.recv()
-                    except (EOFError, OSError):
-                        msg, dead_reason = None, "connection lost (exit code %s)" % w.proc.exitcode
-                    if msg is not None:
-                        # a block of an EARLIER map (one that failed while this block was still running) reports late:
-                        # the worker becomes idle again, the current map's accounting is not touched
-                        mine = w.block is not None and w.block[0] is job and msg[0] != "ready" and msg[1] == job.id
-                        if msg[0] == "ready":
-                            w.ready = True
-                        elif not mine:
-                            if msg[0] == "dead":
-                                w.block = None
-                                dead_reason = msg[3]
-                            else:
-                                w.block = None
-                        elif msg[0] == "done":
-                            job.sum += msg[3] or 0
-                            job.done_blocks += 1
-                            w.block = None
-                            inflight -= 1
-                        elif msg[0] == "error":
-                            w.block = None
-                            inflight -= 1
-                            exc = {"OverflowError": OverflowError, "ValueError": ValueError, "TypeError": TypeError}.get(msg[3], RuntimeError)
-                            self._fail(job, exc(msg[4]))
-                        elif msg[0] == "dead":
-                            dead_reason = msg[3]
-                elif w.proc is not None and w.proc.sentinel in ready and not w.proc.is_alive():
-                    dead_reason = "process exited with code %s" % w.proc.exitcode
+                msg, dead_reason = _receive(w, ready)
+                if msg is not None:
+                    # a block of an EARLIER map (one that failed while this block was still running) reports late:
+                    # the worker becomes idle again, the current map's accounting is not touched
+                    mine = w.block is not None and w.block[0] is job and msg[0] != "ready" and msg[1] == job.id
+                    if msg[0] == "ready":
+                        w.ready = True
+                    elif not mine:
+                        w.block = None
+                    elif msg[0] == "done":
+                        job.sum += msg[3] or 0
+                        job.done_blocks += 1
+                        w.block = None
+                        inflight -= 1
+                    elif msg[0] == "error":
+                        w.block = None
+                        inflight -= 1
+                        self._fail(job, _ERRORS.get(msg[3], RuntimeError)(msg[4]))
                 if dead_reason is not None:
                     if w.block is not None and w.block[0] is job:
                         inflight -= 1
@@ -616,29 +608,17 @@ class ProcessPool:
             except (OSError, ValueError):
                 dead_reason = "pipe closed"
             while dead_reason is None:
-                ready = mpc.wait([w.conn, w.proc.sentinel], timeout=0.5)
-                msg = None
-                if w.conn in ready:
-                    try:
-                        msg = w.conn.recv()
-                    except (EOFError, OSError):
-                        dead_reason = "connection lost (exit code %s)" % w.proc.exitcode
-                elif w.proc.sentinel in ready and not w.proc.is_alive():
-                    dead_reason = "process exited with code %s" % w.proc.exitcode
+                msg, dead_reason = _receive(w, mpc.wait([w.conn, w.proc.sentinel], timeout=0.5))
                 if msg is not None and msg[0] == "ready":
                     w.ready = True
                 elif msg is not None and msg[1] == job.id:
                     if msg[0] == "scanned":
                         job.scan_wrapped.add(msg[2])
-                        continue
-                    if msg[0] == "folded":
+                    elif msg[0] == "folded":
                         return
-                    if msg[0] == "error":
-                        exc = {"ValueError": ValueError, "TypeError": TypeError}.get(msg[3], RuntimeError)
-                        self._fail(job, exc(msg[4]))
+                    elif msg[0] == "error":
+                        self._fail(job, _ERRORS.get(msg[3], RuntimeError)(msg[4]))
                         return
-                    if msg[0] == "dead":
-                        dead_reason = msg[3]
             deaths += 1
             self._on_death(w, dead_reason)                      # no block of its own: nothing is re-queued
             if self._terminated:
