@@ -23,6 +23,7 @@ FBR_BODY_INDEX_ARG, FBR_BODY_NEEDS_SHARED, FBR_BODY_SUMMABLE, FBR_BODY_INDEX_ONL
 FBR_BODY_EMIT = 0x80
 FBR_BODY_FOLD = 0x100
 FBR_BODY_SCAN = 0x200
+FBR_BODY_KEYED = 0x400
 FBR_BODY_MODULE_ABI = 4
 MAX_ITEM_STREAMS = 4        # item streams of one items body (fbr_map_submit_items_n)
 # pool flags
@@ -33,17 +34,20 @@ FBR_ARGS_DEVICE, FBR_OUT_DEVICE, FBR_WANT_SUM, FBR_SHUFFLE, FBR_FULL_WINDOW, FBR
     FBR_RESULTS_ON_DEVICE, FBR_VIA_RING, FBR_NO_ZERO_COPY = 0x10, 0x20, 0x40, 0x80, 0x100, 0x200, 0x400, 0x800, 0x1000, 0x2000
 FBR_FOLD = 0x4000
 FBR_SCAN = 0x8000
+FBR_FOLD_KEYS = 0x10000
+FBR_MAX_KEYS = 65536
 FBR_PLAN_FOLD = 0xFFFFFFFF   # fbr_plan_query's chunksize for the plan of a fold map
 # fbr_task_error
 FBR_TASK_OK, FBR_TASK_OVERFLOW, FBR_TASK_BADARG, FBR_TASK_FAULT = range(4)
 FBR_TASK_EMIT = 4
+FBR_TASK_KEY = 5
 
 # every symbol include/fiber_b200.h declares (tests check the .so exports each of them)
 SYMBOLS = [
     "fbr_abi_version", "fbr_last_error", "fbr_device_count",
     "fbr_body_count", "fbr_body_info", "fbr_body_lookup", "fbr_register_body", "fbr_body_shared_info",
     "fbr_body_items_info", "fbr_body_emit_info", "fbr_body_items_streams", "fbr_body_fold_info", "fbr_fold_values",
-    "fbr_scan_values",
+    "fbr_scan_values", "fbr_fold_segments",
     "fbr_pool_create", "fbr_pool_close", "fbr_pool_terminate", "fbr_pool_join", "fbr_pool_destroy",
     "fbr_pool_n_workers", "fbr_pool_worker_device",
     "fbr_map_submit", "fbr_map_submit_items", "fbr_map_submit_items_n", "fbr_shared_put", "fbr_shared_drop", "fbr_plan_query",
@@ -85,7 +89,7 @@ class MapDesc(ctypes.Structure):
                 ("index_start", ctypes.c_int64), ("index_step", ctypes.c_int64),
                 ("shared", ctypes.c_void_p), ("shared_bytes", ctypes.c_uint64), ("out", ctypes.c_void_p),
                 ("task_index_base", ctypes.c_uint64), ("shuffle_seed", ctypes.c_uint64), ("n_items", ctypes.c_uint64),
-                ("attempt", ctypes.c_uint32), ("pad", ctypes.c_uint32)]
+                ("attempt", ctypes.c_uint32), ("n_keys", ctypes.c_uint32)]
 
 
 class ItemsDesc(ctypes.Structure):
@@ -161,6 +165,7 @@ def load():
         "fbr_body_fold_info": (i32, [i32, vp, P(u32)]),
         "fbr_fold_values": (i32, [vp, i32, vp, u64, vp]),
         "fbr_scan_values": (i32, [vp, i32, vp, u32, vp, u64]),
+        "fbr_fold_segments": (i32, [vp, i32, vp, vp, u32, vp]),
         "fbr_pool_create": (i32, [i32, P(i32), u64, u32, P(vp)]),
         "fbr_pool_close": (i32, [vp]),
         "fbr_pool_terminate": (i32, [vp]),

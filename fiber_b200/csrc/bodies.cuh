@@ -30,7 +30,7 @@ enum FuncId : int32_t {
     F_COUNT = 13             // compiled-in bodies; bodies registered at run time (fbr_register_body) get ids from here up
 };
 
-enum TaskError : uint32_t { TASK_OK = 0, TASK_OVERFLOW = 1, TASK_BADARG = 2, TASK_FAULT = 3, TASK_EMIT = 4 };
+enum TaskError : uint32_t { TASK_OK = 0, TASK_OVERFLOW = 1, TASK_BADARG = 2, TASK_FAULT = 3, TASK_EMIT = 4, TASK_KEY = 5 };
 
 // Lowest failing task wins, like the first exception a reference worker would have raised on the
 // lowest index.  Packed as (task_index << 8 | code) so a single atomicMin orders by index.

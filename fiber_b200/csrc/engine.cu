@@ -176,6 +176,8 @@ struct BodyEntry {
     void (*fold)(void*, uint64_t, void*, void*) = nullptr;    // FBR_BODY_FOLD record bodies: tree() over device records ...
     std::vector<uint8_t> identity;                            // ... and identity(), result_bytes bytes
     int (*scan)(void*, uint64_t, int, const void*, uint32_t, void*) = nullptr;   // FBR_BODY_SCAN: prefix folds, wraps
+    int (*keys)(const void*, uint64_t, uint32_t, uint64_t, uint32_t*, unsigned long long*, void*) = nullptr;   // FBR_BODY_KEYED:
+    int (*fold_segments)(void*, uint64_t, const uint64_t*, uint32_t, void*, void*) = nullptr;            // keys, segmented tree()
 };
 
 static std::mutex g_body_mu;
@@ -304,6 +306,9 @@ struct PartCtx {                          // constants of one worker's block of 
     bool fold = false;                    // FBR_FOLD: each unit writes its tree to d_fold, no result leaves the device
     uint8_t* fold_total = nullptr;        // FBR_FOLD: the block's total, in the map's pinned segment
     bool scan = false;                    // FBR_SCAN: the block's window becomes its prefix folds after its last round
+    bool keyed = false;                   // FBR_FOLD_KEYS: the block's window is sorted by key and folded per key after its last
+    uint8_t* key_totals = nullptr;        // round into n_keys totals and counts, in the map's pinned segment
+    uint8_t* key_counts = nullptr;
     const uint8_t* d_shared = nullptr;
     uint8_t* window_base = nullptr;       // device output of a FULL_WINDOW part
     const uint8_t* args_full = nullptr;   // device-resident arguments of the whole map (args_dev / resilient)
@@ -711,7 +716,7 @@ static uint32_t pick_unit(const BodyEntry& b, uint32_t chunksize, uint64_t n_tas
 
 // the chunksize a map's units are picked for: a fold map's units ignore it (FBR_PLAN_FOLD)
 static uint32_t map_chunksize(const fbr_map_desc_t& d) {
-    if (d.flags & (FBR_FOLD | FBR_SCAN)) return FBR_PLAN_FOLD;   // a scan map's block cut is the fold plan's
+    if (d.flags & (FBR_FOLD | FBR_SCAN | FBR_FOLD_KEYS)) return FBR_PLAN_FOLD;   // scan and keyed maps cut blocks as a fold
     return d.chunksize ? d.chunksize : 32u;
 }
 
@@ -1062,6 +1067,82 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
     return FBR_OK;
 }
 
+// FBR_FOLD_KEYS, a block's last round, queued on its worker's s_out behind its last wave: the body's keys entry writes each
+// task's key (a bad one goes into the block's error word), a stable LSD radix sort of (key, task) pairs puts the block's
+// tasks in key order, the records are gathered into that order, key_offsets_kernel finds each key's run and count, and the
+// body's fold_segments entry folds every run into the key's total.  Totals and counts are then copied into the block's area
+// of the pinned segment.  With one key nothing is sorted or gathered: the window is folded in place.  Device scratch, all
+// stream-ordered: 4 B per task of keys (16 B with a sort: keys and task indices, twice), a gathered copy of the window with
+// a sort, the sort's (digit, tile) histogram and its scan (16 B per 256 bins per 4096 tasks), and n_keys * (R + 16) bytes.
+static int fold_block_by_key(fbr_pool* p, SeqState& st, SeqPart& part) {
+    Worker& w = p->workers[part.worker];
+    const BodyEntry& body = *body_of(st.func_id);
+    const PartCtx& cx = part.cx;
+    const cudaStream_t s = w.s_out;
+    const uint32_t K = st.desc.n_keys, n = (uint32_t)part.count;
+    const uint64_t R = body.result_bytes;
+    const int passes = K <= 1 ? 0 : K <= 256 ? 1 : 2;   // 8-bit digits of keys below K
+    const uint32_t n_tiles = (n + keyed::kTile - 1) / keyed::kTile;
+    const uint64_t H = (uint64_t)keyed::kBins * n_tiles, scan_tiles = H / scan::kTile + 1;
+    uint64_t at = 0;
+    auto take = [&](uint64_t bytes) { const uint64_t o = at; at = round_up(at + bytes, 256); return o; };
+    const uint64_t o_keys0 = take(4ull * n), o_keys1 = passes ? take(4ull * n) : 0, o_idx0 = passes ? take(4ull * n) : 0,
+                   o_idx1 = passes ? take(4ull * n) : 0, o_hist = passes ? take(8 * H) : 0, o_hoffs = passes ? take(8 * (H + 1)) : 0,
+                   o_state = passes ? take(8 * (scan_tiles + 2)) : 0, o_gather = passes ? take(n * R) : 0;
+    const uint64_t o_offs = take(8ull * (K + 1)), o_counts = take(8ull * K), o_totals = take(K * R);
+    uint8_t* buf = nullptr;
+    cudaError_t e = cudaMallocAsync((void**)&buf, at, s);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return fail(e == cudaErrorMemoryAllocation ? FBR_ENOMEM : FBR_ECUDA, "keyed fold of body %s on worker %d: %llu bytes of device scratch: %s",
+                    body.name.c_str(), part.worker, (unsigned long long)at, cudaGetErrorString(e));
+    }
+    uint32_t* keys[2] = {(uint32_t*)(buf + o_keys0), (uint32_t*)(buf + o_keys1)};
+    uint32_t* idx[2] = {(uint32_t*)(buf + o_idx0), (uint32_t*)(buf + o_idx1)};
+    uint64_t* const hist = (uint64_t*)(buf + o_hist);
+    uint64_t* const hoffs = (uint64_t*)(buf + o_hoffs);
+    uint64_t* const state = (uint64_t*)(buf + o_state);   // scan_counts_kernel: tile states, ticket, total
+    uint64_t* const offs = (uint64_t*)(buf + o_offs);
+    e = (cudaError_t)body.keys(cx.window_base, n, K, st.desc.task_index_base + part.first, keys[0], &w.d_ctrl[part.ctrl_slot].err, (void*)s);
+    const unsigned sort_grid = (unsigned)std::min<uint32_t>(n_tiles, 1u << 16);
+    int cur = 0;
+    for (int pass = 0; pass < passes && e == cudaSuccess; ++pass, cur ^= 1) {
+        radix_hist_kernel<<<sort_grid, keyed::kThreads, 0, s>>>(keys[cur], n, 8 * pass, hist, n_tiles);
+        e = cudaMemsetAsync(state, 0, 8 * (scan_tiles + 2), s);
+        if (e != cudaSuccess) break;
+        scan_counts_kernel<<<(unsigned)scan_tiles, scan::kThreads, 0, s>>>(hist, H, hoffs, (unsigned long long*)state,
+                                                                          (uint32_t*)(state + scan_tiles), state + scan_tiles + 1);
+        radix_scatter_kernel<<<sort_grid, keyed::kThreads, 0, s>>>(keys[cur], pass ? idx[cur] : nullptr, keys[cur ^ 1], idx[cur ^ 1], n,
+                                                                   8 * pass, hoffs, n_tiles);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) {
+        key_offsets_kernel<<<(unsigned)std::min<uint64_t>((K + kThreads) / kThreads, 1024), kThreads, 0, s>>>(
+            keys[cur], n, K, offs, (uint64_t*)(buf + o_counts));
+        e = cudaGetLastError();
+    }
+    uint8_t* src = cx.window_base;
+    if (e == cudaSuccess && passes) {
+        src = buf + o_gather;
+        const uint32_t W = R % 16 == 0 ? 16 : R % 8 == 0 ? 8 : 4;
+        const uint64_t words = R / W, grid = std::min<uint64_t>((n * words + kThreads - 1) / kThreads, 1u << 16);
+        if (W == 16) gather_records_kernel<uint4><<<(unsigned)grid, kThreads, 0, s>>>((const uint4*)cx.window_base, (uint4*)src, idx[cur], n, (uint32_t)words);
+        else if (W == 8) gather_records_kernel<uint2><<<(unsigned)grid, kThreads, 0, s>>>((const uint2*)cx.window_base, (uint2*)src, idx[cur], n, (uint32_t)words);
+        else gather_records_kernel<uint32_t><<<(unsigned)grid, kThreads, 0, s>>>((const uint32_t*)cx.window_base, (uint32_t*)src, idx[cur], n, (uint32_t)words);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = (cudaError_t)body.fold_segments(src, n, offs, K, buf + o_totals, (void*)s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(cx.key_totals, buf + o_totals, K * R, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(cx.key_counts, buf + o_counts, 8ull * K, cudaMemcpyDeviceToHost, s);
+    cudaFreeAsync(buf, s);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return fail(FBR_ECUDA, "keyed fold of body %s on worker %d: %s", body.name.c_str(), part.worker, cudaGetErrorString(e));
+    }
+    STAT_ADD(p, d2h_bytes, K * (R + 8));
+    return FBR_OK;
+}
+
 // Control block (+ lost list) back to the pinned mirror, completion event.
 static int finish_round(fbr_pool* p, SeqState& st, SeqPart& part, bool copy_window) {
     Worker& w = p->workers[part.worker];
@@ -1078,13 +1159,18 @@ static int finish_round(fbr_pool* p, SeqState& st, SeqPart& part, bool copy_wind
     }
     // a scan block after the first keeps its window on the device: scan_finish wraps it there, then copies it out once
     const bool scan_later = cx.scan && part.first != 0;
-    if (copy_window && cx.full_window && !cx.out_dev && !cx.keep_on_device && !cx.zero_copy && !cx.fold && !scan_later && part.count) {
+    if (copy_window && cx.full_window && !cx.out_dev && !cx.keep_on_device && !cx.zero_copy && !cx.fold && !cx.keyed && !scan_later &&
+        part.count) {
         CK(cudaMemcpyAsync((uint8_t*)st.out + part.first * cx.R, cx.window_base, part.count * cx.R, cudaMemcpyDeviceToHost, w.s_out));
         STAT_ADD(p, d2h_bytes, part.count * cx.R);
     }
     if (copy_window && cx.fold && part.count) {   // the last round: the block's total from its units' partials
         body_of(st.func_id)->fold(part.d_fold, (part.count + cx.unit - 1) / cx.unit, cx.fold_total, (void*)w.s_out);
         CK(cudaGetLastError());
+    }
+    if (copy_window && cx.keyed && part.count) {
+        const int rc = fold_block_by_key(p, st, part);
+        if (rc != FBR_OK) return rc;
     }
     const EmitBlock& e = part.emit;
     if (copy_window && e.host && e.d_values && e.total) {
@@ -1113,7 +1199,8 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
     cx.out_dev = (d.flags & FBR_OUT_DEVICE) != 0;
     cx.fold = (d.flags & FBR_FOLD) != 0;
     cx.scan = (d.flags & FBR_SCAN) != 0;
-    cx.keep_on_device = (d.flags & FBR_RESULTS_ON_DEVICE) != 0 && !cx.fold;
+    cx.keyed = (d.flags & FBR_FOLD_KEYS) != 0;
+    cx.keep_on_device = (d.flags & FBR_RESULTS_ON_DEVICE) != 0 && !cx.fold && !cx.keyed;
     {
         // Output resident on worker 0, computed by another worker: kernels storing over NVLink stay below what a
         // copy engine pushes at the peer-copy rate (TMA bulk or register stores alike).  So the block is
@@ -1133,7 +1220,8 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
     }
     cx.full_window = (cx.out_dev && !cx.peer_out) || cx.resilient || cx.keep_on_device || (d.flags & FBR_FULL_WINDOW) || cx.zero_copy ||
                      cx.fold ||   // a fold block has no output window: nothing is staged or copied out
-                     cx.scan;     // a scan block's results are rewritten in place once all of them are there
+                     cx.scan ||   // a scan block's results are rewritten in place once all of them are there
+                     cx.keyed;    // ... and a keyed block's are sorted by key and folded
     cx.host_args = d.arg_stride != 0 && !cx.args_dev && !cx.resilient;
     {
         // device-resident arguments on worker 0, consumed by another worker: stream them through the staging halves,
@@ -1523,9 +1611,10 @@ static void on_worker_death(fbr_pool* p, int wi, cudaError_t err) {
         if (!touched) continue;
         // device-resident arguments / outputs of a map live on worker 0
         const bool on_w0 = (st.flags & (FBR_ARGS_DEVICE | FBR_OUT_DEVICE)) != 0;
-        // an emit pass's blocks carry the offsets of the workers that counted them, and a fold or scan map's order depends
+        // an emit pass's blocks carry the offsets of the workers that counted them, and a fold, scan or keyed map's order depends
         // on its block cut: both are failed, not re-cut
-        if (!(st.flags & FBR_RESILIENT) || live.empty() || (on_w0 && p->workers[0].dead) || st.emit_pass || (st.flags & (FBR_FOLD | FBR_SCAN))) {
+        if (!(st.flags & FBR_RESILIENT) || live.empty() || (on_w0 && p->workers[0].dead) || st.emit_pass ||
+            (st.flags & (FBR_FOLD | FBR_SCAN | FBR_FOLD_KEYS))) {
             st.dead_worker = wi;
             st.dead_error = (int)err;
             continue;
@@ -1782,6 +1871,14 @@ static std::string descriptor_error(const fbr_body_module_t* m, const char* modu
     } else if (scan && m->scan == nullptr) {
         why = "sets FBR_BODY_SCAN but its descriptor lacks the scan entry";
     }
+    // `keys` and `fold_segments` follow `scan`, and are read only from a descriptor that sets FBR_BODY_KEYED
+    const bool keyed = (m->flags & FBR_BODY_KEYED) != 0;
+    if (why) {
+    } else if (keyed && !fold) {
+        why = "FBR_BODY_KEYED needs FBR_BODY_FOLD (a keyed fold is a fold per key)";
+    } else if (keyed && (m->keys == nullptr || m->fold_segments == nullptr)) {
+        why = "sets FBR_BODY_KEYED but its descriptor lacks the keys or the fold_segments entry";
+    }
     if (why) return strf("module %s: body '%s' %s", module_path, name, why);
     const uint32_t group = m->group_threads;
     if (group > 1 && (group > 32 || (group & (group - 1)) != 0))
@@ -1856,6 +1953,10 @@ int fbr_register_body(const char* name, const char* module_path, const char* ent
         b.identity.assign((const uint8_t*)m->identity, (const uint8_t*)m->identity + m->result_bytes);
     }
     if (m->flags & FBR_BODY_SCAN) b.scan = m->scan;
+    if (m->flags & FBR_BODY_KEYED) {
+        b.keys = m->keys;
+        b.fold_segments = m->fold_segments;
+    }
     b.launch = m->launch; b.occupancy = m->occupancy;
     b.module = h;
     g_bodies.push_back(b);
@@ -2325,6 +2426,21 @@ static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_ite
         if (d->flags & FBR_NO_ZERO_COPY)
             return fail(FBR_EINVAL, "a scan map (FBR_SCAN) always stages its results on the device: FBR_NO_ZERO_COPY does not apply");
     }
+    if (d->flags & FBR_FOLD_KEYS) {
+        if (!(body.flags & FBR_BODY_KEYED))
+            return fail(FBR_EINVAL, "body %s has no key(): its maps cannot fold per key (FBR_FOLD_KEYS needs FBR_BODY_KEYED)", body.name.c_str());
+        if (d->flags & (FBR_FOLD | FBR_SCAN)) return fail(FBR_EINVAL, "FBR_FOLD_KEYS cannot be combined with FBR_FOLD or FBR_SCAN");
+        if (d->out || (d->flags & (FBR_OUT_DEVICE | FBR_WANT_SUM | FBR_NO_ZERO_COPY)))
+            return fail(FBR_EINVAL, "a keyed fold map (FBR_FOLD_KEYS) of body %s owns its result records: no out, FBR_OUT_DEVICE, "
+                        "FBR_WANT_SUM or FBR_NO_ZERO_COPY", body.name.c_str());
+        if (d->n_keys < 1 || d->n_keys > FBR_MAX_KEYS)
+            return fail(FBR_EINVAL, "n_keys %u is not in 1 .. %u", d->n_keys, (unsigned)FBR_MAX_KEYS);
+        if ((uint64_t)d->n_keys * body.result_bytes > p->ring_bytes)
+            return fail(FBR_EINVAL, "n_keys %u records of %u bytes exceed ring_bytes %llu", d->n_keys, body.result_bytes,
+                        (unsigned long long)p->ring_bytes);
+        if (d->n_tasks > 0xffffffffull)   // a block's tasks are sorted as uint32 indices
+            return fail(FBR_EINVAL, "a keyed fold map takes fewer than 2^32 tasks (%llu)", (unsigned long long)d->n_tasks);
+    }
     if ((d->flags & FBR_WANT_SUM) && !(body.flags & FBR_BODY_SUMMABLE))
         return fail(FBR_EINVAL, "body %s results cannot be summed", body.name.c_str());
     if (d->flags & FBR_FOLD) {
@@ -2357,8 +2473,8 @@ static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_ite
         memset(st->items, 0, sizeof st->items);
         st->n_item_streams = items ? n_streams : 0;
         for (uint32_t k = 0; k < st->n_item_streams; ++k) st->items[k] = items[k];
-        const bool fold = (d->flags & FBR_FOLD) != 0;
-        const bool need_segment = !st->out && d->n_tasks && !(d->flags & FBR_RESULTS_ON_DEVICE) && !fold;
+        const bool fold = (d->flags & FBR_FOLD) != 0, keyed = (d->flags & FBR_FOLD_KEYS) != 0;
+        const bool need_segment = !st->out && d->n_tasks && !(d->flags & FBR_RESULTS_ON_DEVICE) && !fold && !keyed;
         // host allocations fail with the sticky error too once a context of this process has died: tell the two apart
         auto died_meanwhile = [&]() {
             bool any = false;
@@ -2385,6 +2501,20 @@ static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_ite
             if (rc != FBR_OK) return rc;
             st->own_out = true;
             for (size_t k = 0; k < st->parts.size(); ++k) st->parts[k].cx.fold_total = (uint8_t*)st->out + (1 + k) * body.result_bytes;
+        }
+        if (keyed) {
+            // the result: n_keys records, then n_keys uint64 counts.  A single block writes its totals and counts there;
+            // several each write theirs to an area of the same layout after it, combined by complete_map
+            const uint64_t K = d->n_keys, area = K * (body.result_bytes + sizeof(uint64_t));
+            const size_t nb = st->parts.size();
+            int rc = pinned_acquire(p, (nb > 1 ? 1 + nb : 1) * area, &st->out);
+            if (rc != FBR_OK) return rc;
+            st->own_out = true;
+            for (size_t k = 0; k < nb; ++k) {
+                uint8_t* const a = (uint8_t*)st->out + (nb > 1 ? 1 + k : 0) * area;
+                st->parts[k].cx.key_totals = a;
+                st->parts[k].cx.key_counts = a + K * body.result_bytes;
+            }
         }
         if (counted) {
             // the emit pass runs over the blocks the count pass counted
@@ -2492,6 +2622,60 @@ static int fold_host_records(fbr_pool* p, const BodyEntry& body, const void* val
     }
     p->stats.h2d_bytes += n * R;
     p->stats.d2h_bytes += R;
+    return FBR_OK;
+}
+
+// tree() of each segment [offsets[k], offsets[k + 1]) of the host records `values` of keyed body `body` into out[k] (host),
+// identity() for an empty segment, on the pool's first live worker's s_fold; blocks until done.  As fold_host_records.
+static int fold_segments_host(fbr_pool* p, const BodyEntry& body, const void* values, const uint64_t* offsets, uint32_t S, void* out) {
+    const uint64_t R = body.result_bytes, n = offsets[S];
+    if (S == 0) return FBR_OK;
+    const int wi = first_live_worker(p);
+    if (wi < 0) return fail(FBR_ECUDA, "every worker of this pool has died");
+    Worker& w = p->workers[wi];
+    uint8_t* d = nullptr;   // the n records, the S results, the S + 1 offsets
+    const uint64_t o_out = n * R, o_offs = round_up(o_out + S * R, 8);
+    cudaError_t e = cudaSetDevice(w.device);
+    if (e == cudaSuccess) e = cudaMallocAsync((void**)&d, o_offs + (S + 1) * 8ull, w.s_fold);
+    if (e == cudaSuccess && n) e = cudaMemcpyAsync(d, values, n * R, cudaMemcpyHostToDevice, w.s_fold);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d + o_offs, offsets, (S + 1) * 8ull, cudaMemcpyHostToDevice, w.s_fold);
+    if (e == cudaSuccess) e = (cudaError_t)body.fold_segments(d, n, (const uint64_t*)(d + o_offs), S, d + o_out, (void*)w.s_fold);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(out, d + o_out, S * R, cudaMemcpyDeviceToHost, w.s_fold);
+    if (d) cudaFreeAsync(d, w.s_fold);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(w.s_fold);
+    if (e != cudaSuccess) {
+        retire_if_dead(p, wi);
+        return fail(FBR_ECUDA, "folding %u segments of %llu records of body %s on worker %d: %s", S, (unsigned long long)n,
+                    body.name.c_str(), wi, cudaGetErrorString(e));
+    }
+    p->stats.h2d_bytes += n * R + (S + 1) * 8ull;
+    p->stats.d2h_bytes += S * R;
+    return FBR_OK;
+}
+
+// FBR_FOLD_KEYS with several blocks, once every block is done: each block's totals and counts are in its area of the pinned
+// segment.  Record k is tree() over the totals of the blocks where key k has tasks, in block order -- one fold_segments_host
+// over the key-major sequence of those totals -- and count k the sum of the blocks' counts.
+static int keyed_finish(fbr_pool* p, SeqState& st) {
+    const BodyEntry& body = *body_of(st.func_id);
+    const uint64_t K = st.desc.n_keys, R = body.result_bytes;
+    const std::vector<SeqPart*> blocks = parts_in_order(st);
+    std::vector<uint64_t> offs(K + 1, 0), counts(K, 0);
+    std::vector<uint8_t> values;
+    for (uint64_t k = 0; k < K; ++k) {
+        offs[k] = values.size() / R;
+        for (const SeqPart* b : blocks) {
+            uint64_t c;
+            memcpy(&c, b->cx.key_counts + k * 8, 8);
+            if (!c) continue;
+            values.insert(values.end(), b->cx.key_totals + k * R, b->cx.key_totals + (k + 1) * R);
+            counts[k] += c;
+        }
+    }
+    offs[K] = values.size() / R;
+    const int rc = fold_segments_host(p, body, values.data(), offs.data(), (uint32_t)K, st.out);
+    if (rc != FBR_OK) return rc;
+    memcpy((uint8_t*)st.out + K * R, counts.data(), K * 8);
     return FBR_OK;
 }
 
@@ -2646,6 +2830,7 @@ static int complete_map(fbr_pool* p, SeqState& st, bool block, bool* ready) {
     int rc = FBR_OK;
     if (st.flags & FBR_FOLD) rc = fold_host_records(p, body, (const uint8_t*)st.out + body.result_bytes, st.parts.size(), st.out);
     else if (st.flags & FBR_SCAN) rc = scan_finish(p, st, block, ready);
+    else if ((st.flags & FBR_FOLD_KEYS) && st.parts.size() > 1) rc = keyed_finish(p, st);
     if (rc != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc;
     st.completed = *ready;
     return FBR_OK;
@@ -2821,7 +3006,7 @@ int fbr_result_poll(fbr_pool_t* p, uint64_t seq, uint64_t* n_done) {
         done += part_done;
         if (part_done < part.count) break;
     }
-    if (st.flags & (FBR_FOLD | FBR_SCAN)) {   // results are final once the map is complete: 0 tasks done until then
+    if (st.flags & (FBR_FOLD | FBR_SCAN | FBR_FOLD_KEYS)) {   // results are final once the map is complete: 0 tasks done until then
         bool ready = false;
         if (done >= st.n_tasks) {                 // every part is done: fold and scan blocks count only then (above)
             const int rc = complete_map(p, st, false, &ready);
@@ -2891,6 +3076,8 @@ int fbr_result_fetch(fbr_pool_t* p, uint64_t seq, uint64_t first, uint64_t count
     if (it == p->seqs.end()) return fail(FBR_ENOENT, "unknown seq %llu", (unsigned long long)seq);
     SeqState& st = *it->second;
     if (st.flags & FBR_FOLD) return fail(FBR_EINVAL, "seq %llu is a fold map: its one result record is fbr_result_t.data", (unsigned long long)seq);
+    if (st.flags & FBR_FOLD_KEYS)
+        return fail(FBR_EINVAL, "seq %llu is a keyed fold map: its records and counts are fbr_result_t.data", (unsigned long long)seq);
     if (!(st.flags & FBR_RESULTS_ON_DEVICE)) return fail(FBR_EINVAL, "seq %llu does not keep its results on the device", (unsigned long long)seq);
     if (first + count > st.n_tasks) return fail(FBR_EINVAL, "range out of bounds");
     const uint64_t R = st.result_bytes;
@@ -2943,6 +3130,19 @@ int fbr_fold_values(fbr_pool_t* p, int func_id, const void* values, uint64_t n, 
     if (!(bp->flags & FBR_BODY_FOLD)) return fail(FBR_EINVAL, "body %s has no combine(): it cannot fold", bp->name.c_str());
     std::lock_guard<std::mutex> g(p->mu);
     return fold_host_records(p, *bp, values, n, out);
+}
+
+int fbr_fold_segments(fbr_pool_t* p, int func_id, const void* values, const uint64_t* offsets, uint32_t n_segments, void* out) {
+    if (!p || !offsets || (n_segments && !out)) return fail(FBR_EINVAL, "NULL argument");
+    const BodyEntry* bp = body_of(func_id);
+    if (!bp) return fail(FBR_EINVAL, "bad func_id %d", func_id);
+    if (!(bp->flags & FBR_BODY_KEYED)) return fail(FBR_EINVAL, "body %s has no key(): it exports no fold_segments entry", bp->name.c_str());
+    if (offsets[0] != 0) return fail(FBR_EINVAL, "offsets[0] must be 0");
+    for (uint32_t k = 0; k < n_segments; ++k)
+        if (offsets[k + 1] < offsets[k]) return fail(FBR_EINVAL, "offsets decrease at segment %u", k);
+    if (offsets[n_segments] && !values) return fail(FBR_EINVAL, "NULL argument");
+    std::lock_guard<std::mutex> g(p->mu);
+    return fold_segments_host(p, *bp, values, offsets, n_segments, out);
 }
 
 int fbr_scan_values(fbr_pool_t* p, int func_id, const void* pieces, uint32_t n_pieces, void* values, uint64_t n) {

@@ -1193,6 +1193,18 @@ struct FoldOf<B, std::void_t<decltype(&B::combine)>> {
     static_assert(std::is_default_constructible<Res>::value, "fold bodies: Res is default-constructible (the fold pass holds "
                   "results in registers)");
 };
+// a keyed fold body: a fold body that also defines `static uint32_t key(const Res&)` (FBR_BODY_KEYED)
+template <class B, class = void>
+struct KeyOf {
+    static constexpr bool kOn = false;
+};
+template <class B>
+struct KeyOf<B, std::void_t<decltype(&B::key)>> {
+    static constexpr bool kOn = true;
+    static_assert(FoldOf<B>::kOn, "keyed bodies: key() needs identity() and combine() (a keyed fold is a fold per key)");
+    static_assert(std::is_same<decltype(&B::key), uint32_t (*)(const typename B::Res&)>::value,
+                  "keyed bodies: key is `__device__ static uint32_t key(const Res& r)`");
+};
 template <class B>
 struct FoldPass : B {
     static constexpr bool kFoldPass = true;
@@ -1821,6 +1833,189 @@ __global__ void __launch_bounds__(scan::kThreads) scan_counts_kernel(const uint6
         offs[n] = run;
         *total = run;
         __threadfence_system();
+    }
+}
+
+// ================================================================================================
+// Keyed folds (FBR_FOLD_KEYS).  After a block's last round its window holds its n results in task order; the body's keys
+// entry (keys_kernel) writes key[i] for each, a stable LSD radix sort of (key, task) pairs puts the tasks in key order, the
+// records are gathered into that order, and the body's fold_segments entry folds each key's run with tree().  The sort is
+// body-independent: 8-bit digits, ceil(log2(n_keys) / 8) passes (0 for one key, 1 up to 256 keys, 2 up to 65536), each a
+// per-tile digit histogram, an exclusive scan over (digit, tile) (scan_counts_kernel), and a stable scatter.  Tasks are
+// uint32 within a block.
+// ================================================================================================
+namespace keyed {
+constexpr int kThreads = 256, kItems = 16, kWarps = kThreads / 32;
+constexpr uint32_t kTile = kThreads * kItems;   // keys per sort tile; warp w of a tile owns its w-th run of 32 * kItems
+constexpr int kBins = 256;
+}  // namespace keyed
+
+// hist[d * n_tiles + t] = number of keys of tile t whose digit (key >> shift) & 255 is d
+__global__ void __launch_bounds__(keyed::kThreads) radix_hist_kernel(const uint32_t* keys, uint32_t n, int shift,
+                                                                     uint64_t* hist, uint32_t n_tiles) {
+    __shared__ uint32_t s_bins[keyed::kBins];
+    for (uint32_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        for (int d = threadIdx.x; d < keyed::kBins; d += keyed::kThreads) s_bins[d] = 0;
+        __syncthreads();
+        const uint32_t base = t * keyed::kTile;
+#pragma unroll 4
+        for (uint32_t k = threadIdx.x; k < keyed::kTile; k += keyed::kThreads)
+            if (base + k < n) atomicAdd(&s_bins[(keys[base + k] >> shift) & 255u], 1u);
+        __syncthreads();
+        for (int d = threadIdx.x; d < keyed::kBins; d += keyed::kThreads) hist[(uint64_t)d * n_tiles + t] = s_bins[d];
+        __syncthreads();
+    }
+}
+
+// Stable scatter of one pass: the key at i goes to offs[d * n_tiles + t] (the exclusive scan of radix_hist_kernel's
+// counts) plus its rank among the keys of digit d before it in tile t.  Each warp ranks its run 32 keys at a time with
+// __match_any_sync and keeps one counter per digit; the warps' counts are scanned in warp order first.  idx_in == nullptr
+// is the identity permutation (the first pass).
+__global__ void __launch_bounds__(keyed::kThreads) radix_scatter_kernel(const uint32_t* keys_in, const uint32_t* idx_in,
+                                                                        uint32_t* keys_out, uint32_t* idx_out, uint32_t n,
+                                                                        int shift, const uint64_t* offs, uint32_t n_tiles) {
+    using keyed::kWarps; using keyed::kBins; using keyed::kItems; using keyed::kTile;
+    __shared__ uint32_t s_cnt[kWarps][kBins];
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    const uint32_t lt = (1u << lane) - 1u;
+    for (uint32_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        for (int d = lane; d < kBins; d += 32) s_cnt[warp][d] = 0;
+        __syncwarp();
+        const uint32_t base = t * kTile + warp * (32u * kItems);
+        uint32_t key[kItems];
+#pragma unroll
+        for (int j = 0; j < kItems; ++j) {
+            const uint32_t i = base + j * 32u + lane;
+            key[j] = i < n ? keys_in[i] : 0u;
+        }
+        // this warp's count of each digit
+#pragma unroll
+        for (int j = 0; j < kItems; ++j) {
+            const bool valid = base + j * 32u + lane < n;
+            const uint32_t d = valid ? (key[j] >> shift) & 255u : 256u;
+            const uint32_t peers = __match_any_sync(0xffffffffu, d);
+            if (valid && (peers & lt) == 0) s_cnt[warp][d] += __popc(peers);
+            __syncwarp();
+        }
+        __syncthreads();
+        // each counter becomes where the warp's first key of that digit goes
+        for (int d = threadIdx.x; d < kBins; d += keyed::kThreads) {
+            uint64_t run = offs[(uint64_t)d * n_tiles + t];
+            for (int w = 0; w < kWarps; ++w) {
+                const uint32_t c = s_cnt[w][d];
+                s_cnt[w][d] = (uint32_t)run;
+                run += c;
+            }
+        }
+        __syncthreads();
+#pragma unroll
+        for (int j = 0; j < kItems; ++j) {
+            const uint32_t i = base + j * 32u + lane;
+            const bool valid = i < n;
+            const uint32_t d = valid ? (key[j] >> shift) & 255u : 256u;
+            const uint32_t peers = __match_any_sync(0xffffffffu, d);
+            if (valid) {
+                const uint32_t at = s_cnt[warp][d] + __popc(peers & lt);
+                keys_out[at] = key[j];
+                idx_out[at] = idx_in ? idx_in[i] : i;
+            }
+            __syncwarp();
+            if (valid && (peers & lt) == 0) s_cnt[warp][d] += __popc(peers);
+            __syncwarp();
+        }
+        __syncthreads();
+    }
+}
+
+// offs[k] = the first place of key k in the n sorted keys (offs[n_keys] = n) and counts[k] = its number of tasks
+__global__ void __launch_bounds__(kThreads) key_offsets_kernel(const uint32_t* sorted, uint32_t n, uint32_t n_keys,
+                                                               uint64_t* offs, uint64_t* counts) {
+    auto lower = [&](uint32_t k) {
+        uint32_t lo = 0, hi = n;
+        while (lo < hi) {
+            const uint32_t mid = lo + (hi - lo) / 2;
+            if (sorted[mid] < k) lo = mid + 1; else hi = mid;
+        }
+        return lo;
+    };
+    for (uint32_t k = blockIdx.x * kThreads + threadIdx.x; k <= n_keys; k += gridDim.x * kThreads) {
+        const uint32_t a = lower(k);
+        offs[k] = a;
+        if (k < n_keys) counts[k] = lower(k + 1) - a;
+    }
+}
+
+// dst record j <- src record perm[j], records of `words` W-byte words (W = 16, 8 or 4, the widest that divides R)
+template <class W>
+__global__ void __launch_bounds__(kThreads) gather_records_kernel(const W* src, W* dst, const uint32_t* perm, uint64_t n,
+                                                                  uint32_t words) {
+    const uint64_t total = n * words;
+    for (uint64_t v = blockIdx.x * (uint64_t)kThreads + threadIdx.x; v < total; v += (uint64_t)gridDim.x * kThreads) {
+        const uint64_t j = v / words, w = v - j * words;
+        dst[v] = src[(uint64_t)perm[j] * words + w];
+    }
+}
+
+// keys_kernel: key[i] = B::key(x[i]) for the n records of a keyed fold body.  A key >= n_keys is stored as 0, so the sort
+// stays in bounds, and min((first_task + i) << 8 | FBR_TASK_KEY) goes into *err (the block's error word).
+template <class B>
+__global__ void __launch_bounds__(kThreads) keys_kernel(const uint8_t* x, uint64_t n, uint32_t n_keys, uint64_t first_task,
+                                                        uint32_t* key, unsigned long long* err) {
+    using Res = typename B::Res;
+    for (uint64_t i = blockIdx.x * (uint64_t)kThreads + threadIdx.x; i < n; i += (uint64_t)gridDim.x * kThreads) {
+        const uint32_t k = B::key(*reinterpret_cast<const Res*>(x + i * sizeof(Res)));
+        if (k >= n_keys) atomicMin(err, (unsigned long long)(((first_task + i) << 8) | TASK_KEY));
+        key[i] = k < n_keys ? k : 0u;
+    }
+}
+
+// Segmented tree(): segment k is records [offs[k], offs[k + 1]) of x.  At level `step` (1, kFoldTile, kFoldTile^2, ...)
+// segment k holds c = ceil(size / step) partial records, step records apart, and is cut into tiles of kFoldTile of them
+// aligned at its start -- aligned subtrees of its tree(), as fold_tree_kernel cuts one array.  seg_tiles_kernel counts
+// each segment's tiles with more than one record; their exclusive scan (scan_counts_kernel) numbers the tiles, and
+// fold_segments_kernel folds tile g of segment k in place, leaving its total at the tile's first record.
+__global__ void __launch_bounds__(kThreads) seg_tiles_kernel(const uint64_t* offs, uint32_t S, uint64_t step, uint64_t* tiles) {
+    for (uint32_t k = blockIdx.x * kThreads + threadIdx.x; k < S; k += gridDim.x * kThreads) {
+        const uint64_t c = (offs[k + 1] - offs[k] + step - 1) / step;
+        tiles[k] = c > 1 ? (c + record::kFoldTile - 1) / record::kFoldTile : 0;
+    }
+}
+
+template <class B>
+__global__ void __launch_bounds__(kThreads) fold_segments_kernel(uint8_t* x, const uint64_t* offs, uint32_t S, uint64_t step,
+                                                                 const uint64_t* tile_offs) {
+    using Res = typename B::Res;
+    constexpr uint32_t T = record::kFoldTile;
+    const uint64_t total = tile_offs[S];
+    const uint64_t stride = step * sizeof(Res);
+    for (uint64_t g = blockIdx.x; g < total; g += gridDim.x) {
+        uint32_t lo = 0, hi = S - 1;   // the last segment whose first tile is <= g
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi + 1) / 2;
+            if (tile_offs[mid] <= g) lo = mid; else hi = mid - 1;
+        }
+        const uint64_t b = g - tile_offs[lo];
+        const uint64_t c_seg = (offs[lo + 1] - offs[lo] + step - 1) / step;
+        uint8_t* const base = x + offs[lo] * sizeof(Res) + b * T * stride;
+        const uint32_t c = (uint32_t)(c_seg - b * T < T ? c_seg - b * T : T);
+        for (uint32_t s = 1; s < c; s <<= 1) {
+            for (uint32_t j = threadIdx.x * 2u * s; j + s < c; j += kThreads * 2u * s)
+                B::combine(*reinterpret_cast<Res*>(base + j * stride), *reinterpret_cast<const Res*>(base + (j + s) * stride));
+            __syncthreads();
+        }
+    }
+}
+
+// dst[k] <- segment k's total (its first record), or the identity record for an empty segment; one warp per segment
+template <class B>
+__global__ void __launch_bounds__(kThreads) fold_segments_out_kernel(const uint8_t* x, const uint64_t* offs, uint32_t S,
+                                                                     uint8_t* dst, const uint8_t* identity) {
+    constexpr uint32_t R = sizeof(typename B::Res);
+    const uint32_t lane = threadIdx.x & 31u;
+    for (uint64_t k = (blockIdx.x * (uint64_t)kThreads + threadIdx.x) / 32; k < S; k += (uint64_t)gridDim.x * (kThreads / 32)) {
+        const uint8_t* src = offs[k + 1] > offs[k] ? x + offs[k] * R : identity;
+        for (uint32_t w = lane * 4; w < R; w += 32 * 4)
+            *reinterpret_cast<uint32_t*>(dst + k * R + w) = *reinterpret_cast<const uint32_t*>(src + w);
     }
 }
 

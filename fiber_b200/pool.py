@@ -281,14 +281,39 @@ class EmitResultArray(ResultArray):
                         % self._spec.name)
 
 
+class KeyedResultArray(ResultArray):
+    """The result of a keyed fold (``Pool.fold_by_key``): record k is the fold of the results whose ``key()`` is k, read like
+    a map result, and ``counts`` (uint64 per key) the number of tasks of each key."""
+
+    def __init__(self, spec, array, counts):
+        super().__init__(spec, array)
+        self._counts = counts
+
+    @property
+    def counts(self):
+        return self._counts
+
+    def __repr__(self):
+        return "KeyedResultArray(%s%s, n_keys=%d, body=%s)" % (self[:6], "..." if len(self) > 6 else "", len(self), self._spec.name)
+
+
 def host_result(spec, kind, data, n=0, total=None, values=None):
     """What a finished map whose results are in host memory returns, in either isolation.  ``kind`` is "plain", "bits"
-    (one bit per bool result), "emit" (variable-length results) or "fold"; ``spec`` is the body the caller mapped; ``n``
-    the number of results the caller sees.  ``data`` holds the result records as uint8 (the bit-packed bytes, the end
-    offsets of an emit map, a fold's one record), or is None for a map over no tasks; ``values`` are an emit map's
-    values; ``total`` is the device-side sum, or None."""
+    (one bit per bool result), "emit" (variable-length results), "fold" or "keyed"; ``spec`` is the body the caller mapped;
+    ``n`` the number of results the caller sees (a keyed fold's n_keys).  ``data`` holds the result records as uint8 (the
+    bit-packed bytes, the end offsets of an emit map, a fold's one record, a keyed fold's n records then n uint64 counts),
+    or is None for a map over no tasks; ``values`` are an emit map's values; ``total`` is the device-side sum, or None."""
     if kind == "fold":
         return spec.unpack_result(fold_identity(spec) if data is None else bytes(data))
+    if kind == "keyed":
+        dtype, sub = spec.result_dtype()
+        if data is None:        # no task: every key gets identity()
+            records = np.frombuffer(fold_identity(spec) * n, np.uint8)
+            counts = np.zeros(n, np.uint64)
+        else:
+            records = data[:n * spec.result_bytes]
+            counts = data[n * spec.result_bytes:n * (spec.result_bytes + 8)].copy().view(np.uint64)
+        return KeyedResultArray(spec, records.view(dtype).reshape((n,) + sub), counts)
     if kind == "emit":
         if data is None:
             return EmitResultArray(spec, np.empty(0, np.uint64), np.empty(0, spec.out_dtype))
@@ -301,9 +326,23 @@ def host_result(spec, kind, data, n=0, total=None, values=None):
     return ResultArray(spec, data.view(dtype).reshape((n,) + sub), total)
 
 
-def _raise_task_error(name, code, task, emit_count=None):
+def _n_keys(n_keys):
+    """``n_keys`` of a keyed fold as an int in 1 .. FBR_MAX_KEYS: any integer (a NumPy one too), never a bool."""
+    try:
+        k = operator.index(n_keys) if not isinstance(n_keys, (bool, np.bool_)) else None
+    except TypeError:
+        k = None
+    if k is None or not 1 <= k <= _abi.FBR_MAX_KEYS:
+        raise ValueError("n_keys must be an int in 1 .. %d, not %r" % (_abi.FBR_MAX_KEYS, n_keys))
+    return k
+
+
+def _raise_task_error(name, code, task, emit_count=None, n_keys=None):
     """Raise the exception of a map's first failed task (``err_code`` / ``err_task`` of its fbr_result_t) for body
-    ``name``; ``emit_count(task)`` gives the number of values an emit body's task was counted to push."""
+    ``name``; ``emit_count(task)`` gives the number of values an emit body's task was counted to push, and ``n_keys`` is a
+    keyed fold's number of keys."""
+    if code == _abi.FBR_TASK_KEY:
+        raise ValueError("%s: key() of task %d is not below n_keys=%d" % (name, task, n_keys))
     if code == _abi.FBR_TASK_EMIT:
         raise RuntimeError("%s: task %d emitted another number of values than the %d its count pass gave"
                            % (name, task, emit_count(task)))
@@ -318,16 +357,17 @@ def _raise_task_error(name, code, task, emit_count=None):
 class MapResult:
     """Handle of an asynchronous map (fiber/pool.py:731-743)."""
 
-    def __init__(self, pool, engine, spec, seq, n, keepalive, flags=0, user_spec=None, n_items=None):
+    def __init__(self, pool, engine, spec, seq, n, keepalive, flags=0, user_spec=None, n_items=None, n_keys=0):
         """``flags``: the map's FBR_* flags.  A bit-packed map runs ``spec``, the bit-packed twin of the bool body
-        ``user_spec`` the caller mapped, over ``n`` = ceil(n_items / 8) byte tasks."""
+        ``user_spec`` the caller mapped, over ``n`` = ceil(n_items / 8) byte tasks.  ``n_keys``: a keyed fold's keys."""
         self._pool, self._engine, self._spec, self._seq, self._n = pool, engine, spec, seq, n
         self._keepalive = keepalive   # argument buffers must outlive the asynchronous H2D copies
         self._flags = flags
         self._user_spec = user_spec or spec
         self._n_items = n if n_items is None else n_items      # the items the caller mapped
-        self._kind = "fold" if flags & _abi.FBR_FOLD else "bits" if user_spec is not None else \
-            "emit" if spec.flags & _abi.FBR_BODY_EMIT else "plain"
+        self._n_keys = n_keys
+        self._kind = "fold" if flags & _abi.FBR_FOLD else "keyed" if flags & _abi.FBR_FOLD_KEYS else \
+            "bits" if user_spec is not None else "emit" if spec.flags & _abi.FBR_BODY_EMIT else "plain"
         self._result = None
         self._exc = None              # a task error is raised again by every later get()
         self._segment = _Segment(engine, seq) if n else None   # owns the seq from submission on
@@ -339,7 +379,7 @@ class MapResult:
         if self._exc is not None:
             raise self._exc
         if self._n == 0:
-            self._result = host_result(self._user_spec, self._kind, None)
+            self._result = host_result(self._user_spec, self._kind, None, self._n_keys)
             return self._result
         res = self._engine_wait(timeout)
         # exact, unbounded sum: the device folds the two halves of int64 results separately (nothing wraps)
@@ -348,6 +388,9 @@ class MapResult:
         if self._kind == "fold":
             self.raw = ctypes.string_at(res.data, res.result_bytes)     # process-isolated pools ship these bytes
             self._result = host_result(self._spec, "fold", self.raw)
+        elif self._kind == "keyed":         # n_keys records, then n_keys uint64 counts
+            self.raw = ctypes.string_at(res.data, self._n_keys * (res.result_bytes + 8))
+            self._result = host_result(self._spec, "keyed", np.frombuffer(self.raw, np.uint8), self._n_keys)
         elif self._flags & _abi.FBR_RESULTS_ON_DEVICE:
             self._result = self._device_result(res, dsum)
         else:
@@ -393,7 +436,8 @@ class MapResult:
             raise TimeoutError("map %d not finished" % self._seq)
         if rc == _abi.FBR_ETASK:
             try:
-                _raise_task_error(self._user_spec.name, res.err_code, res.err_task, lambda task: self._emit_count(res, task))
+                _raise_task_error(self._user_spec.name, res.err_code, res.err_task, lambda task: self._emit_count(res, task),
+                                  self._n_keys)
             except Exception as e:      # noqa: BLE001 -- remembered: later get() calls raise it without touching the engine
                 self._exc = e
                 raise
@@ -482,6 +526,14 @@ class FoldResult(MapResult):
 
     def _iter_ready(self):
         raise TypeError("%s: a fold has one result, not one per task: use get()" % self._spec.name)
+
+
+class KeyedFoldResult(MapResult):
+    """Handle of an asynchronous keyed fold (``Pool.fold_by_key_async``): ``get()`` returns a KeyedResultArray of n_keys
+    records and their counts (FBR_FOLD_KEYS in include/fiber_b200.h)."""
+
+    def _iter_ready(self):
+        raise TypeError("%s: a keyed fold has one result per key, not one per task: use get()" % self._spec.name)
 
 
 class ApplyResult(MapResult):
@@ -706,7 +758,8 @@ class Pool:
             eng.lib.fbr_shared_drop(eng.handle, old)
         return h.value
 
-    def _submit(self, func, enc, kind, chunksize, cls=MapResult, want_sum=True, extra_flags=0, spec=None, user_spec=None):
+    def _submit(self, func, enc, kind, chunksize, cls=MapResult, want_sum=True, extra_flags=0, spec=None, user_spec=None,
+                n_keys=0):
         spec = spec or registry.spec(registry.body_name_of(func))
         eng = self._engine
         d = _abi.MapDesc()
@@ -741,6 +794,7 @@ class Pool:
         d.n_items = enc.n_items
         d.task_index_base = enc.task_index_base
         d.attempt = self._attempt
+        d.n_keys = n_keys
         d.flags = flags
         seq = ctypes.c_uint64(0)
         if enc.n and enc.streams is not None:
@@ -754,31 +808,36 @@ class Pool:
             _abi.check(eng.lib.fbr_map_submit(eng.handle, ctypes.byref(d), ctypes.byref(seq)))
         n_items = enc.n if user_spec is None else enc.n_items
         self.sent_tasks += n_items
-        return cls(self, eng, spec, seq.value, enc.n, keep, flags, user_spec, n_items)
+        return cls(self, eng, spec, seq.value, enc.n, keep, flags, user_spec, n_items, n_keys)
 
     @staticmethod
     def _spec_of(func):
         return registry.spec(registry.body_name_of(func))
 
-    def _start(self, func, iterable, *, star, mode, chunksize=None, streaming=False):
-        """The one submission path of maps (``mode`` "map"), folds and accumulates of ``func`` over ``iterable``, whose
-        items are argument tuples with ``star``: a MapResult, or a FoldResult for a fold."""
+    def _start(self, func, iterable, *, star, mode, chunksize=None, streaming=False, n_keys=0):
+        """The one submission path of maps (``mode`` "map"), folds, keyed folds ("fold_by_key") and accumulates of ``func``
+        over ``iterable``, whose items are argument tuples with ``star``: a MapResult, a FoldResult for a fold, or a
+        KeyedFoldResult for a keyed fold."""
         self._check_running()
         if chunksize is None:
             chunksize = DEFAULT_CHUNKSIZE if mode == "map" else 0     # a fold's order does not depend on a chunksize
-        spec = self._spec_of(func) if mode == "map" else self._fold_spec(func, scan=mode == "accumulate")
+        spec = self._spec_of(func) if mode == "map" else \
+            self._fold_spec(func, scan=mode == "accumulate", keyed=mode == "fold_by_key")
+        if mode == "fold_by_key":
+            n_keys = _n_keys(n_keys)
         if not hasattr(iterable, "__len__"):
             iterable = list(iterable)
         self.lazy_start_workers(func)
         if self._proc is not None:
-            return self._submit_proc(spec, ("star" if star else "") + mode, iterable, chunksize)
+            return self._submit_proc(spec, ("star" if star else "") + mode, iterable, chunksize, n_keys)
         # imap wants ordered prefixes as they complete: results are staged and copied out wave by wave instead of being
         # stored straight into the pinned segment by one kernel (zero copy, final only when the whole block is)
         cls, want_sum, flags = {"map": (MapResult, True, _abi.FBR_NO_ZERO_COPY if streaming else 0),
                                 "fold": (FoldResult, False, _abi.FBR_FOLD),
+                                "fold_by_key": (KeyedFoldResult, False, _abi.FBR_FOLD_KEYS),
                                 "accumulate": (MapResult, False, _abi.FBR_SCAN)}[mode]
         if mode != "map" and len(iterable) == 0:          # identity() / no prefixes: nothing to bind or submit
-            return cls(self, self._engine, spec, 0, 0, None, flags)
+            return cls(self, self._engine, spec, 0, 0, None, flags, n_keys=n_keys)
         enc = spec.encode_starmap(iterable) if star else spec.encode_map(iterable)
         kind = _abi.FBR_STARMAP if star else _abi.FBR_MAP
         if mode == "map" and self._results_bits and spec.name in registry.BITS_TWIN:
@@ -787,18 +846,19 @@ class Pool:
             twin = registry.spec(registry.BITS_TWIN[spec.name])
             return self._submit(func, twin.from_encoded(enc), kind, max(1, chunksize // 8), extra_flags=flags, spec=twin,
                                 user_spec=spec)
-        return self._submit(func, enc, kind, chunksize, cls=cls, want_sum=want_sum, extra_flags=flags, spec=spec)
+        return self._submit(func, enc, kind, chunksize, cls=cls, want_sum=want_sum, extra_flags=flags, spec=spec, n_keys=n_keys)
 
-    def _submit_proc(self, spec, kind, items, chunksize):
+    def _submit_proc(self, spec, kind, items, chunksize, n_keys=0):
         """Process-isolated workers: the map is cut into blocks that worker processes pull (procpool.py).  ``kind`` is the
-        block kind: "map", "apply", "fold" or "accumulate", with "star" in front for argument tuples."""
+        block kind: "map", "apply", "fold", "fold_by_key" (with ``n_keys``) or "accumulate", with "star" in front for
+        argument tuples."""
         if (kind.startswith("star") and not isinstance(items, registry.Columns)) or \
                 not isinstance(items, (range, list, np.ndarray, registry.Ragged, registry.Columns)):
             items = list(items)         # a Ragged (or Columns) stays one: its blocks are slices with rebased offsets
         if kind == "map" and len(items):
             spec.encode_map(items[:1] if not isinstance(items, range) else items)      # argument validation up front
         twin = registry.BITS_TWIN.get(spec.name) if self._results_bits and kind in ("map", "starmap") else None
-        r = self._proc.submit(spec, twin, kind, items, chunksize, single=kind in ("apply", "fold", "starfold"))
+        r = self._proc.submit(spec, twin, kind, items, chunksize, single=kind in ("apply", "fold", "starfold"), n_keys=n_keys)
         self.sent_tasks += len(items)
         return r
 
@@ -817,7 +877,7 @@ class Pool:
         return self.starmap_async(func, iterable, chunksize).get()
 
     # -- folds: a map reduced on the device with the body's combine() ------------------------------------------------
-    def _fold_spec(self, func, scan=False):
+    def _fold_spec(self, func, scan=False, keyed=False):
         spec = self._spec_of(func)
         if not spec.flags & _abi.FBR_BODY_FOLD:
             if not spec.flags & _abi.FBR_BODY_RECORD:
@@ -828,6 +888,9 @@ class Pool:
         if scan and not spec.flags & _abi.FBR_BODY_SCAN:
             raise TypeError("%s cannot accumulate: its module exports no scan entry (rebuild it with "
                             "FBR_EXPORT_RECORD_BODY)" % spec.name)
+        if keyed and not spec.flags & _abi.FBR_BODY_KEYED:
+            raise TypeError("%s cannot fold by key: it has no key() (a fold body groups its results when it defines "
+                            "`__device__ static uint32_t key(const Res& r)` next to combine())" % spec.name)
         return spec
 
     def fold_async(self, func, iterable):
@@ -844,6 +907,25 @@ class Pool:
 
     def starfold(self, func, iterable):
         return self.starfold_async(func, iterable).get()
+
+    # -- keyed folds: a fold per key() of the results, on the device -------------------------------------------------
+    def fold_by_key_async(self, func, iterable, n_keys):
+        """A fold of the results of each key: a KeyedFoldResult whose ``get()`` gives a KeyedResultArray of ``n_keys``
+        records, record k the fold of the results whose body ``key()`` is k in the order of FBR_FOLD_KEYS
+        (include/fiber_b200.h) -- on one worker ``fold(func, [x for x in iterable if key(func(x)) == k])`` bit for bit, and
+        identity() for a key without tasks -- and ``counts``, the tasks of each key.  There is no chunksize, as for
+        ``fold``.  A task whose key is not below ``n_keys`` raises ValueError."""
+        return self._start(func, iterable, star=False, mode="fold_by_key", n_keys=n_keys)
+
+    def fold_by_key(self, func, iterable, n_keys):
+        return self.fold_by_key_async(func, iterable, n_keys).get()
+
+    def starfold_by_key_async(self, func, iterable, n_keys):
+        """``fold_by_key_async`` over argument tuples, bound as ``starmap`` binds them."""
+        return self._start(func, iterable, star=True, mode="fold_by_key", n_keys=n_keys)
+
+    def starfold_by_key(self, func, iterable, n_keys):
+        return self.starfold_by_key_async(func, iterable, n_keys).get()
 
     # -- accumulates: every prefix of a fold, on the device ------------------------------------------------------------
     def accumulate_async(self, func, iterable):

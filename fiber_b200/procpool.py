@@ -180,6 +180,9 @@ def gpu_worker_main(device, conn, results, sys_path, init=None):
         if msg[0] == "scan":
             _scan_blocks_in_worker(pool, conn, segments, msg)
             continue
+        if msg[0] == "keyed":
+            _fold_keyed_totals_in_worker(pool, conn, segments, msg)
+            continue
         _, job, blk, body, kind, chunksize, payload, shm_name, off, attempt, module = msg
         with _reporting(conn, job, blk):
             _register(body, module)
@@ -191,10 +194,12 @@ def gpu_worker_main(device, conn, results, sys_path, init=None):
             mode = kind.removeprefix("star")
             if mode == "apply":
                 handle = pool.apply_async(f, items[0][0], items[0][1])
+            elif mode == "fold_by_key":                            # a keyed block's parameter is n_keys, not a chunksize
+                handle = pool._start(f, items, star=mode != kind, mode=mode, n_keys=chunksize)
             else:
                 handle = pool._start(f, items, star=mode != kind, mode=mode, chunksize=chunksize)
             res = handle._wait()
-            if mode == "fold":                                     # the block's total, R bytes
+            if mode in ("fold", "fold_by_key"):                    # the block's total (R bytes), or its n_keys totals and counts
                 raw = np.frombuffer(handle.raw, np.uint8)
             else:
                 raw = res.packed if res.packed is not None else np.ascontiguousarray(np.asarray(res)).view(np.uint8).reshape(-1)
@@ -265,6 +270,40 @@ def _fold_totals_in_worker(pool, conn, segments, msg):
         conn.send(("folded", job))
 
 
+def keyed_sequence(areas, n_keys, R):
+    """The key-major sequence of the non-empty block totals of a keyed fold, its n_keys + 1 offsets, and the summed counts.
+    ``areas`` are the blocks' areas in block order, each n_keys records of R bytes then n_keys uint64 counts (uint8)."""
+    counts = [np.array(a[n_keys * R:n_keys * (R + 8)]).view(np.uint64) for a in areas]
+    recs = [np.asarray(a[:n_keys * R]).reshape(n_keys, R) for a in areas]
+    order = [(k, b) for k in range(n_keys) for b in range(len(areas)) if counts[b][k]]
+    per_key = np.bincount([k for k, _ in order], minlength=n_keys)
+    offsets = np.concatenate([[0], np.cumsum(per_key)]).astype(np.uint64)
+    values = np.concatenate([recs[b][k] for k, b in order]) if order else np.zeros(0, np.uint8)
+    return values, offsets, np.sum(counts, axis=0, dtype=np.uint64)
+
+
+def _fold_keyed_totals_in_worker(pool, conn, segments, msg):
+    """A keyed fold map's last step, in the worker the master picked: the n_blocks areas after the result area of the map's
+    segment (each n_keys totals, then n_keys counts) become the result area -- record k is tree() over the totals of the
+    blocks where key k has tasks, in block order (fbr_fold_segments), and count k the sum of the blocks' counts."""
+    from fiber_b200 import registry
+    _, job, n_blocks, n_keys, body, shm_name, module = msg
+    with _reporting(conn, job, -1):
+        _register(body, module)
+        spec = registry.spec(body)
+        R = spec.result_bytes
+        area = n_keys * (R + 8)
+        seg = _attach(segments, shm_name)
+        values, offsets, counts = keyed_sequence([seg.array[(1 + b) * area:(2 + b) * area] for b in range(n_blocks)], n_keys, R)
+        out = np.zeros(n_keys * R, np.uint8)
+        values = np.ascontiguousarray(values)
+        _abi.check(pool._engine.lib.fbr_fold_segments(pool._engine.handle, spec.func_id, values.ctypes.data, offsets.ctypes.data,
+                                                      n_keys, out.ctypes.data))
+        seg.array[:n_keys * R] = out
+        seg.array[n_keys * R:area] = counts.view(np.uint8)
+        conn.send(("folded", job))
+
+
 # ------------------------------------------------------------------------------------------------
 # master side
 # ------------------------------------------------------------------------------------------------
@@ -277,10 +316,16 @@ class _Worker:
 
 
 class _Job:
-    def __init__(self, jid, body, kind, chunksize, n, result_bytes, bits, blocks, payload_of, module, out_dtype=None):
+    def __init__(self, jid, body, kind, chunksize, n, result_bytes, bits, blocks, payload_of, module, out_dtype=None, n_keys=0):
         self.id, self.body, self.kind, self.chunksize, self.n = jid, body, kind, chunksize, n
         # fold maps: the segment holds the result record, then each block's total in block order
         self.fold = kind in ("fold", "starfold")
+        # keyed fold maps: the result area (n_keys records, then n_keys uint64 counts), then each block's area in block
+        # order; a keyed block's parameter (the block message's chunksize) is n_keys
+        self.keyed = kind in ("fold_by_key", "starfold_by_key")
+        self.n_keys = n_keys
+        if self.keyed:
+            self.chunksize = n_keys
         # accumulate maps: each block places its own prefix folds like a map; blocks after the first are wrapped at the end
         self.scan = kind in ("accumulate", "staraccumulate")
         self.scan_wrapped = set()                     # blocks (b > 0) already wrapped and placed
@@ -291,7 +336,8 @@ class _Job:
         self.blocks = collections.deque(blocks)       # (blk id, lo, hi, attempt)
         self.n_blocks, self.done_blocks = len(blocks), 0
         self.payload_of, self.module = payload_of, module
-        nbytes = ((n + 7) // 8) if bits else ((1 + len(blocks)) * result_bytes if self.fold else n * result_bytes)
+        nbytes = ((n + 7) // 8) if bits else ((1 + len(blocks)) * result_bytes if self.fold else
+                                              (1 + len(blocks)) * n_keys * (result_bytes + 8) if self.keyed else n * result_bytes)
         self.shm = SharedSegment("fbr_%d_%d_%d" % (os.getpid(), jid, int(time.time() * 1e6) & 0xFFFFFF), nbytes) if n else None
         self.nbytes = nbytes
         self.sum, self.error = 0, None
@@ -304,6 +350,8 @@ class _Job:
     def offset(self, lo, blk):
         if self.fold:
             return (1 + blk) * self.result_bytes
+        if self.keyed:
+            return (1 + blk) * self.n_keys * (self.result_bytes + 8)
         return lo // 8 if self.bits else lo * self.result_bytes
 
 
@@ -363,14 +411,16 @@ class ProcessResult:
                 raise TimeoutError("map %d not finished" % job.id)
             if job.error is not None:
                 raise job.error
-            kind = "fold" if job.fold else "emit" if job.out_dtype is not None else "bits" if job.bits else "plain"
+            kind = "fold" if job.fold else "keyed" if job.keyed else "emit" if job.out_dtype is not None else \
+                "bits" if job.bits else "plain"
             data = values = None
             if kind == "emit" and job.n:
                 data, values = self._emit_parts()
             elif job.n:
-                data = job.shm.array[:job.result_bytes if job.fold else job.nbytes]
+                data = job.shm.array[:job.result_bytes if job.fold else
+                                     job.n_keys * (job.result_bytes + 8) if job.keyed else job.nbytes]
             total = job.sum if (self._spec.flags & _abi.FBR_BODY_SUMMABLE) else None
-            result = host_result(self._spec, kind, data, job.n, total, values)
+            result = host_result(self._spec, kind, data, job.n_keys if job.keyed else job.n, total, values)
             if job.shm is not None:
                 if not job.fold:
                     result._shm = job.shm    # the mapping lives as long as the result; workers are done with the name
@@ -445,8 +495,14 @@ class ProcessPool:
         before them, so record i of block b is tree(t_0, ..., t_{b-1}, p_i) over the blocks of ``fold_blocks``."""
         return self.submit(spec, None, "accumulate" if kind == "map" else "staraccumulate", items, 0)
 
-    def submit(self, spec, twin, kind, items, chunksize, single=False):
-        """items: a ``range`` or a list/array of per-task items (tuples for starmap)."""
+    def submit_fold_by_key(self, spec, kind, items, n_keys):
+        """A keyed fold map (``kind`` "map" or "starmap"): each block runs ``Pool.fold_by_key`` in its worker and places its
+        n_keys totals and counts; once every block is in, one live worker folds each key's non-empty totals in block order
+        (fbr_fold_segments) and sums the counts."""
+        return self.submit(spec, None, "fold_by_key" if kind == "map" else "starfold_by_key", items, 0, n_keys=n_keys)
+
+    def submit(self, spec, twin, kind, items, chunksize, single=False, n_keys=0):
+        """items: a ``range`` or a list/array of per-task items (tuples for starmap).  ``n_keys``: a keyed fold's keys."""
         from . import registry
         n = len(items)
         bits = twin is not None
@@ -463,7 +519,7 @@ class ProcessPool:
                 raise ValueError("Pool is not running")
             self._next_job += 1
             job = _Job(self._next_job, spec.name, kind, chunksize, n, spec.result_bytes, bits, blocks, payload_of,
-                       registry.module_of(spec.name), getattr(spec, "out_dtype", None))
+                       registry.module_of(spec.name), getattr(spec, "out_dtype", None), n_keys)
             if n == 0:
                 job.event.set()
             else:
@@ -572,13 +628,14 @@ class ProcessPool:
                     if w.block is not None and w.block[0] is job:
                         inflight -= 1
                     self._on_death(w, dead_reason)
-        if (job.fold or (job.scan and job.n_blocks > 1)) and job.n and job.error is None:
+        if (job.fold or job.keyed or (job.scan and job.n_blocks > 1)) and job.n and job.error is None:
             self._fold_totals(job)
         job.event.set()
 
     def _fold_totals(self, job):
         """A fold map whose blocks have all placed their totals: one live worker folds them in block order into the result
-        record; an accumulate map's wraps every block after the first (_scan_blocks_in_worker).  This runs after close()
+        record; a keyed fold map's per key (_fold_keyed_totals_in_worker); an accumulate map's wraps every block after the
+        first (_scan_blocks_in_worker).  This runs after close()
         too, like the blocks of queued maps; terminate() abandons it.  A worker that dies meanwhile is replaced and the fold goes to the next live one, as a block would be re-queued: without error_handling
         the first death fails the map, and MAX_ATTEMPTS deaths fail it in any case.  The map always ends folded or failed."""
         deaths = 0
@@ -603,6 +660,8 @@ class ProcessPool:
                         job.scan_totals = b"".join(bytes(job.shm.array[(hi - 1) * R:hi * R]) for _, hi in job.ranges)
                     todo = [b for b in range(1, job.n_blocks) if b not in job.scan_wrapped]
                     w.conn.send(("scan", job.id, job.ranges, todo, job.scan_totals, job.body, job.shm.name, job.module))
+                elif job.keyed:
+                    w.conn.send(("keyed", job.id, job.n_blocks, job.n_keys, job.body, job.shm.name, job.module))
                 else:
                     w.conn.send(("fold", job.id, job.n_blocks, job.body, job.shm.name, job.module))
             except (OSError, ValueError):

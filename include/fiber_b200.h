@@ -92,6 +92,9 @@ typedef enum fbr_result_kind {
                                      the fold (FBR_SCAN, fbr_scan_values).  Set exactly when `scan` is exported, and only
                                      with FBR_BODY_FOLD; `scan` is read only from descriptors that set it, so a fold
                                      descriptor that ends at identity_bytes stays a valid fold body */
+#define FBR_BODY_KEYED 0x400u     /* FBR_BODY_FOLD body with key(): its maps may fold per key (FBR_FOLD_KEYS, fbr_fold_segments).
+                                     Set exactly when the descriptor exports `keys` and `fold_segments`, and only with
+                                     FBR_BODY_FOLD; both are read only from descriptors that set it */
 
 typedef struct fbr_body_info {
     int32_t func_id;
@@ -157,6 +160,15 @@ typedef struct fbr_body_module {
        (scan_level_kernel, scan_wrap_kernel, and stream-ordered scratch of fewer than n records); returns the launch's
        cudaError_t.  Left out of (or NULL in) a descriptor without FBR_BODY_SCAN */
     int (*scan)(void* values, uint64_t n, int prefix, const void* pieces, uint32_t n_pieces, void* cuda_stream);
+    /* FBR_BODY_KEYED bodies, both queued on `cuda_stream` and returning the launch's cudaError_t.  `keys`: keys[i] = key() of
+       the n device records at `values`; a key >= n_keys is stored as 0, and the lowest such task, first_task + i, goes into
+       the device word *err as min(*err, (task << 8) | FBR_TASK_KEY).  `fold_segments`: the n device records at `values` are
+       in key order (overwritten); dst[k] (device-accessible) <- tree() of records [offsets[k], offsets[k + 1]) for each of
+       the n_segments segments, identity() for an empty one; `offsets` are n_segments + 1 non-decreasing device words.  Left
+       out of (or NULL in) a descriptor without FBR_BODY_KEYED */
+    int (*keys)(const void* values, uint64_t n, uint32_t n_keys, uint64_t first_task, uint32_t* keys, unsigned long long* err,
+                void* cuda_stream);
+    int (*fold_segments)(void* values, uint64_t n, const uint64_t* offsets, uint32_t n_segments, void* dst, void* cuda_stream);
 } fbr_body_module_t;
 typedef const fbr_body_module_t* (*fbr_body_entry_fn)(void);
 int fbr_register_body(const char* name, const char* module_path, const char* entry, int* func_id);
@@ -259,6 +271,22 @@ int fbr_pool_worker_device(fbr_pool_t* pool, int worker, int* device_id);
                                    Blocks after the first are wrapped once every block is done (from fbr_result_wait,
                                    fbr_result_poll or fbr_result_fetch), so fbr_result_poll reports 0 tasks done until
                                    the whole map is, and a worker that dies under it fails it */
+#define FBR_FOLD_KEYS 0x10000u  /* fold per key (FBR_BODY_KEYED bodies): fbr_result_t.data holds n_keys records, then n_keys
+                                   uint64 counts (tasks per key).  Record k is defined on the results whose key() is k, in
+                                   task order (x_k): each block's total for k is tree() of its own x_k, and record k is
+                                   tree() over those totals in block order, counting only blocks where k has a task (so one
+                                   worker gives tree(x_k)); identity() for a key without tasks.  The block cut is the fold
+                                   plan's (FBR_PLAN_FOLD); nothing else -- chunksize, unit size, ring_bytes, waves,
+                                   FBR_SHUFFLE, FBR_VIA_RING, re-dispatched units -- changes a bit.  With n_keys = 1 it is
+                                   FBR_FOLD's record.  desc.n_keys must be 1 .. 65536 with n_keys * result_bytes <= ring_bytes,
+                                   and a block holds fewer than 2^32 tasks.  Refused with FBR_FOLD, FBR_SCAN, out,
+                                   FBR_OUT_DEVICE, FBR_WANT_SUM or FBR_NO_ZERO_COPY; FBR_RESULTS_ON_DEVICE changes nothing.
+                                   A task whose key() is >= n_keys fails the map with FBR_TASK_KEY.  Each block is a
+                                   full-window map; after its last round it sorts its tasks by key on the device (a stable
+                                   LSD radix sort), gathers its records into key order and folds each key's run, and only
+                                   its n_keys totals and counts cross PCIe.  fbr_result_poll reports 0 tasks done until the
+                                   whole map is, fbr_result_fetch refuses the map, and a worker that dies under it fails it */
+#define FBR_MAX_KEYS 65536u
 
 typedef struct fbr_map_desc {
     int32_t func_id;
@@ -281,7 +309,7 @@ typedef struct fbr_map_desc {
     uint32_t attempt;        /* how many times this block of tasks has been dispatched before (a resilient pool that
                                 re-queues a dead worker's chunk, fiber/pool.py:1635-1654, passes attempt + 1); bodies
                                 see it as their `attempt` argument */
-    uint32_t pad;
+    uint32_t n_keys;         /* FBR_FOLD_KEYS: number of keys (1 .. FBR_MAX_KEYS); ignored without it */
 } fbr_map_desc_t;
 
 int fbr_map_submit(fbr_pool_t* pool, const fbr_map_desc_t* desc, uint64_t* seq);
@@ -346,6 +374,10 @@ int fbr_fold_values(fbr_pool_t* pool, int func_id, const void* values, uint64_t 
  * ranges of block totals t_0 .. t_{b-1} given by the set bits of b (largest first, fbr_fold_values), this turns block b's
  * own prefix folds into the FBR_SCAN records of a map cut into blocks elsewhere (process-isolated pools). */
 int fbr_scan_values(fbr_pool_t* pool, int func_id, const void* pieces, uint32_t n_pieces, void* values, uint64_t n);
+/* tree() (see FBR_FOLD) of each segment [offsets[k], offsets[k + 1]) of the host records at `values` (result_bytes each) of
+ * FBR_BODY_KEYED body func_id into out[k] (host), identity() for an empty segment, on the pool's first live worker; blocks
+ * until done.  offsets are n_segments + 1 non-decreasing host words from 0.  A keyed map's blocks are combined this way. */
+int fbr_fold_segments(fbr_pool_t* pool, int func_id, const void* values, const uint64_t* offsets, uint32_t n_segments, void* out);
 
 /* ---- result collection ----------------------------------------------------------------------
  * fbr_result_wait    <- MapResult.get -> Inventory.get (fiber/pool.py:736-737, 666-679)
@@ -372,7 +404,8 @@ typedef enum fbr_task_error {
     FBR_TASK_OVERFLOW = 1,   /* int64 result overflow (Python ints are unbounded: fail loudly) */
     FBR_TASK_BADARG = 2,
     FBR_TASK_FAULT = 3,      /* injected fault (resilient-pool tests) */
-    FBR_TASK_EMIT = 4        /* an emit body's task pushed another number of values than its count pass gave */
+    FBR_TASK_EMIT = 4,       /* an emit body's task pushed another number of values than its count pass gave */
+    FBR_TASK_KEY = 5         /* FBR_FOLD_KEYS: the task's key() is not below n_keys */
 } fbr_task_error;
 
 int fbr_result_wait(fbr_pool_t* pool, uint64_t seq, int timeout_ms, fbr_result_t* res);

@@ -66,6 +66,19 @@
 // It is computed without a running carry: with F_1 .. F_k the aligned power-of-two pieces of [0, i) given by the set bits
 // of i, largest first (each a complete aligned subtree of tree()), y[i] = F_1 (+) (F_2 (+) ( ... (+) (F_k (+) x[i]))).
 //
+// A fold body may also define a key for each result (FBR_BODY_KEYED):
+//
+//     __device__ static uint32_t key(const Res& r);               // which group the result belongs to
+//
+// Pool.fold_by_key(f, xs, n_keys) then returns n_keys records and a count per key: record k folds the results whose key()
+// is k, taken in task order (the subsequence x_k).  On one worker record k is tree(x_k), so it equals
+// Pool.fold(f, [x for x in xs if key(f(x)) == k]) bit for bit; on several it is tree() over the per-block trees of x_k in
+// block order, counting only blocks where key k has a task.  A key with no task gets identity().  The key is part of the
+// result: run() computes it (the nearest centroid, a label taken from the argument), and combine() normally leaves acc's
+// key field alone, so a non-empty group's record carries its key and an empty group's record is identity().  A task whose
+// key() is not below n_keys fails the map with FBR_TASK_KEY.  FBR_EXPORT_RECORD_BODY exports the keys entry (keys_kernel)
+// and the fold_segments entry (a segmented tree()) after scan.
+//
 // A record body may also read one array every task of a map shares (the pool initializer's initargs, or the same array
 // in every task tuple): it declares the array's element type and a shared-memory budget, and run() gets the block
 // after the result:
@@ -371,6 +384,69 @@ int launch_scan(void* values, uint64_t n, int prefix, const void* pieces, uint32
     if (buf) cudaFreeAsync(buf, s);
     return (int)e;
 }
+// keyed fold bodies: key[i] = B::key(values[i]) for n device records; a key >= n_keys is stored as 0 and the lowest such
+// task, first_task + i, goes into *err as (task << 8 | FBR_TASK_KEY) by atomicMin.  Returns the launch's cudaError_t.
+template <class B>
+int launch_keys(const void* values, uint64_t n, uint32_t n_keys, uint64_t first_task, uint32_t* keys, unsigned long long* err,
+                void* sv) {
+    if (n == 0) return (int)cudaSuccess;
+    (void)cudaGetLastError();
+    fbr::keys_kernel<B><<<(unsigned)std::min<uint64_t>((n + fbr::kThreads - 1) / fbr::kThreads, 8192), fbr::kThreads, 0, (cudaStream_t)sv>>>(
+        (const uint8_t*)values, n, n_keys, first_task, keys, err);
+    return (int)cudaGetLastError();
+}
+// tree() of each of the S segments [offsets[k], offsets[k + 1]) of the n key-ordered device records at `values` (folded in
+// place) into dst[k], identity() for an empty segment.  offsets are S + 1 device words, non-decreasing, offsets[S] <= n.  Each
+// level folds kFoldTile-record tiles aligned at every segment's start, then the next level folds the tile totals, until no
+// segment has more than one record left (at most ceil(log_kFoldTile(n)) levels).  The tile numbering and the identity live in
+// stream-ordered scratch.
+template <class B>
+int launch_fold_segments(void* values, uint64_t n, const uint64_t* offsets, uint32_t S, void* dst, void* sv) {
+    constexpr uint64_t R = sizeof(typename B::Res), T = fbr::record::kFoldTile;
+    const cudaStream_t s = (cudaStream_t)sv;
+    if (S == 0) return (int)cudaSuccess;
+    (void)cudaGetLastError();
+    const uint64_t states = S / fbr::scan::kTile + 1;   // scan_counts_kernel: the tile holding index S writes the end
+    // tiles[S] | tile_offs[S + 1] | tile_state[states] | total | ticket | identity
+    const uint64_t o_offs = S, o_state = o_offs + S + 1, o_total = o_state + states, o_ticket = o_total + 1, o_id = o_ticket + 1;
+    uint64_t* buf = nullptr;
+    cudaError_t e = cudaMallocAsync((void**)&buf, o_id * 8 + R, s);
+    if (e != cudaSuccess) {
+        (void)cudaGetLastError();
+        return (int)e;
+    }
+    uint8_t* const id = (uint8_t*)(buf + o_id);
+    e = cudaMemcpyAsync(id, fold_identity<B>(), R, cudaMemcpyHostToDevice, s);
+    const unsigned seg_grid = (unsigned)std::min<uint64_t>((S + fbr::kThreads - 1) / fbr::kThreads, 1024);
+    for (uint64_t step = 1; e == cudaSuccess && step < n; step *= T) {
+        e = cudaMemsetAsync(buf + o_state, 0, (states + 2) * 8, s);
+        if (e != cudaSuccess) break;
+        fbr::seg_tiles_kernel<<<seg_grid, fbr::kThreads, 0, s>>>(offsets, S, step, buf);
+        fbr::scan_counts_kernel<<<(unsigned)states, fbr::scan::kThreads, 0, s>>>(buf, S, buf + o_offs, (unsigned long long*)(buf + o_state),
+                                                                               (uint32_t*)(buf + o_ticket), buf + o_total);
+        // at most one tile per kFoldTile records at this level, plus one partial tile per segment
+        const uint64_t grid = std::min<uint64_t>((n + step * T - 1) / (step * T) + S, 1u << 16);
+        fbr::fold_segments_kernel<B><<<(unsigned)grid, fbr::kThreads, 0, s>>>((uint8_t*)values, offsets, S, step, buf + o_offs);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) {
+        fbr::fold_segments_out_kernel<B><<<(unsigned)std::min<uint64_t>((S + 7) / 8, 8192), fbr::kThreads, 0, s>>>(
+            (const uint8_t*)values, offsets, S, (uint8_t*)dst, id);
+        e = cudaGetLastError();
+    }
+    cudaFreeAsync(buf, s);
+    return (int)e;
+}
+template <class B>
+constexpr int (*record_keys())(const void*, uint64_t, uint32_t, uint64_t, uint32_t*, unsigned long long*, void*) {
+    if constexpr (fbr::record::KeyOf<B>::kOn) return launch_keys<B>;
+    else return nullptr;
+}
+template <class B>
+constexpr int (*record_fold_segments())(void*, uint64_t, const uint64_t*, uint32_t, void*, void*) {
+    if constexpr (fbr::record::KeyOf<B>::kOn) return launch_fold_segments<B>;
+    else return nullptr;
+}
 template <class B>
 constexpr fbr_body_launch_fn record_launch() {
     if constexpr (fbr::record::EmitOf<B>::kOn) return launch_emit<B>;
@@ -407,7 +483,7 @@ template <class B>
 constexpr uint32_t record_flags() {
     return FBR_BODY_RECORD | (fbr::record::BroadcastOf<B>::kOn ? (FBR_BODY_NEEDS_SHARED | FBR_BODY_BROADCAST) : 0u) |
            (fbr::record::ItemsOf<B>::kOn ? FBR_BODY_ITEMS : 0u) | (fbr::record::EmitOf<B>::kOn ? FBR_BODY_EMIT : 0u) |
-           (fbr::record::FoldOf<B>::kOn ? (FBR_BODY_FOLD | FBR_BODY_SCAN) : 0u);
+           (fbr::record::FoldOf<B>::kOn ? (FBR_BODY_FOLD | FBR_BODY_SCAN) : 0u) | (fbr::record::KeyOf<B>::kOn ? FBR_BODY_KEYED : 0u);
 }
 // the descriptor's group_threads: kGroup of a group body, 0 for a one-thread body
 template <class B>
@@ -424,7 +500,7 @@ constexpr uint32_t record_group() {
 // its element size and staging budget; a body with kGroup gets group_threads = kGroup; a body with an Item type (or an
 // Items = fbr::ItemTypes<...> list) gets FBR_BODY_ITEMS, its item streams and their item sizes; a body with combine() gets
 // FBR_BODY_FOLD | FBR_BODY_SCAN, its fold entry (fold_tree_kernel), its identity() and its scan entry (scan_level_kernel,
-// scan_wrap_kernel).
+// scan_wrap_kernel); a fold body with key() also gets FBR_BODY_KEYED and its keys and fold_segments entries.
 #define FBR_EXPORT_RECORD_BODY(Body, body_name, entry, body_flags)                                                \
     static_assert(fbr_body_export::record_body_ok<Body>(), "record body");                                       \
     static_assert((((body_flags) & FBR_BODY_INDEX_ARG) != 0) == Body::kIndexArg,                                 \
@@ -444,7 +520,8 @@ constexpr uint32_t record_group() {
                                              fbr::record::ItemsOf<Body>::elem(3)},                               \
                                             fbr_body_export::record_fold<Body>(), fbr_body_export::fold_identity<Body>(), \
                                             fbr::record::FoldOf<Body>::kOn ? fbr::record::Layout<Body>::R : 0u,   \
-                                            fbr_body_export::record_scan<Body>()};                               \
+                                            fbr_body_export::record_scan<Body>(),                                \
+                                            fbr_body_export::record_keys<Body>(), fbr_body_export::record_fold_segments<Body>()}; \
         return &m;                                                                                               \
     }
 
