@@ -1343,11 +1343,14 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
     // ring -- unit t of a wave is tasks [wave_first + t*unit, ...) and its results belong at exactly that
     // index of the ordered window, so the dispatch kernel stores them there and no gather is launched.
     // (Shuffled arrival, several attempts per unit and FBR_VIA_RING keep the ring + gather_ordered path.)
+    static const bool env_records = getenv("FBR_RECORDS") && atoi(getenv("FBR_RECORDS")) != 0;
     {
         static const bool env_off = getenv("FBR_DIRECT") && atoi(getenv("FBR_DIRECT")) == 0;
         const bool unit_ok = ((uint64_t)unit * R) % 16 == 0 || unit == 1;   // full vectors are stored 16 B at a time
         const bool base_ok = !cx.out_dev || (((uintptr_t)d.out + part.first * R) & 15) == 0;
-        cx.direct = !env_off && !cx.resilient && !(d.flags & (FBR_SHUFFLE | FBR_VIA_RING)) && unit_ok && base_ok;
+        // explicit task records (FBR_RECORDS=1) take every wave through the ring (run_wave), so such a block is not direct:
+        // its waves must be cut to the ring's and the record window's capacity
+        cx.direct = !env_off && !env_records && !cx.resilient && !(d.flags & (FBR_SHUFFLE | FBR_VIA_RING)) && unit_ok && base_ok;
     }
     // wave capacity in claim units
     uint64_t units_cap = cx.direct ? (1ull << 31) :   // 32-bit unit counter; a direct wave needs no ring space
@@ -1454,7 +1457,6 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
         // Task records go through the pinned ring window only when they are not an arithmetic
         // progression the kernels can compute (shuffled arrival), or when FBR_RECORDS=1 asks for the
         // explicit-record path.  (The host may not overwrite a window whose previous H2D is in flight.)
-        static const bool env_records = getenv("FBR_RECORDS") && atoi(getenv("FBR_RECORDS")) != 0;
         const bool have_records = (d.flags & FBR_SHUFFLE) || env_records;
         if (have_records) {
             CK(cudaEventSynchronize(w.ev_rec_h2d[rw]));
