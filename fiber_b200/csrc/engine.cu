@@ -118,27 +118,22 @@ static void launch_payload_map(const void* wpv, int grid, void* sv) {
     cudaStream_t s = (cudaStream_t)sv;
     // contiguous records: TMA-staged, warp-specialised kernel (2 CTAs of 5 warps per SM); strided
     // records (arg_stride > 4096) keep the register-streaming kernel
-    static const bool use_tma = !(getenv("FBR_DISPATCH_TMA") && atoi(getenv("FBR_DISPATCH_TMA")) == 0);
-    if (use_tma && wp.arg_stride == kPayloadBytes) {
+    if (wp.arg_stride == kPayloadBytes) {
         int sm = 132, dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, dev);
-        static const bool deep = getenv("FBR_TMA_DEEP") && atoi(getenv("FBR_TMA_DEEP")) != 0;
-        int per_sm = deep ? 1 : 2;
+        int per_sm = 2;
         if (const char* e = getenv("FBR_DISPATCH_OCC")) per_sm = std::max(1, std::min(per_sm, atoi(e)));
         const int g = (int)std::min<uint32_t>(wp.n_units, (uint32_t)(sm * per_sm));
-        if (deep) dispatch_payload_map_tma_kernel<6, 3><<<g, 160, tma_map::smem_bytes(6, 3), s>>>(wp);
-        else dispatch_payload_map_tma_kernel<3, 2><<<g, 160, tma_map::kSmemBytes, s>>>(wp);
+        dispatch_payload_map_tma_kernel<<<g, 160, tma_map::kSmemBytes, s>>>(wp);
         return;
     }
     dispatch_payload_map_kernel<<<grid, kThreads, 0, s>>>(wp);
 }
 static int occ_payload_map(int) {
-    cudaFuncSetAttribute(dispatch_payload_map_tma_kernel<3, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tma_map::kSmemBytes);
-    cudaFuncSetAttribute(dispatch_payload_map_tma_kernel<6, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tma_map::smem_bytes(6, 3));
+    cudaFuncSetAttribute(dispatch_payload_map_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tma_map::kSmemBytes);
     cudaFuncAttributes at;
-    cudaFuncGetAttributes(&at, (const void*)dispatch_payload_map_tma_kernel<3, 2>);   // force-load
-    cudaFuncGetAttributes(&at, (const void*)dispatch_payload_map_tma_kernel<6, 3>);
+    cudaFuncGetAttributes(&at, (const void*)dispatch_payload_map_tma_kernel);   // force-load
     return occupancy_of((const void*)dispatch_payload_map_kernel, kThreads, 0);
 }
 static void launch_payload_checksum(const void* wpv, int grid, void* sv) {
@@ -986,18 +981,12 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
                                                                           (uint64_t)w.sm_count * w.occ_gather));
         // kernel choice for this wave (see kernels.cuh): TMA bulk pipeline, row streaming, or flat
         const bool aligned = !cx.fold && (((uintptr_t)gp.out & 15) == 0) && (((uint64_t)cx.unit * cx.R) == cx.slot_stride);
-        const bool rows_ok = aligned && (cx.slot_stride % 4096 == 0) && getenv("FBR_GATHER_FLAT") == nullptr;
-        const bool bulk_ok = rows_ok && !cx.resilient &&
-                             (cx.slot_stride % bulk::kChunk == 0 || getenv("FBR_BULK_SMALL") != nullptr) &&   // 4 KB slots: the rows kernel
-                             (cx.slot_stride <= bulk::kChunk || cx.slot_stride % bulk::kChunk == 0) &&
-                             !(getenv("FBR_GATHER_BULK") && atoi(getenv("FBR_GATHER_BULK")) == 0);
+        const bool rows_ok = aligned && (cx.slot_stride % 4096 == 0);
+        const bool bulk_ok = rows_ok && !cx.resilient && cx.slot_stride % bulk::kChunk == 0;   // 4-12 KB slots: the rows kernel
         uint32_t* gticket = w.d_tickets + kTickets + (wno % kTickets);   // zero at launch, re-armed below
         if (bulk_ok) {
-            const uint32_t stage = std::min<uint32_t>(cx.slot_stride, bulk::kChunk);
-            const size_t smem_bytes = (size_t)bulk::kStages * stage;
-            // big chunks: ONE warp per SM keeps enough bulk copies in flight to saturate HBM;
-            // 4 KB chunks need more CTAs to keep enough bytes in flight
-            int per_sm = stage >= bulk::kChunk ? 1 : (int)std::min<size_t>(8, (200u << 10) / smem_bytes);
+            // ONE warp per SM keeps enough bulk copies in flight to saturate HBM
+            int per_sm = 1;
             if (const char* e = getenv("FBR_GATHER_OCC")) per_sm = std::max(1, atoi(e));
             // ~256 KB of ring per ticket (<= 32 slots: one header per lane), >= ~8 tickets per CTA
             const uint64_t max_ctas = (uint64_t)w.sm_count * per_sm;
@@ -1006,7 +995,7 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
             if (const char* e = getenv("FBR_BULK_GROUP")) group_slots = std::max(1, std::min(32, atoi(e)));
             const uint32_t n_groups = (n_units + group_slots - 1) / group_slots;
             const int grid_b = (int)std::min<uint64_t>(n_groups, max_ctas);
-            gather_bulk_kernel<<<grid_b, 32, smem_bytes, s_g>>>(gp, gticket, stage, group_slots);
+            gather_bulk_kernel<<<grid_b, 32, (size_t)bulk::kStages * bulk::kChunk, s_g>>>(gp, gticket, group_slots);
             CK(cudaMemsetAsync(gticket, 0, sizeof(uint32_t), s_g));
         } else if (rows_ok) {
             // ~128 KB of ring per ticket, but never fewer than ~4 tickets per resident CTA (small waves);
@@ -1019,11 +1008,8 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
             const int grid_r = (int)std::min<uint64_t>(n_groups, max_ctas);
             // newest slots first (see the kernel): the ring's most recently written part is still in the L2.  On the H100
             // (50 MB L2) this costs nothing for waves that fit the L2 and gains for larger ones -- 8-9 % at 95 MB, 4 % at
-            // 190 MB per wave (profiles/r03_gather_order.txt) -- so it is the default at every size.  FBR_GATHER_REVERSE=0
-            // selects oldest-first.
-            bool reverse = true;
-            if (const char* e = getenv("FBR_GATHER_REVERSE")) reverse = atoi(e) != 0;
-            gather_rows_kernel<<<grid_r, kThreads, 0, s_g>>>(gp, gticket, group_slots, reverse);
+            // 190 MB per wave (profiles/r03_gather_order.txt) -- so it is the order at every size.
+            gather_rows_kernel<<<grid_r, kThreads, 0, s_g>>>(gp, gticket, group_slots);
             CK(cudaMemsetAsync(gticket, 0, sizeof(uint32_t), s_g));
         } else {
             gather_ordered_kernel<<<grid_g, kThreads, 0, s_g>>>(gp);
@@ -1212,10 +1198,9 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
     {
         // Bit-packed bool results are small (1/8 B per task): instead of staging them in HBM and copying them out wave
         // by wave (6 x (2 MB D2H + copy set-up) = the critical path of the e2e step), the dispatch kernel can store them
-        // straight into the pinned host segment (zero copy): the PCIe writes spread over the whole kernel (FBR_ZERO_COPY=0
-        // selects the staged path).
-        static const int zc = getenv("FBR_ZERO_COPY") ? atoi(getenv("FBR_ZERO_COPY")) : 1;
-        cx.zero_copy = zc != 0 && body.result_kind == FBR_RES_BITS8 && !cx.out_dev && !cx.resilient && !cx.keep_on_device &&
+        // straight into the pinned host segment (zero copy): the PCIe writes spread over the whole kernel
+        // (FBR_NO_ZERO_COPY selects the staged path).
+        cx.zero_copy = body.result_kind == FBR_RES_BITS8 && !cx.out_dev && !cx.resilient && !cx.keep_on_device &&
                        !(d.flags & (FBR_FULL_WINDOW | FBR_SHUFFLE | FBR_VIA_RING | FBR_NO_ZERO_COPY)) && st.out != nullptr;
     }
     cx.full_window = (cx.out_dev && !cx.peer_out) || cx.resilient || cx.keep_on_device || (d.flags & FBR_FULL_WINDOW) || cx.zero_copy ||
@@ -1343,14 +1328,10 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
     // ring -- unit t of a wave is tasks [wave_first + t*unit, ...) and its results belong at exactly that
     // index of the ordered window, so the dispatch kernel stores them there and no gather is launched.
     // (Shuffled arrival, several attempts per unit and FBR_VIA_RING keep the ring + gather_ordered path.)
-    static const bool env_records = getenv("FBR_RECORDS") && atoi(getenv("FBR_RECORDS")) != 0;
     {
-        static const bool env_off = getenv("FBR_DIRECT") && atoi(getenv("FBR_DIRECT")) == 0;
         const bool unit_ok = ((uint64_t)unit * R) % 16 == 0 || unit == 1;   // full vectors are stored 16 B at a time
         const bool base_ok = !cx.out_dev || (((uintptr_t)d.out + part.first * R) & 15) == 0;
-        // explicit task records (FBR_RECORDS=1) take every wave through the ring (run_wave), so such a block is not direct:
-        // its waves must be cut to the ring's and the record window's capacity
-        cx.direct = !env_off && !env_records && !cx.resilient && !(d.flags & (FBR_SHUFFLE | FBR_VIA_RING)) && unit_ok && base_ok;
+        cx.direct = !cx.resilient && !(d.flags & (FBR_SHUFFLE | FBR_VIA_RING)) && unit_ok && base_ok;
     }
     // wave capacity in claim units
     uint64_t units_cap = cx.direct ? (1ull << 31) :   // 32-bit unit counter; a direct wave needs no ring space
@@ -1455,9 +1436,9 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
         const uint64_t wave_first = part.first + done_tasks;  // map index of the wave's first task
 
         // Task records go through the pinned ring window only when they are not an arithmetic
-        // progression the kernels can compute (shuffled arrival), or when FBR_RECORDS=1 asks for the
-        // explicit-record path.  (The host may not overwrite a window whose previous H2D is in flight.)
-        const bool have_records = (d.flags & FBR_SHUFFLE) || env_records;
+        // progression the kernels can compute (shuffled arrival).  (The host may not overwrite a window
+        // whose previous H2D is in flight.)
+        const bool have_records = (d.flags & FBR_SHUFFLE) != 0;
         if (have_records) {
             CK(cudaEventSynchronize(w.ev_rec_h2d[rw]));
             TaskRecord* hrec = w.h_records + (size_t)rw * kRecCapacity;
@@ -1724,7 +1705,7 @@ int fbr_internal_preload(int device) {
     cudaFuncGetAttributes(&at, (const void*)gather_ordered_kernel);
     cudaFuncGetAttributes(&at, (const void*)gather_rows_kernel);
     cudaFuncGetAttributes(&at, (const void*)gather_bulk_kernel);
-    cudaFuncGetAttributes(&at, (const void*)dispatch_payload_map_tma_kernel<3, 2>);
+    cudaFuncGetAttributes(&at, (const void*)dispatch_payload_map_tma_kernel);
     cudaFuncGetAttributes(&at, (const void*)payload_fill_kernel);
     cudaGetLastError();
     return FBR_OK;
@@ -2552,8 +2533,7 @@ static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_ite
             st->own_out = true;
         }
         int failed_worker = -1, rc = FBR_OK;
-        static const bool serial = getenv("FBR_SERIAL_SUBMIT") && atoi(getenv("FBR_SERIAL_SUBMIT")) != 0;
-        if (st->parts.size() > 1 && !serial) {
+        if (st->parts.size() > 1) {
             // one submit thread per worker (see SubmitThread); this thread holds the pool lock meanwhile
             if (p->submitters.size() < p->workers.size()) p->submitters.resize(p->workers.size());
             SeqState* stp = st.get();

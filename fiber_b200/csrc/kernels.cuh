@@ -563,8 +563,8 @@ __global__ void __launch_bounds__(kThreads) dispatch_parzen_kernel(const WavePar
 // holds one slot per claim unit in task-record (arrival) order; each slot's header says which
 // tasks it carries.  Three kernels, picked per wave by the host:
 //
-//   gather_bulk_kernel     TMA path (cp.async.bulk, UBLKCP in SASS) for slots of >= 4 KB whose units
-//                          are all valid: one elected thread per CTA pipelines
+//   gather_bulk_kernel     TMA path (cp.async.bulk, UBLKCP in SASS) for slots of whole 16 KB chunks
+//                          whose units are all valid: one elected thread per CTA pipelines
 //                          ring --bulk load--> shared stage --bulk store--> output; no payload byte
 //                          touches a register.  ONE CTA of one warp per SM keeps enough bulk
 //                          copies in flight for big slots.
@@ -668,7 +668,7 @@ __global__ void __launch_bounds__(kThreads) gather_ordered_kernel(const GatherPa
 
 // ---- rows: a CTA claims ~128 KB of ring by ticket and streams it as 4 KB rows ---------------------
 // Thread j owns the j-th 16 B column of every row, 4 rows in flight.
-__global__ void __launch_bounds__(kThreads) gather_rows_kernel(const GatherParams gp, uint32_t* ticket, uint32_t group_slots, bool reverse) {
+__global__ void __launch_bounds__(kThreads) gather_rows_kernel(const GatherParams gp, uint32_t* ticket, uint32_t group_slots) {
     __shared__ uint32_t s_ticket;
     TicketClaimer tc{ticket, 0u};
     tc.prime();
@@ -692,7 +692,7 @@ __global__ void __launch_bounds__(kThreads) gather_rows_kernel(const GatherParam
         if (gt >= n_groups) break;
         // newest slots first: the dispatch kernel filled the ring in ticket order just before this
         // launch, so its tail is still in the L2 (50 MB on the H100) while its head has been written back
-        const uint32_t g = reverse ? n_groups - 1 - gt : gt;
+        const uint32_t g = n_groups - 1 - gt;
         const uint32_t slot0 = g * group_slots;
         const uint32_t nslots = min(group_slots, gp.n_units - slot0);
         const uint32_t nrows = nslots * rps;
@@ -720,7 +720,7 @@ __global__ void __launch_bounds__(kThreads) gather_rows_kernel(const GatherParam
 
 // ---- bulk: TMA pipeline -------------------------------------------------------------------------------
 namespace bulk {
-constexpr uint32_t kChunk = 16384;     // bytes per bulk copy (a slot smaller than this is one chunk)
+constexpr uint32_t kChunk = 16384;     // bytes per bulk copy and per shared stage
 constexpr int kStages = 6;             // 96 KB of shared memory per CTA
 constexpr int kLag = 4;                // loads run this many chunks ahead of their store
 constexpr uint32_t kGroup = 32;        // slots per ticket: their headers are prefetched by the 32 lanes
@@ -757,10 +757,9 @@ __device__ __forceinline__ void bulk_wait_read() {
 }
 }  // namespace bulk
 
-// Requirements checked by the host: slot_stride % 16 == 0 and >= 4 KB, slot_stride <= kChunk or a
-// multiple of kChunk, R % 16 == 0 or every unit full, output window 16 B aligned, no lost units.
-__global__ void __launch_bounds__(32) gather_bulk_kernel(const GatherParams gp, uint32_t* ticket, uint32_t stage_stride,
-                                                         uint32_t group_slots /* <= kGroup */) {
+// Requirements checked by the host: slot_stride a multiple of kChunk, R % 16 == 0 or every unit full,
+// output window 16 B aligned, no lost units.
+__global__ void __launch_bounds__(32) gather_bulk_kernel(const GatherParams gp, uint32_t* ticket, uint32_t group_slots /* <= kGroup */) {
     using namespace bulk;
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ uint64_t full[kStages];
@@ -773,7 +772,6 @@ __global__ void __launch_bounds__(32) gather_bulk_kernel(const GatherParams gp, 
     }
     __syncwarp();
 
-    const uint32_t chunk = gp.slot_stride < kChunk ? gp.slot_stride : kChunk;
     const uint32_t n_groups = (gp.n_units + group_slots - 1) / group_slots;
     uint32_t it = 0, st = 0;                             // chunks loaded / stored so far (lane 0)
     uint8_t* pend_dst[kStages] = {};
@@ -782,7 +780,7 @@ __global__ void __launch_bounds__(32) gather_bulk_kernel(const GatherParams gp, 
     auto store_one = [&]() {
         const int sg = st % kStages;
         mbar_wait(&full[sg], (st / kStages) & 1);
-        bulk_store(pend_dst[sg], smem + (size_t)sg * stage_stride, pend_bytes[sg]);
+        bulk_store(pend_dst[sg], smem + (size_t)sg * kChunk, pend_bytes[sg]);
         ++st;
     };
 
@@ -804,8 +802,8 @@ __global__ void __launch_bounds__(32) gather_bulk_kernel(const GatherParams gp, 
                 // a tail unit whose byte count is not a multiple of 16: the last <16 bytes go by hand
                 const uint32_t valid16 = valid & ~15u;
                 for (uint32_t b = valid16; b < valid; ++b) dst[b] = src[b];
-                for (uint32_t off = 0; off < valid16; off += chunk) {
-                    const uint32_t bytes = min(chunk, valid16 - off);
+                for (uint32_t off = 0; off < valid16; off += kChunk) {
+                    const uint32_t bytes = min(kChunk, valid16 - off);
                     const int sg = it % kStages;
                     // the stage was last used by chunk it-kStages, whose store was issued at least
                     // kStages-kLag-1 groups ago: wait until it has finished reading shared memory
@@ -813,7 +811,7 @@ __global__ void __launch_bounds__(32) gather_bulk_kernel(const GatherParams gp, 
                     pend_dst[sg] = dst + off;
                     pend_bytes[sg] = bytes;
                     mbar_expect_tx(&full[sg], bytes);
-                    bulk_load(smem + (size_t)sg * stage_stride, src + off, bytes, &full[sg]);
+                    bulk_load(smem + (size_t)sg * kChunk, src + off, bytes, &full[sg]);
                     ++it;
                     while (it - st > (uint32_t)kLag) store_one();
                 }
@@ -843,14 +841,11 @@ namespace tma_map {
 constexpr uint32_t kMapChunk = 16384;
 constexpr int kConsumers = 128;
 struct ChunkDesc { uint8_t* dst; uint32_t bytes; uint32_t tbase; };
-constexpr size_t smem_bytes(int in_stages, int out_stages) { return (size_t)(in_stages + out_stages) * kMapChunk; }
-constexpr size_t kSmemBytes = smem_bytes(3, 2);      // the default instantiation: 80 KB, two CTAs per SM
+// 3 IN and 2 OUT stages at 2 CTAs per SM: 96 KB of loads in flight per SM from local HBM
+constexpr int kInStages = 3, kOutStages = 2;
+constexpr size_t kSmemBytes = (size_t)(kInStages + kOutStages) * kMapChunk;   // 80 KB
 }  // namespace tma_map
 
-// <3 IN, 2 OUT> stages, 2 CTAs/SM: local HBM (96 KB of loads in flight per SM).  <6, 3>, 1 CTA/SM: the same bytes
-// in flight from ONE producer per SM -- for records that live in a peer GPU's memory (NVLink round trips are ~4x
-// longer and the link prefers fewer, deeper request streams).
-template <int kInStages, int kOutStages>
 __global__ void __launch_bounds__(160) dispatch_payload_map_tma_kernel(const WaveParams wp) {
     using namespace bulk;
     using namespace tma_map;

@@ -2,7 +2,7 @@
 
 The engine picks a gather kernel per wave (engine.cu, the ``aligned`` / ``rows_ok`` / ``bulk_ok`` lines of run_wave) and the
 payload body picks its dispatch kernel per launch (``launch_payload_map``), from the claim unit, the slot stride, the
-output pointer, the map flags and the environment knobs.  ``expected_kernel`` and ``expected_dispatch`` restate those rules;
+output pointer and the map flags.  ``expected_kernel`` and ``expected_dispatch`` restate those rules;
 ``CASES`` lists the maps, each with the cell (kernel and the edge of its index arithmetic) it is meant to reach; ``CELLS``
 says what each cell is and which task counts it must be run at.  tests/test_kernel_choice_cpu.py checks through
 ``fbr_plan_query`` that every case lands in its cell and that every cell is covered, so a change to the selection rule or to
@@ -96,39 +96,34 @@ def case_plan(c):
     return plan_of(c.body, c.n, c.chunksize, c.ring, c.env)
 
 
-def expected_kernel(plan, R, flags, out_ptr, env):
+def expected_kernel(plan, R, flags, out_ptr):
     """The kernel that places a wave's results (engine.cu run_wave): "direct" (the dispatch kernel stores at the final
     index, no gather), or the gather kernel "bulk", "rows" or "flat".  out_ptr: the caller's device output (FBR_OUT_DEVICE)
-    or 0; env: the knobs of the process (FBR_DIRECT is read once per process)."""
+    or 0."""
     unit, slot = plan.unit_tasks, plan.slot_stride
     resilient = bool(flags & _abi.FBR_RESILIENT)
     out_dev = bool(flags & _abi.FBR_OUT_DEVICE)
-    direct_off = env.get("FBR_DIRECT") is not None and int(env["FBR_DIRECT"]) == 0
     unit_ok = (unit * R) % 16 == 0 or unit == 1
     base_ok = not out_dev or out_ptr % 16 == 0
-    if not direct_off and not resilient and not flags & (_abi.FBR_SHUFFLE | _abi.FBR_VIA_RING) and unit_ok and base_ok:
+    if not resilient and not flags & (_abi.FBR_SHUFFLE | _abi.FBR_VIA_RING) and unit_ok and base_ok:
         return "direct"
     # the gather writes into the caller's device output (FBR_OUT_DEVICE) or into a buffer of the engine (16 B aligned)
     aligned = (out_ptr if out_dev else 0) % 16 == 0 and unit * R == slot
-    rows_ok = aligned and slot % 4096 == 0 and "FBR_GATHER_FLAT" not in env
-    bulk_ok = (rows_ok and not resilient and (slot % CHUNK == 0 or "FBR_BULK_SMALL" in env) and (slot <= CHUNK or slot % CHUNK == 0)
-               and not ("FBR_GATHER_BULK" in env and int(env["FBR_GATHER_BULK"]) == 0))
+    rows_ok = aligned and slot % 4096 == 0
+    bulk_ok = rows_ok and not resilient and slot % CHUNK == 0
     return "bulk" if bulk_ok else "rows" if rows_ok else "flat"
 
 
-def expected_dispatch(body, arg_stride, env):
-    """The dispatch kernel of a payload body (engine.cu launch_payload_map / launch_payload_checksum): "tma" (the
-    warp-specialised <3,2> kernel), "tma_deep" (<6,3>), "regs" (dispatch_payload_map_kernel) or "checksum"."""
+def expected_dispatch(body, arg_stride):
+    """The dispatch kernel of a payload body (engine.cu launch_payload_map / launch_payload_checksum): "tma"
+    (dispatch_payload_map_tma_kernel), "regs" (dispatch_payload_map_kernel) or "checksum"."""
     if body == "payload_checksum_4k":
         return "checksum"
-    tma = not ("FBR_DISPATCH_TMA" in env and int(env["FBR_DISPATCH_TMA"]) == 0)
-    if tma and arg_stride == 4096:
-        return "tma_deep" if "FBR_TMA_DEEP" in env and int(env["FBR_TMA_DEEP"]) != 0 else "tma"
-    return "regs"
+    return "tma" if arg_stride == 4096 else "regs"
 
 
-def kernel_of(c, env=None):
-    return expected_kernel(case_plan(c), c.result_bytes, c.flags, c.out_offset, dict(env or {}, **c.env))
+def kernel_of(c):
+    return expected_kernel(case_plan(c), c.result_bytes, c.flags, c.out_offset)
 
 
 def kinds_of(c, plan):
@@ -162,7 +157,6 @@ def _group_cell(g):
 CELLS = {
     "flat/stride_not_4k": (lambda c, p, k: k == "flat" and p.slot_stride % 4096 != 0, ALL_KINDS),
     "flat/vps_npot": (lambda c, p, k: k == "flat" and not _pow2(p.slot_stride // 16), ALL_KINDS),
-    "flat/forced": (lambda c, p, k: k == "flat" and "FBR_GATHER_FLAT" in c.env and p.slot_stride % 4096 == 0, ALL_KINDS),
     "flat/out_plus4": (lambda c, p, k: k == "flat" and c.place == "out4", ALL_KINDS),
     "rows/rps1": (lambda c, p, k: k == "rows" and p.slot_stride == 4096, ALL_KINDS),
     "rows/rps_npot": (lambda c, p, k: k == "rows" and not _pow2(p.slot_stride >> 12), ALL_KINDS),
@@ -173,29 +167,24 @@ CELLS = {
     "rows/grouped_npot": (lambda c, p, k: k == "rows" and not _pow2(p.slot_stride >> 12) and c.env.get("FBR_GATHER_OCC") == "1"
                           and c.env.get("FBR_WAVES") == "1" and min((128 << 10) // p.slot_stride, p.n_units // (4 * SM_COUNT)) >= 2,
                           frozenset(("minus_one", "exact", "plus_one"))),
-    "rows/forward": (lambda c, p, k: k == "rows" and c.env.get("FBR_GATHER_REVERSE") == "0", ALL_KINDS),
-    "rows/reverse": (lambda c, p, k: k == "rows" and c.env.get("FBR_GATHER_REVERSE", "1") != "0", ALL_KINDS),
     "bulk/16k": (lambda c, p, k: k == "bulk" and p.slot_stride == CHUNK, ALL_KINDS),
     "bulk/multi_chunk": (lambda c, p, k: k == "bulk" and p.slot_stride > CHUNK, ALL_KINDS),
     # a tail unit of count * R bytes, not a multiple of 16: no stable unit of a bulk slot has R % 16 != 0 at n = 1, and
     # a map of whole units has no tail
     "bulk/tail_bytes": (lambda c, p, k: k == "bulk" and (c.n % p.unit_tasks) * c.result_bytes % 16 != 0,
                         frozenset(("minus_one", "plus_one", "waves"))),
-    "bulk/small_4k": (lambda c, p, k: k == "bulk" and p.slot_stride == 4096 and "FBR_BULK_SMALL" in c.env, ALL_KINDS),
-    "bulk/small_8k": (lambda c, p, k: k == "bulk" and p.slot_stride == 8192 and "FBR_BULK_SMALL" in c.env, ALL_KINDS),
-    "bulk/small_12k": (lambda c, p, k: k == "bulk" and p.slot_stride == 12288 and "FBR_BULK_SMALL" in c.env, ALL_KINDS),
     "bulk/group_1": _group_cell(1),
     "bulk/group_3": _group_cell(3),
     "bulk/group_32": _group_cell(32),
     "bulk/occ1": (lambda c, p, k: k == "bulk" and c.env.get("FBR_GATHER_OCC") == "1", ALL_KINDS),
-    "payload/tma": (lambda c, p, k: c.body == "payload_map_4k" and expected_dispatch(c.body, c.arg_stride, c.env) == "tma", ALL_KINDS),
+    "payload/tma": (lambda c, p, k: c.body == "payload_map_4k" and expected_dispatch(c.body, c.arg_stride) == "tma", ALL_KINDS),
     "payload/strided_map": (lambda c, p, k: c.body == "payload_map_4k" and c.arg_stride in (4112, 8192, 12288)
-                            and expected_dispatch(c.body, c.arg_stride, c.env) == "regs", ALL_KINDS),
+                            and expected_dispatch(c.body, c.arg_stride) == "regs", ALL_KINDS),
     "payload/strided_checksum": (lambda c, p, k: c.body == "payload_checksum_4k" and c.arg_stride in (4112, 8192, 12288)
                                  and c.want_sum, ALL_KINDS),
     "grid/occ1_record": (lambda c, p, k: c.env.get("FBR_DISPATCH_OCC") == "1" and c.body in LB.BY_NAME, ALL_KINDS),
     "grid/occ1_payload_tma": (lambda c, p, k: c.env.get("FBR_DISPATCH_OCC") == "1"
-                              and expected_dispatch(c.body, c.arg_stride, c.env) == "tma", ALL_KINDS),
+                              and expected_dispatch(c.body, c.arg_stride) == "tma", ALL_KINDS),
     # pi_inside_bits8 runs through Pool.map (8 indices per byte-task), so its kinds are not named by unit; its results
     # go straight into the pinned output (zero copy), which makes every such map one wave
     "grid/occ1_pi_bits": (lambda c, p, k: c.env.get("FBR_DISPATCH_OCC") == "1" and c.body == "pi_inside_bits8",
@@ -240,7 +229,6 @@ def _build():
     C += _cases("flat/stride_not_4k", "payload_checksum_4k", place="shuffle")     # 256 x 4 B = 1 KB slots
     C += _cases("flat/vps_npot", "lay_a2052_r2052", place="shuffle")              # 1026 vectors per slot
     C += _cases("flat/vps_npot", "payload_checksum_4k", chunksize=3)              # 252 tasks: 63 vectors
-    C += _cases("flat/forced", "payload_map_4k", env={"FBR_GATHER_FLAT": "1"})
     C += _cases("flat/out_plus4", "payload_map_4k", place="out4")
     C += _cases("flat/out_plus4", "payload_checksum_4k", place="out4", ns=[5, 1000])
     # ---- rows: gather_rows_kernel
@@ -248,21 +236,23 @@ def _build():
     C += _cases("rows/rps1", "bc_e4_s0", env=u256)                                # 256 x 16 B: one row per slot
     big = 200 * 4096
     C += _cases("rows/rps1", "pi_inside_det", args="range", ns=[big - 1, big, big + 1])
+    C += _cases("rows/rps1", "pi_inside_det", args="range", place="shuffle", ns=[big + 1])
     C += _cases("rows/rps_npot", "payload_map_4k", chunksize=3, ring=32 << 10)    # 3 tasks: 3 rows
+    C += _cases("rows/rps_npot", "payload_map_4k", chunksize=3, ring=32 << 10, place="shuffle")
     C += _cases("rows/rps_npot", "lay_a8_r24", place="shuffle", ns=[200 * 1024 - 1, 200 * 1024 + 1], wave_ring=0)   # 6 rows
+    C += _cases("rows/rps_npot", "lay_i8_r12", args="range", ns=[200 * 1024 + 1, 200 * 1024 + 5, 200 * 1024 - 1],
+                wave_ring=0)                                                      # 12 KB slots, 12-byte records
+    C += _cases("rows/rps_npot", "payload_map_4k", chunksize=9, place="shuffle")  # 27 tasks: 27 rows of 108 KB slots
+    C += _cases("rows/rps_npot", "payload_map_4k", chunksize=9)
     C += _cases("rows/big_slot", "payload_map_4k", chunksize=3, place="shuffle")  # 30 tasks: 30 rows of 120 KB slots
     C += _cases("rows/big_slot", "payload_map_4k", chunksize=17)                  # 17 rows
-    C += _cases("rows/big_slot", "payload_map_4k", env={"FBR_GATHER_BULK": "0"}, ns=[33], wave_ring=0)   # 128 KB, TMA off
+    C += _cases("rows/big_slot", "lay_a12_r4096", place="resilient")              # 32 KB slots
     C += _cases("rows/resilient_lost", "flt_a4_r4096", place="resilient")         # 32 KB slots, ~5 % of the tasks lost twice
-    C += _cases("rows/forward", "payload_map_4k", chunksize=3, ring=32 << 10, env={"FBR_GATHER_REVERSE": "0"})
     grouped = {"FBR_GATHER_OCC": "1", "FBR_WAVES": "1"}
-    C += _cases("rows/grouped_npot", "lay_a8_r24", env=grouped, ns=[1600 * 1024 - 1, 1600 * 1024], wave_ring=0)   # 24 KB slots
+    C += _cases("rows/grouped_npot", "lay_a8_r24", env=grouped, ns=[1600 * 1024 - 1, 1600 * 1024, 1600 * 1024 + 1],
+                wave_ring=0)                                                      # 24 KB slots
     C += _cases("rows/grouped_npot", "pi_inside_det", args="range", env=dict(grouped, FBR_UNIT_TASKS="12288"),
                 ns=[2200 * 12288 + 1], wave_ring=0)                                                       # 12 KB slots
-    C += _cases("rows/forward", "lay_a8_r24", env=dict(grouped, FBR_GATHER_REVERSE="0"), ns=[1600 * 1024 + 1], wave_ring=0)
-    C += _cases("rows/forward", "payload_map_4k", chunksize=9, env={"FBR_GATHER_REVERSE": "0"}, place="shuffle")
-    C += _cases("rows/reverse", "payload_map_4k", chunksize=9, env={"FBR_GATHER_REVERSE": "1"})
-    C += _cases("rows/reverse", "lay_a12_r4096", place="resilient")
     # ---- bulk: gather_bulk_kernel
     C += _cases("bulk/16k", "payload_map_4k", ring=32 << 10)                      # 4 tasks of 4 KB
     C += _cases("bulk/16k", "lay_a4_r4096", ring=32 << 10, place="shuffle")
@@ -271,13 +261,6 @@ def _build():
     u16k = {"FBR_UNIT_TASKS": "16384"}
     pi_u = 140 * 16384
     C += _cases("bulk/tail_bytes", "pi_inside_det", args="range", env=u16k, ns=[pi_u - 1, pi_u + 1, pi_u + 9])
-    small = {"FBR_BULK_SMALL": "1"}
-    C += _cases("bulk/tail_bytes", "lay_i8_r12", args="range", env=small, ns=[200 * 1024 + 1, 200 * 1024 + 5, 200 * 1024 - 1],
-                wave_ring=0)                                                      # 12 KB slots, 12-byte records
-    C += _cases("bulk/small_4k", "bc_e4_s0", env=dict(u256, **small))
-    C += _cases("bulk/small_4k", "pi_inside_det", args="range", env=small, place="shuffle", ns=[big + 1])
-    C += _cases("bulk/small_8k", "payload_map_4k", ring=16 << 10, env=small)
-    C += _cases("bulk/small_12k", "payload_map_4k", chunksize=3, ring=32 << 10, env=small, place="shuffle")
     many = [1, 7, 8, 9, 8 * 96 + 1, 8 * 100 + 3, 8 * 101 + 2]                  # 1 .. 102 units of 8 tasks
     for g in (1, 3, 32):
         C += _cases("bulk/group_%d" % g, "lay_a4_r4096", env={"FBR_BULK_GROUP": str(g)}, ns=[n for n in many if g == 1 or -(-n // 8) % g])
@@ -435,8 +418,11 @@ def _delta(a, b):
 
 def check_stats(c, kernel, waves, st):
     """Messages for stats that contradict the path a case was meant to take: direct placement or a gather launch per
-    wave, and at least one dispatch launch per wave."""
+    wave, at least one dispatch launch per wave, and no task records copied for a map that is neither shuffled nor
+    resilient."""
     bad = []
+    if c.place not in ("shuffle", "resilient") and st["records_copied"] != 0:
+        bad.append("records_copied %d on a map that is not shuffled" % st["records_copied"])
     if waves is not None and st["dispatch_launches"] < waves:
         bad.append("dispatch_launches %d < %d waves" % (st["dispatch_launches"], waves))
     if kernel == "direct" and not (st["direct_waves"] >= 1 and st["gather_launches"] == 0):

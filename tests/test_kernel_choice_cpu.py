@@ -34,7 +34,7 @@ def test_every_cell_is_run_at_every_task_count():
 def test_cells_cover_every_kernel_and_dispatch_path():
     kernels = {K.kernel_of(c) for c in K.CASES}
     assert kernels == {"direct", "flat", "rows", "bulk"}
-    dispatch = {K.expected_dispatch(c.body, c.arg_stride, c.env) for c in K.CASES if c.body in K.PAYLOAD}
+    dispatch = {K.expected_dispatch(c.body, c.arg_stride) for c in K.CASES if c.body in K.PAYLOAD}
     assert dispatch == {"tma", "regs", "checksum"}
     strided = {(c.arg_stride, c.args, c.place) for c in K.CASES if c.cell == "payload/strided_map"}
     for stride in (4112, 8192, 12288):
@@ -55,21 +55,16 @@ def test_rule_restatement_edges():
         p.unit_tasks, p.slot_stride = unit, slot
         return p
     ring, res = _abi.FBR_VIA_RING, _abi.FBR_RESILIENT
-    assert K.expected_kernel(plan(32, 32 * 4096), 4096, 0, 0, {}) == "direct"
-    assert K.expected_kernel(plan(32, 32 * 4096), 4096, 0, 0, {"FBR_DIRECT": "0"}) == "bulk"
-    assert K.expected_kernel(plan(32, 32 * 4096), 4096, ring, 0, {}) == "bulk"
-    assert K.expected_kernel(plan(32, 32 * 4096), 4096, res, 0, {}) == "rows"
-    assert K.expected_kernel(plan(32, 32 * 4096), 4096, ring, 0, {"FBR_GATHER_BULK": "0"}) == "rows"
-    assert K.expected_kernel(plan(32, 32 * 4096), 4096, ring, 0, {"FBR_GATHER_FLAT": "0"}) == "flat"   # set at all
-    assert K.expected_kernel(plan(32, 32 * 4096), 4096, _abi.FBR_OUT_DEVICE, 4, {}) == "flat"
-    assert K.expected_kernel(plan(32, 32 * 4096), 4096, _abi.FBR_OUT_DEVICE, 16, {}) == "direct"
-    assert K.expected_kernel(plan(1, 4096), 4096, ring, 0, {}) == "rows"
-    assert K.expected_kernel(plan(1, 4096), 4096, ring, 0, {"FBR_BULK_SMALL": "1"}) == "bulk"
-    assert K.expected_kernel(plan(5, 20480), 4096, ring, 0, {"FBR_BULK_SMALL": "1"}) == "rows"   # > 16 KB, no multiple
-    assert K.expected_kernel(plan(3, 16), 4, ring, 0, {}) == "flat"                                # slot rounded up to 16 B
-    assert K.expected_kernel(plan(3, 16), 4, 0, 0, {}) == "flat"                                   # 12 B units: no direct
-    assert K.expected_kernel(plan(1, 16), 4, 0, 0, {}) == "direct"
-    assert K.expected_dispatch("payload_map_4k", 4096, {}) == "tma"
-    assert K.expected_dispatch("payload_map_4k", 4096, {"FBR_TMA_DEEP": "1"}) == "tma_deep"
-    assert K.expected_dispatch("payload_map_4k", 4096, {"FBR_DISPATCH_TMA": "0"}) == "regs"
-    assert K.expected_dispatch("payload_map_4k", 4112, {}) == "regs"
+    assert K.expected_kernel(plan(32, 32 * 4096), 4096, 0, 0) == "direct"
+    assert K.expected_kernel(plan(32, 32 * 4096), 4096, ring, 0) == "bulk"
+    assert K.expected_kernel(plan(32, 32 * 4096), 4096, res, 0) == "rows"
+    assert K.expected_kernel(plan(32, 32 * 4096), 4096, _abi.FBR_OUT_DEVICE, 4) == "flat"
+    assert K.expected_kernel(plan(32, 32 * 4096), 4096, _abi.FBR_OUT_DEVICE, 16) == "direct"
+    assert K.expected_kernel(plan(1, 4096), 4096, ring, 0) == "rows"
+    assert K.expected_kernel(plan(1, 16384), 16384, ring, 0) == "bulk"            # the smallest slot of the bulk kernel
+    assert K.expected_kernel(plan(5, 20480), 4096, ring, 0) == "rows"             # > 16 KB, no multiple
+    assert K.expected_kernel(plan(3, 16), 4, ring, 0) == "flat"                   # slot rounded up to 16 B
+    assert K.expected_kernel(plan(3, 16), 4, 0, 0) == "flat"                      # 12 B units: no direct
+    assert K.expected_kernel(plan(1, 16), 4, 0, 0) == "direct"
+    assert K.expected_dispatch("payload_map_4k", 4096) == "tma"
+    assert K.expected_dispatch("payload_map_4k", 4112) == "regs"
