@@ -284,36 +284,69 @@ static int worker_occ(Worker& w, int func_id, const BodyEntry& body, bool index_
 
 struct TimedPair { cudaEvent_t a, b; };
 
-struct PartCtx {                          // constants of one worker's block of one map
+// Where a block's results go (BlockPlan::sink):
+//   Staged        the worker's out-staging halves, copied to the host segment wave by wave
+//   StagedPeer    the out-staging halves, pushed wave by wave by this worker's copy engine to the ordered output on worker 0
+//                 (another GPU): kernels storing over NVLink stay below what a copy engine pushes (FBR_PEER_OUT=0: CallerDevice)
+//   CallerDevice  the caller's device output (FBR_OUT_DEVICE), stored in place
+//   ZeroCopy      the pinned host segment, stored into over PCIe by the dispatch kernel itself (bit-packed bools)
+//   WindowToHost  an engine window, copied to the host in one piece once no unit is lost (resilient, FBR_FULL_WINDOW)
+//   WindowOnDevice  an engine window that stays on the device (FBR_RESULTS_ON_DEVICE)
+//   ScanWindow    an engine window, rewritten into the block's prefix folds after its last round (FBR_SCAN)
+//   KeyedWindow   an engine window, sorted by key and folded per key after its last round (FBR_FOLD_KEYS)
+//   FoldPartials  each unit's tree, in d_fold: no result leaves the device (FBR_FOLD)
+enum class Sink : uint8_t { Staged, StagedPeer, CallerDevice, ZeroCopy, WindowToHost, WindowOnDevice, ScanWindow, KeyedWindow, FoldPartials };
+// Where a block's argument records come from: none (range() indices), the caller's device memory read in place
+// (FBR_ARGS_DEVICE), a device copy of the block's records made once (Resident: a resilient unit may be re-dispatched at any
+// time), the host wave by wave through the d_args staging halves, or device memory of worker 0 pushed wave by wave into the
+// staging halves by worker 0's copy engine (FBR_PEER_PUSH=0: the kernel loads them itself, DeviceInPlace).
+enum class ArgSource : uint8_t { None, DeviceInPlace, Resident, Staged, Pushed };
+// Where an items body's items and offsets come from: the caller's device memory read in place, the host wave by wave
+// through the d_items staging halves, or a device copy of the block's item span and offsets made once (resilient).
+enum class ItemSource : uint8_t { None, DeviceInPlace, Staged, Resident };
+
+// The placement of one worker's block of one map: decided once by plan_block, before anything is allocated, then acted on.
+struct BlockPlan {
     uint32_t unit = 0, slot_stride = 0, R = 0, sum_kind = 0;
-    bool args_dev = false, out_dev = false, full_window = false, host_args = false, resilient = false, keep_on_device = false;
-    bool overlap = false;                 // gather(w) on s_gath concurrently with dispatch(w+1); ring used in halves
-    bool zero_copy = false;               // small host-resident results: the dispatch kernel stores them straight into the pinned
-                                          // result segment over PCIe (no staging, no D2H copy, one wave)
-    bool peer_out = false;                // the ordered output lives on worker 0 (another GPU): results are computed into the local
-                                          // out-staging halves and PUSHED there by this worker's copy engine (the D2H machinery)
-    bool peer_push = false;               // arguments live on worker 0 (another GPU): worker 0's copy engine PUSHES each wave's
-                                          // records into this worker's staging halves over NVLink (host_args machinery)
-    bool host_items = false;              // items bodies, host-resident items, not resilient: each wave copies each stream's
-                                          // offsets slice and item span into the worker's d_items staging half
+    Sink sink = Sink::Staged;
+    ArgSource args = ArgSource::None;
+    ItemSource items = ItemSource::None;
+    bool resilient = false;
     bool direct = false;                  // contiguous, unshuffled, non-resilient block: the dispatch kernel stores every
                                           // unit at its final index (no ring, no task records, no gather launch)
-    bool fold = false;                    // FBR_FOLD: each unit writes its tree to d_fold, no result leaves the device
+    bool overlap = false;                 // gather(w) on s_gath concurrently with dispatch(w+1); ring used in halves
+    uint64_t wave_tasks_cap = 0;          // tasks per regular wave (0: the ring holds no claim unit)
+    uint64_t redispatch_units_cap = 0;    // claim units per re-dispatch wave
+    uint64_t args_limit_bytes = 0;        // host arguments end here (n_items records); 0 = n_tasks * arg_stride
+    // results pass through the out-staging halves; else they go to one window of the whole block (or d_fold)
+    bool staged() const { return sink == Sink::Staged || sink == Sink::StagedPeer; }
+    // the engine allocates the block's window on the device
+    bool engine_window() const { return !staged() && sink != Sink::CallerDevice && sink != Sink::ZeroCopy && sink != Sink::FoldPartials; }
+    // nothing of the block is final before its last round is: its results reach the host in one copy at the end, are
+    // stored over PCIe by the kernel, or are rewritten (scan, keyed, fold) behind its last wave
+    bool final_at_block_end() const { return !staged() && sink != Sink::CallerDevice && sink != Sink::WindowOnDevice; }
+    // each wave copies its argument records in (from the host, or pushed by worker 0)
+    bool args_streamed() const { return args == ArgSource::Staged || args == ArgSource::Pushed; }
+    // the bytes of the argument records of tasks [first, first + n): a bit-packed map's last task may cover fewer items
+    uint64_t arg_bytes(uint64_t first, uint64_t n, uint32_t stride) const {
+        const uint64_t start = first * stride, bytes = n * stride;
+        return !args_limit_bytes ? bytes : start >= args_limit_bytes ? 0 : std::min(bytes, args_limit_bytes - start);
+    }
+};
+
+// The runtime state of a block's placement: the pointers its plan asked for, once they are allocated.
+struct PartCtx {
+    BlockPlan plan;
     uint8_t* fold_total = nullptr;        // FBR_FOLD: the block's total, in the map's pinned segment
-    bool scan = false;                    // FBR_SCAN: the block's window becomes its prefix folds after its last round
-    bool keyed = false;                   // FBR_FOLD_KEYS: the block's window is sorted by key and folded per key after its last
-    uint8_t* key_totals = nullptr;        // round into n_keys totals and counts, in the map's pinned segment
+    uint8_t* key_totals = nullptr;        // FBR_FOLD_KEYS: the block's n_keys totals and counts, in the map's pinned segment
     uint8_t* key_counts = nullptr;
     const uint8_t* d_shared = nullptr;
-    uint8_t* window_base = nullptr;       // device output of a FULL_WINDOW part
-    const uint8_t* args_full = nullptr;   // device-resident arguments of the whole map (args_dev / resilient)
-    uint64_t wave_tasks_cap = 0;
-    uint64_t args_limit_bytes = 0;        // host arguments end here (n_items records); 0 = n_tasks * arg_stride
-    // items bodies: where the kernel finds the part's items and offsets of each stream for the whole map (WaveParams::items
-    // ..., more_items)
-    const uint8_t* items[kMaxItemStreams] = {};
-    const uint64_t* item_offs[kMaxItemStreams] = {};
-    uint64_t item_first = 0, item_base[kMaxItemStreams] = {}, item_count[kMaxItemStreams] = {};
+    uint8_t* window_base = nullptr;       // the block's window (BlockPlan::windowed)
+    const uint8_t* args_full = nullptr;   // device-resident arguments of the whole map (DeviceInPlace / Resident)
+    // items bodies: where the kernel finds the items and offsets of each stream for the whole map (WaveParams::items ...,
+    // more_items), and the map index of the task offsets[0] belongs to
+    ItemStream items[kMaxItemStreams] = {};
+    uint64_t item_first = 0;
 };
 
 // A worker block of an emit map's emit pass: the part-local exclusive offsets its scan produced (count + 1 of them, the last
@@ -715,6 +748,99 @@ static uint32_t map_chunksize(const fbr_map_desc_t& d) {
     return d.chunksize ? d.chunksize : 32u;
 }
 
+// The placement of tasks [first, first + count) of map `d` on worker `worker` (BlockPlan).  Pure: no CUDA call, no
+// allocation.  host_out: the map has a pinned host result segment; root_alive: worker 0 is alive (it can push arguments);
+// item_bytes_per_task: the mean bytes a task's host-resident items and offsets take of a staging half, over every stream.
+static BlockPlan plan_block(const BodyEntry& body, const fbr_map_desc_t& d, uint32_t pool_flags, int worker, uint64_t first,
+                            uint64_t count, bool host_out, int sm_count, uint64_t ring_bytes, bool root_alive,
+                            uint64_t item_bytes_per_task) {
+    BlockPlan pl;
+    pl.R = body.result_bytes;
+    pl.resilient = (d.flags & FBR_RESILIENT) != 0;
+    pl.unit = pick_unit(body, map_chunksize(d), count, sm_count, ring_bytes);
+    pl.slot_stride = (uint32_t)round_up((uint64_t)pl.unit * pl.R, 16);
+    const uint32_t unit = pl.unit, R = pl.R;
+
+    static const bool out_off = getenv("FBR_PEER_OUT") && atoi(getenv("FBR_PEER_OUT")) == 0;
+    // Bit-packed bool results are small (1/8 B per task): instead of staging them in HBM and copying them out wave by wave
+    // (6 x (2 MB D2H + copy set-up) = the critical path of the e2e step), the dispatch kernel stores them straight into the
+    // pinned host segment (ZeroCopy): the PCIe writes spread over the whole kernel (FBR_NO_ZERO_COPY selects Staged).
+    const bool zero_copy_ok = body.result_kind == FBR_RES_BITS8 && host_out && !pl.resilient &&
+                              !(d.flags & (FBR_FULL_WINDOW | FBR_SHUFFLE | FBR_VIA_RING | FBR_NO_ZERO_COPY));
+    if (d.flags & FBR_FOLD) pl.sink = Sink::FoldPartials;
+    else if (d.flags & FBR_FOLD_KEYS) pl.sink = Sink::KeyedWindow;
+    else if (d.flags & FBR_SCAN) pl.sink = Sink::ScanWindow;
+    else if (d.flags & FBR_OUT_DEVICE)
+        pl.sink = worker != 0 && !pl.resilient && !out_off && !(d.flags & FBR_FULL_WINDOW) ? Sink::StagedPeer : Sink::CallerDevice;
+    else if (d.flags & FBR_RESULTS_ON_DEVICE) pl.sink = Sink::WindowOnDevice;
+    else if (zero_copy_ok) pl.sink = Sink::ZeroCopy;
+    else if (pl.resilient || (d.flags & FBR_FULL_WINDOW)) pl.sink = Sink::WindowToHost;
+    else pl.sink = Sink::Staged;
+
+    static const bool push_off = getenv("FBR_PEER_PUSH") && atoi(getenv("FBR_PEER_PUSH")) == 0;
+    if (d.flags & FBR_ARGS_DEVICE)
+        pl.args = d.arg_stride != 0 && worker != 0 && !pl.resilient && !push_off && root_alive ? ArgSource::Pushed : ArgSource::DeviceInPlace;
+    else if (d.arg_stride == 0) pl.args = ArgSource::None;
+    else pl.args = pl.resilient ? ArgSource::Resident : ArgSource::Staged;
+    if (d.n_items && d.arg_stride && body.result_kind == FBR_RES_BITS8)
+        pl.args_limit_bytes = d.n_items * (uint64_t)(d.arg_stride / 8);   // a byte-task's record is 8 items
+    if (body.flags & FBR_BODY_ITEMS)
+        pl.items = (d.flags & FBR_ARGS_DEVICE) ? ItemSource::DeviceInPlace : pl.resilient ? ItemSource::Resident : ItemSource::Staged;
+
+    // Opt-in (FBR_POOL_OVERLAP): gather(w) runs on a second, higher-priority stream while the next wave's / next map's
+    // dispatch kernel computes; the ring is then used in alternating halves.  On the pi map (ALU-bound dispatch + HBM-bound
+    // gather) the gather is a small share of the step and the two kernels contend for SM slots, so it is off by default.
+    pl.overlap = !pl.staged() && !pl.resilient && (pool_flags & FBR_POOL_OVERLAP) != 0;
+    // Direct placement: a contiguous, unshuffled, non-resilient block needs neither task records nor the ring -- unit t of
+    // a wave is tasks [wave_first + t*unit, ...) and its results belong at exactly that index of the ordered window, so the
+    // dispatch kernel stores them there and no gather is launched.  (Shuffled arrival, several attempts per unit and
+    // FBR_VIA_RING keep the ring + gather path.)
+    {
+        const bool unit_ok = ((uint64_t)unit * R) % 16 == 0 || unit == 1;   // full vectors are stored 16 B at a time
+        const bool base_ok = !(d.flags & FBR_OUT_DEVICE) || (((uintptr_t)d.out + first * R) & 15) == 0;
+        pl.direct = !pl.resilient && !(d.flags & (FBR_SHUFFLE | FBR_VIA_RING)) && unit_ok && base_ok;
+    }
+    // wave capacity in claim units
+    uint64_t units_cap = pl.direct ? (1ull << 31) :   // 32-bit unit counter; a direct wave needs no ring space
+        std::min<uint64_t>(kRecCapacity, (pl.overlap ? ring_bytes / 2 : ring_bytes) / pl.slot_stride);
+    if (pl.args_streamed()) units_cap = std::min<uint64_t>(units_cap, ring_bytes / ((uint64_t)unit * d.arg_stride));
+    if (pl.staged()) units_cap = std::min<uint64_t>(units_cap, ring_bytes / ((uint64_t)unit * R));
+    pl.wave_tasks_cap = units_cap * unit;
+    // Host-resident output: cut large maps into ~8 waves (>= 8 MiB of results each) so the D2H of
+    // wave w overlaps the kernels of wave w+1 instead of trailing one monolithic launch.
+    if (pl.staged() || pl.args_streamed() || pl.items == ItemSource::Staged) {
+        uint64_t bytes_per_task = std::max<uint64_t>(R, pl.args_streamed() ? d.arg_stride : 0);
+        if (pl.items == ItemSource::Staged) bytes_per_task = std::max(bytes_per_task, item_bytes_per_task);
+        // a wave must carry enough kernel time to hide its launches: 8 MiB of byte results is tens of us of
+        // pi dispatch; a byte of bit-packed results stands for 8 tasks, so 1 MiB is the same work
+        uint64_t min_wave_bytes = body.result_kind == FBR_RES_BITS8 ? (1ull << 20) : (8ull << 20);
+        if (const char* e = getenv("FBR_MIN_WAVE_KB")) min_wave_bytes = std::max<uint64_t>(4096, (uint64_t)atoll(e) << 10);   // tuning knob
+        const uint64_t min_wave_tasks = round_up(std::max<uint64_t>(1, min_wave_bytes / bytes_per_task), unit);
+        // 8 waves for ~100 MB maps, up to 64 for multi-GB ones (~64 MiB per wave): the first wave's
+        // H2D and the last wave's D2H are the only copies nothing overlaps with
+        uint64_t n_waves = std::min<uint64_t>(64, std::max<uint64_t>(8, count * bytes_per_task / (64ull << 20)));
+        // small outputs (bit-packed bools): per-copy set-up weighs more: T_kernel/n + n * T_setup is flattest at a few waves
+        if (body.result_kind == FBR_RES_BITS8 && !pl.args_streamed()) n_waves = 6;
+        if (const char* e = getenv("FBR_WAVES")) n_waves = std::max<uint64_t>(1, (uint64_t)atoll(e));                          // tuning knob
+        const uint64_t share = round_up((count + n_waves - 1) / n_waves, unit);
+        pl.wave_tasks_cap = std::min(pl.wave_tasks_cap, std::max(min_wave_tasks, share));
+    }
+    pl.redispatch_units_cap = std::max<uint64_t>(1, std::min<uint64_t>(kRecCapacity, ring_bytes / pl.slot_stride));
+    pl.sum_kind = (d.flags & FBR_WANT_SUM) ? 1 : 0;   // the dispatch kernel folds sum(results) while they are in registers
+    return pl;
+}
+
+// Worker i's block [b0, b1) of `count` tasks cut over n_workers: contiguous, in order, whole claim units of the map-level
+// unit (every block gets the same number of units, the last ones may get fewer or none).
+static void cut_block(const BodyEntry& body, uint32_t chunksize, uint64_t count, int n_workers, int i, int sm_count,
+                      uint64_t ring_bytes, uint64_t* b0, uint64_t* b1) {
+    const uint32_t unit = pick_unit(body, chunksize, (count + n_workers - 1) / n_workers, sm_count, ring_bytes);
+    const uint64_t units_total = (count + unit - 1) / unit;
+    const uint64_t units_per = (units_total + n_workers - 1) / n_workers;
+    *b0 = std::min<uint64_t>(count, (uint64_t)i * units_per * unit);
+    *b1 = std::min<uint64_t>(count, (uint64_t)(i + 1) * units_per * unit);
+}
+
 static void shuffle_records(TaskRecord* r, uint32_t n, uint64_t seed) {
     for (uint32_t i = n; i > 1; --i) {
         seed = splitmix64(seed);
@@ -765,6 +891,71 @@ static StagedStream staged_items(const SeqState& st, const SeqPart& part) {
     return s;
 }
 
+// The most whole units (or the rest of the block) from task `done` on, at most `wt` tasks, whose wave fits one staging half
+// in every stream; at least one unit (submit_part checked that each fits).  Binary search over the host offsets.
+static uint64_t fit_staged_wave(const std::vector<StagedStream>& streams, uint64_t done, uint64_t wt, uint32_t unit,
+                                uint64_t ring_bytes) {
+    auto fits = [&](uint64_t tasks) {
+        for (const StagedStream& s : streams)
+            if (s.staged_bytes(done, done + tasks) > ring_bytes) return false;
+        return true;
+    };
+    uint64_t lo_u = 0, hi_u = (wt + unit - 1) / unit;               // fits(lo_u units) holds (0 tasks always fit)
+    while (lo_u < hi_u) {
+        const uint64_t mid = (lo_u + hi_u + 1) / 2;
+        if (fits(std::min<uint64_t>(mid * unit, wt))) lo_u = mid; else hi_u = mid - 1;
+    }
+    return std::min<uint64_t>(std::max<uint64_t>(lo_u, 1) * unit, wt);
+}
+
+// Grid of a wave's dispatch kernel: `occ` resident CTAs per SM of the body's kernel, at most the body's max_ctas_per_sm,
+// one fewer for an overlapped wave (its gather CTAs run beside it), FBR_DISPATCH_OCC at most, no more CTAs than units.
+static int dispatch_grid(const BodyEntry& body, int occ, bool overlapped, uint32_t n_units, int sm_count) {
+    if (body.max_ctas_per_sm) occ = std::min(occ, body.max_ctas_per_sm);
+    if (overlapped && occ > 1) occ -= 1;     // leave SM slots for the concurrently running gather CTAs
+    if (const char* e = getenv("FBR_DISPATCH_OCC")) occ = std::max(1, std::min(occ, atoi(e)));
+    return (int)std::min<uint64_t>(n_units, (uint64_t)sm_count * occ);
+}
+
+// How a wave's results reach their final place (kernels.cuh): the dispatch kernel stores them there itself (Direct), or a
+// gather kernel moves them from the ring -- the TMA bulk pipeline (Bulk), row streaming (Rows) or the flat vector loop
+// (Flat) -- on `grid` CTAs, Bulk and Rows in ticket groups of `group_slots` slots.
+struct GatherChoice { enum Kind { Direct, Flat, Rows, Bulk } kind; int grid; uint32_t group_slots; };
+
+// listed: the wave's units are task records (shuffled, re-dispatched), not its contiguous range; out: its ordered window.
+static GatherChoice pick_gather(const BlockPlan& pl, const void* out, uint32_t n_units, bool listed, int sm_count, int occ_gather,
+                                int occ_gather_rows) {
+    if (pl.direct && !listed) return {GatherChoice::Direct, 0, 0};
+    const bool aligned = pl.sink != Sink::FoldPartials && (((uintptr_t)out & 15) == 0) && (((uint64_t)pl.unit * pl.R) == pl.slot_stride);
+    const bool rows_ok = aligned && (pl.slot_stride % 4096 == 0);
+    const bool bulk_ok = rows_ok && !pl.resilient && pl.slot_stride % bulk::kChunk == 0;   // 4-12 KB slots: the rows kernel
+    if (bulk_ok) {
+        // ONE warp per SM keeps enough bulk copies in flight to saturate HBM
+        int per_sm = 1;
+        if (const char* e = getenv("FBR_GATHER_OCC")) per_sm = std::max(1, atoi(e));
+        // ~256 KB of ring per ticket (<= 32 slots: one header per lane), >= ~8 tickets per CTA
+        const uint64_t max_ctas = (uint64_t)sm_count * per_sm;
+        uint32_t group_slots = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(
+            std::min<uint64_t>(bulk::kGroup, (256u << 10) / pl.slot_stride), n_units / (8 * max_ctas)));
+        if (const char* e = getenv("FBR_BULK_GROUP")) group_slots = std::max(1, std::min(32, atoi(e)));
+        const uint32_t n_groups = (n_units + group_slots - 1) / group_slots;
+        return {GatherChoice::Bulk, (int)std::min<uint64_t>(n_groups, max_ctas), group_slots};
+    }
+    if (rows_ok) {
+        // ~128 KB of ring per ticket, but never fewer than ~4 tickets per resident CTA (small waves);
+        // big slots (>= 32 KB): at most 4 fat streams per SM
+        int occ_g = pl.slot_stride >= (32u << 10) ? std::min(occ_gather_rows, 4) : occ_gather_rows;
+        if (const char* e = getenv("FBR_GATHER_OCC")) occ_g = std::max(1, std::min(occ_g, atoi(e)));
+        const uint64_t max_ctas = (uint64_t)sm_count * occ_g;
+        const uint32_t group_slots = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((128u << 10) / pl.slot_stride, n_units / (4 * max_ctas)));
+        const uint32_t n_groups = (n_units + group_slots - 1) / group_slots;
+        return {GatherChoice::Rows, (int)std::min<uint64_t>(n_groups, max_ctas), group_slots};
+    }
+    const uint64_t total_vec = (uint64_t)n_units * (pl.slot_stride >> 4);
+    return {GatherChoice::Flat, (int)std::max<uint64_t>(1, std::min<uint64_t>((total_vec + kThreads * 4 - 1) / (kThreads * 4),
+                                                                              (uint64_t)sm_count * occ_gather)), 0};
+}
+
 // One wave: `n_units` claim units -> copy-in, dispatch, gather, (streaming parts) copy-out.
 // `wave_first`/`wt` describe the contiguous task window of a regular wave; a re-dispatch wave
 // (arbitrary lost units) passes contiguous=false.  `have_records`: the caller wrote the wave's task
@@ -774,12 +965,18 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
                     uint64_t wave_first, uint64_t wt, bool contiguous, bool have_records, uint64_t wno) {
     Worker& w = p->workers[part.worker];
     const PartCtx& cx = part.cx;
+    const BlockPlan& pl = cx.plan;
     const fbr_map_desc_t& d = st.desc;
     const bool timing = (p->flags & FBR_POOL_TIMING) != 0;
     const int rw = (int)(wno % kRecWindows);
     const int half = (int)(wno & 1);
     const int slot = part.ctrl_slot;
-    const bool direct = cx.direct && contiguous && !have_records;
+    // the ordered output of this wave's window, and the map index of out_window[0]
+    uint8_t* const out_window = pl.staged() ? w.d_out[half] : cx.window_base;
+    const uint64_t out_first = pl.staged() ? wave_first : part.first;
+    const GatherChoice gather = pick_gather(pl, out_window, n_units, !contiguous || have_records, w.sm_count, w.occ_gather,
+                                            w.occ_gather_rows);
+    const bool direct = gather.kind == GatherChoice::Direct;
     TaskRecord* hrec = w.h_records + (size_t)rw * kRecCapacity;
     TaskRecord* drec = w.d_records + (size_t)rw * kRecCapacity;
 
@@ -787,7 +984,7 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
     // nothing in (computed records, range() or device-resident arguments) skips the hop through s_in -- every
     // cross-stream event costs the GPU a few microseconds per wave -- except the first wave of a block, which
     // has to see the control block (and shared block) its submit_part put on s_in.
-    const bool in_copies = have_records || cx.host_args || cx.host_items || part.first_wave_pending;
+    const bool in_copies = have_records || pl.args_streamed() || pl.items == ItemSource::Staged || part.first_wave_pending;
     part.first_wave_pending = false;
     if (in_copies) {
         CK(cudaStreamWaitEvent(w.s_in, w.ev_comp[rw], 0));  // wave wno-4 kernels done (device window free)
@@ -800,14 +997,10 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
     }
     const uint8_t* wave_args = cx.args_full;
     bool pushed = false;
-    if (cx.host_args) {   // streaming arguments (contiguous waves only): from the host, or pushed by the root GPU
-        uint64_t bytes = wt * d.arg_stride;
-        if (cx.args_limit_bytes) {   // the last task of the map may cover fewer argument items than a full record
-            const uint64_t start = wave_first * (uint64_t)d.arg_stride;
-            bytes = start >= cx.args_limit_bytes ? 0 : std::min(bytes, cx.args_limit_bytes - start);
-        }
+    if (pl.args_streamed()) {   // streaming arguments (contiguous waves only): from the host, or pushed by the root GPU
+        const uint64_t bytes = pl.arg_bytes(wave_first, wt, d.arg_stride);
         const uint8_t* src = (const uint8_t*)d.args + wave_first * (uint64_t)d.arg_stride;
-        if (cx.peer_push) {
+        if (pl.args == ArgSource::Pushed) {
             // The copy runs on a stream of the ROOT device, so the root's copy engine WRITES the wave into this
             // worker's staging half (posted NVLink writes, root TX), while this worker's kernels store their results
             // into the root's output (posted writes, root RX): both directions of the root's links carry payload at
@@ -833,13 +1026,10 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
     }
     // items of a streaming wave, stream by stream in the staging half (StagedStream): its wt + 1 offsets, then its item span
     // one 256 B-rounded header further on
-    const uint8_t* wave_items[kMaxItemStreams];
-    const uint64_t* wave_offs[kMaxItemStreams];
-    uint64_t item_first = cx.item_first, item_base[kMaxItemStreams], item_count[kMaxItemStreams];
-    for (uint32_t k = 0; k < kMaxItemStreams; ++k) {
-        wave_items[k] = cx.items[k]; wave_offs[k] = cx.item_offs[k]; item_base[k] = cx.item_base[k]; item_count[k] = cx.item_count[k];
-    }
-    if (cx.host_items) {
+    ItemStream wave_items[kMaxItemStreams];
+    std::copy(cx.items, cx.items + kMaxItemStreams, wave_items);
+    uint64_t item_first = cx.item_first;
+    if (pl.items == ItemSource::Staged) {
         const StagedStream s = staged_items(st, part);
         const uint64_t t0 = wave_first - part.first, t1 = t0 + wt;
         const uint64_t obytes = (wt + 1) * sizeof(uint64_t), hbytes = s.header_bytes(t0, t1);
@@ -851,9 +1041,7 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
             if (ibytes)
                 CK(cudaMemcpyAsync(w.d_items[half] + at + hbytes, (const uint8_t*)it.items + lo * it.item_bytes, ibytes, cudaMemcpyHostToDevice, w.s_in));
             STAT_ADD(p, h2d_bytes, obytes + ibytes);
-            wave_offs[k] = (const uint64_t*)(w.d_items[half] + at);
-            wave_items[k] = w.d_items[half] + at + hbytes;
-            item_base[k] = lo; item_count[k] = hi;
+            wave_items[k] = ItemStream{w.d_items[half] + at + hbytes, (const uint64_t*)(w.d_items[half] + at), lo, hi};
         }
         item_first = wave_first;
     }
@@ -862,7 +1050,7 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
     // compute streams: dispatch on s_comp; gather on s_comp too, or -- overlapped waves -- on the
     // higher-priority s_gath so that it runs while the next wave's dispatch kernel computes.
     // Overlapped waves use alternating halves of the ring / header array.  Direct waves use neither.
-    const bool ov = cx.overlap && !direct;
+    const bool ov = pl.overlap && !direct;
     cudaStream_t s_g = ov ? w.s_gath : w.s_comp;
     uint8_t* ring_base = ov ? w.d_ring + (size_t)half * (p->ring_bytes / 2) : w.d_ring;
     SlotHeader* hdr_base = ov ? w.d_headers + (size_t)half * kRecCapacity : w.d_headers;
@@ -876,17 +1064,15 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
     }
     w.prev_wave_overlap = ov;
     w.gath_hist = ((w.gath_hist << 1) | (ov ? 1u : 0u)) & 3u;
-    if (!cx.full_window) CK(cudaStreamWaitEvent(w.s_comp, w.ev_out[half], 0));  // out half drained
-    uint8_t* const out_window = cx.full_window ? cx.window_base : w.d_out[half];      // ordered output of this wave's window
-    const uint64_t out_first = cx.full_window ? part.first : wave_first;               // map index of out_window[0]
+    if (pl.staged()) CK(cudaStreamWaitEvent(w.s_comp, w.ev_out[half], 0));  // out half drained
     WaveParams wp;
     memset(&wp, 0, sizeof wp);
     wp.records = have_records ? drec : nullptr;
     wp.headers = direct ? nullptr : hdr_base;
-    wp.ring = direct ? out_window + (wave_first - out_first) * cx.R : ring_base;
+    wp.ring = direct ? out_window + (wave_first - out_first) * pl.R : ring_base;
     wp.ticket = w.d_tickets + (wno % kTickets);
     wp.n_units = n_units;
-    wp.slot_stride = direct ? cx.unit * cx.R : cx.slot_stride;
+    wp.slot_stride = direct ? pl.unit * pl.R : pl.slot_stride;
     wp.args = wave_args;
     wp.arg_stride = d.arg_stride;
     wp.index_start = d.index_start;
@@ -895,23 +1081,23 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
     wp.shared = cx.d_shared;
     wp.shared_bytes = d.shared_bytes;
     wp.err_word = &w.d_ctrl[slot].err;
-    wp.resilient = cx.resilient ? 1u : 0u;
-    wp.sum = cx.sum_kind ? &w.d_ctrl[slot].sum : nullptr;
-    wp.sum_hi = cx.sum_kind ? &w.d_ctrl[slot].sum_hi : nullptr;
+    wp.resilient = pl.resilient ? 1u : 0u;
+    wp.sum = pl.sum_kind ? &w.d_ctrl[slot].sum : nullptr;
+    wp.sum_hi = pl.sum_kind ? &w.d_ctrl[slot].sum_hi : nullptr;
     wp.syn_first = wave_first;
     wp.syn_tasks = wt;
-    wp.syn_arg_off = cx.host_args ? 0 : wave_first * (uint64_t)d.arg_stride;
-    wp.syn_unit = cx.unit;
+    wp.syn_arg_off = pl.args_streamed() ? 0 : wave_first * (uint64_t)d.arg_stride;
+    wp.syn_unit = pl.unit;
     wp.syn_seq = (uint32_t)st.seq;
     wp.syn_func = (uint32_t)st.func_id;
     wp.syn_attempt = part.attempt;
     wp.n_items = d.n_items ? d.n_items : ~0ull;
-    wp.items = wave_items[0];
-    wp.item_offs = wave_offs[0];
+    wp.items = wave_items[0].items;
+    wp.item_offs = wave_items[0].offs;
     wp.item_first = item_first;
-    wp.item_base = item_base[0];
-    wp.item_count = item_count[0];
-    for (uint32_t k = 1; k < st.n_item_streams; ++k) wp.more_items[k - 1] = ItemStream{wave_items[k], wave_offs[k], item_base[k], item_count[k]};
+    wp.item_base = wave_items[0].base;
+    wp.item_count = wave_items[0].count;
+    for (uint32_t k = 1; k < st.n_item_streams; ++k) wp.more_items[k - 1] = wave_items[k];
     const EmitBlock& emit = part.emit;
     uint64_t v_lo = 0, v_hi = 0;            // staged emit waves: the wave's span of the block's values
     if (emit.d_offs) {
@@ -926,16 +1112,13 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
             wp.emit_values = (uint8_t*)emit.d_values;
         }
     }
-    if (cx.fold) {   // no unit stores results: each writes its tree to its place in d_fold
+    const bool fold = pl.sink == Sink::FoldPartials;
+    if (fold) {   // no unit stores results: each writes its tree to its place in d_fold
         wp.ring = nullptr;
         wp.fold_partials = (uint8_t*)part.d_fold;
         wp.fold_first = part.first;
     }
-    int occ_d = worker_occ(w, st.func_id, body, d.arg_stride == 0, cx.fold);
-    if (body.max_ctas_per_sm) occ_d = std::min(occ_d, body.max_ctas_per_sm);
-    if (ov && occ_d > 1) occ_d -= 1;     // leave SM slots for the concurrently running gather CTAs
-    if (const char* e = getenv("FBR_DISPATCH_OCC")) occ_d = std::max(1, std::min(occ_d, atoi(e)));
-    const int grid_d = (int)std::min<uint64_t>(n_units, (uint64_t)w.sm_count * occ_d);
+    const int grid_d = dispatch_grid(body, worker_occ(w, st.func_id, body, d.arg_stride == 0, fold), ov, n_units, w.sm_count);
     TimedPair td{nullptr, nullptr}, tg{nullptr, nullptr};
     if (timing) {
         CK(cudaEventCreate(&td.a)); CK(cudaEventCreate(&td.b));
@@ -949,7 +1132,7 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
     }
     STAT_ADD(p, dispatch_launches, 1);
     STAT_ADD(p, units_dispatched, n_units);
-    STAT_ADD(p, dispatch_bytes, wt * ((uint64_t)(d.arg_stride ? body.arg_bytes : 0) + cx.R));
+    STAT_ADD(p, dispatch_bytes, wt * ((uint64_t)(d.arg_stride ? body.arg_bytes : 0) + pl.R));
 
     if (direct) {
         STAT_ADD(p, direct_waves, 1);
@@ -967,52 +1150,27 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
         gp.headers = hdr_base;
         gp.ring = ring_base;
         gp.n_units = n_units;
-        gp.slot_stride = cx.fold ? 0u : cx.slot_stride;   // a fold wave's gather moves no payload, it only lists lost units
-        gp.result_bytes = cx.R;
+        gp.slot_stride = fold ? 0u : pl.slot_stride;   // a fold wave's gather moves no payload, it only lists lost units
+        gp.result_bytes = pl.R;
         gp.pad = 0;
         gp.out = out_window;
         gp.win_first = out_first;
         gp.ticket_to_reset = nullptr;     // dispatch kernels re-arm their own ticket (TicketClaimer::rearm)
-        gp.lost_count = cx.resilient ? &w.d_ctrl[slot].lost_count : nullptr;
+        gp.lost_count = pl.resilient ? &w.d_ctrl[slot].lost_count : nullptr;
         gp.lost_units = part.d_lost;
         gp.lost_capacity = part.lost_cap;
-        const uint64_t total_vec = (uint64_t)n_units * (cx.slot_stride >> 4);
-        const int grid_g = (int)std::max<uint64_t>(1, std::min<uint64_t>((total_vec + kThreads * 4 - 1) / (kThreads * 4),
-                                                                          (uint64_t)w.sm_count * w.occ_gather));
-        // kernel choice for this wave (see kernels.cuh): TMA bulk pipeline, row streaming, or flat
-        const bool aligned = !cx.fold && (((uintptr_t)gp.out & 15) == 0) && (((uint64_t)cx.unit * cx.R) == cx.slot_stride);
-        const bool rows_ok = aligned && (cx.slot_stride % 4096 == 0);
-        const bool bulk_ok = rows_ok && !cx.resilient && cx.slot_stride % bulk::kChunk == 0;   // 4-12 KB slots: the rows kernel
         uint32_t* gticket = w.d_tickets + kTickets + (wno % kTickets);   // zero at launch, re-armed below
-        if (bulk_ok) {
-            // ONE warp per SM keeps enough bulk copies in flight to saturate HBM
-            int per_sm = 1;
-            if (const char* e = getenv("FBR_GATHER_OCC")) per_sm = std::max(1, atoi(e));
-            // ~256 KB of ring per ticket (<= 32 slots: one header per lane), >= ~8 tickets per CTA
-            const uint64_t max_ctas = (uint64_t)w.sm_count * per_sm;
-            uint32_t group_slots = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(
-                std::min<uint64_t>(bulk::kGroup, (256u << 10) / cx.slot_stride), n_units / (8 * max_ctas)));
-            if (const char* e = getenv("FBR_BULK_GROUP")) group_slots = std::max(1, std::min(32, atoi(e)));
-            const uint32_t n_groups = (n_units + group_slots - 1) / group_slots;
-            const int grid_b = (int)std::min<uint64_t>(n_groups, max_ctas);
-            gather_bulk_kernel<<<grid_b, 32, (size_t)bulk::kStages * bulk::kChunk, s_g>>>(gp, gticket, group_slots);
+        if (gather.kind == GatherChoice::Bulk) {
+            gather_bulk_kernel<<<gather.grid, 32, (size_t)bulk::kStages * bulk::kChunk, s_g>>>(gp, gticket, gather.group_slots);
             CK(cudaMemsetAsync(gticket, 0, sizeof(uint32_t), s_g));
-        } else if (rows_ok) {
-            // ~128 KB of ring per ticket, but never fewer than ~4 tickets per resident CTA (small waves);
-            // big slots (>= 32 KB): at most 4 fat streams per SM
-            int occ_g = cx.slot_stride >= (32u << 10) ? std::min(w.occ_gather_rows, 4) : w.occ_gather_rows;
-            if (const char* e = getenv("FBR_GATHER_OCC")) occ_g = std::max(1, std::min(occ_g, atoi(e)));
-            const uint64_t max_ctas = (uint64_t)w.sm_count * occ_g;
-            const uint32_t group_slots = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((128u << 10) / cx.slot_stride, n_units / (4 * max_ctas)));
-            const uint32_t n_groups = (n_units + group_slots - 1) / group_slots;
-            const int grid_r = (int)std::min<uint64_t>(n_groups, max_ctas);
+        } else if (gather.kind == GatherChoice::Rows) {
             // newest slots first (see the kernel): the ring's most recently written part is still in the L2.  On the H100
             // (50 MB L2) this costs nothing for waves that fit the L2 and gains for larger ones -- 8-9 % at 95 MB, 4 % at
             // 190 MB per wave (profiles/r03_gather_order.txt) -- so it is the order at every size.
-            gather_rows_kernel<<<grid_r, kThreads, 0, s_g>>>(gp, gticket, group_slots);
+            gather_rows_kernel<<<gather.grid, kThreads, 0, s_g>>>(gp, gticket, gather.group_slots);
             CK(cudaMemsetAsync(gticket, 0, sizeof(uint32_t), s_g));
         } else {
-            gather_ordered_kernel<<<grid_g, kThreads, 0, s_g>>>(gp);
+            gather_ordered_kernel<<<gather.grid, kThreads, 0, s_g>>>(gp);
         }
         CK(cudaGetLastError());
         if (timing) {
@@ -1021,21 +1179,21 @@ static int run_wave(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry& b
         }
         CK(cudaEventRecord(w.ev_comp[rw], s_g));
         STAT_ADD(p, gather_launches, 1);
-        STAT_ADD(p, gather_bytes, 2 * wt * cx.R);
+        STAT_ADD(p, gather_bytes, 2 * wt * pl.R);
     }
 
     // copy-out stream (streaming parts): D2H of the ordered window of this wave
     if (contiguous) {
         cudaEvent_t wd;
         CK(cudaEventCreateWithFlags(&wd, cudaEventDisableTiming));
-        if (!cx.full_window) {
+        if (pl.staged()) {
             CK(cudaStreamWaitEvent(w.s_out, w.ev_comp[rw], 0));
-            if (cx.peer_out) {      // this worker's copy engine writes the wave into the root's ordered output (posted NVLink writes)
-                CK(cudaMemcpyPeerAsync((uint8_t*)st.out + wave_first * cx.R, p->workers[0].device, w.d_out[half], w.device, wt * cx.R, w.s_out));
-                STAT_ADD(p, peer_push_bytes, wt * cx.R);
+            if (pl.sink == Sink::StagedPeer) {      // this worker's copy engine writes the wave into the root's ordered output (posted NVLink writes)
+                CK(cudaMemcpyPeerAsync((uint8_t*)st.out + wave_first * pl.R, p->workers[0].device, w.d_out[half], w.device, wt * pl.R, w.s_out));
+                STAT_ADD(p, peer_push_bytes, wt * pl.R);
             } else {
-                CK(cudaMemcpyAsync((uint8_t*)st.out + wave_first * cx.R, w.d_out[half], wt * cx.R, cudaMemcpyDeviceToHost, w.s_out));
-                STAT_ADD(p, d2h_bytes, wt * cx.R);
+                CK(cudaMemcpyAsync((uint8_t*)st.out + wave_first * pl.R, w.d_out[half], wt * pl.R, cudaMemcpyDeviceToHost, w.s_out));
+                STAT_ADD(p, d2h_bytes, wt * pl.R);
             }
             if (v_hi > v_lo) {   // the wave's values, exactly its span, into the pinned segment
                 const uint64_t ob = body.out_bytes;
@@ -1138,25 +1296,28 @@ static int finish_round(fbr_pool* p, SeqState& st, SeqPart& part, bool copy_wind
     // Every block finishes on s_out, behind its copy-outs, even one without any: finishing on the compute stream puts a
     // DMA hop between back-to-back kernels of pipelined maps, which costs them what a blocking map() gains.
     CK(cudaStreamWaitEvent(w.s_out, w.ev_comp[last_rw], 0));
-    if (copy_window && cx.scan && part.count) {   // the last round: the block's own prefix folds, in place in its window
-        const cudaError_t e = (cudaError_t)body_of(st.func_id)->scan(cx.window_base, part.count, 1, nullptr, 0, (void*)w.s_out);
-        if (e != cudaSuccess) return fail(FBR_ECUDA, "scan of body %s on worker %d: %s", body_of(st.func_id)->name.c_str(),
-                                          part.worker, cudaGetErrorString(e));
-    }
-    // a scan block after the first keeps its window on the device: scan_finish wraps it there, then copies it out once
-    const bool scan_later = cx.scan && part.first != 0;
-    if (copy_window && cx.full_window && !cx.out_dev && !cx.keep_on_device && !cx.zero_copy && !cx.fold && !cx.keyed && !scan_later &&
-        part.count) {
-        CK(cudaMemcpyAsync((uint8_t*)st.out + part.first * cx.R, cx.window_base, part.count * cx.R, cudaMemcpyDeviceToHost, w.s_out));
-        STAT_ADD(p, d2h_bytes, part.count * cx.R);
-    }
-    if (copy_window && cx.fold && part.count) {   // the last round: the block's total from its units' partials
-        body_of(st.func_id)->fold(part.d_fold, (part.count + cx.unit - 1) / cx.unit, cx.fold_total, (void*)w.s_out);
-        CK(cudaGetLastError());
-    }
-    if (copy_window && cx.keyed && part.count) {
-        const int rc = fold_block_by_key(p, st, part);
-        if (rc != FBR_OK) return rc;
+    const BlockPlan& pl = cx.plan;
+    if (copy_window && part.count) {   // the last round
+        bool to_host = pl.sink == Sink::WindowToHost;
+        if (pl.sink == Sink::ScanWindow) {   // the block's own prefix folds, in place in its window
+            const cudaError_t e = (cudaError_t)body_of(st.func_id)->scan(cx.window_base, part.count, 1, nullptr, 0, (void*)w.s_out);
+            if (e != cudaSuccess) return fail(FBR_ECUDA, "scan of body %s on worker %d: %s", body_of(st.func_id)->name.c_str(),
+                                              part.worker, cudaGetErrorString(e));
+            // a scan block after the first keeps its window on the device: scan_finish wraps it there, then copies it out once
+            to_host = part.first == 0 && !(st.flags & FBR_RESULTS_ON_DEVICE);
+        }
+        if (to_host) {
+            CK(cudaMemcpyAsync((uint8_t*)st.out + part.first * pl.R, cx.window_base, part.count * pl.R, cudaMemcpyDeviceToHost, w.s_out));
+            STAT_ADD(p, d2h_bytes, part.count * pl.R);
+        }
+        if (pl.sink == Sink::FoldPartials) {   // the block's total from its units' partials
+            body_of(st.func_id)->fold(part.d_fold, (part.count + pl.unit - 1) / pl.unit, cx.fold_total, (void*)w.s_out);
+            CK(cudaGetLastError());
+        }
+        if (pl.sink == Sink::KeyedWindow) {
+            const int rc = fold_block_by_key(p, st, part);
+            if (rc != FBR_OK) return rc;
+        }
     }
     const EmitBlock& e = part.emit;
     if (copy_window && e.host && e.d_values && e.total) {
@@ -1165,7 +1326,7 @@ static int finish_round(fbr_pool* p, SeqState& st, SeqPart& part, bool copy_wind
         STAT_ADD(p, d2h_bytes, vbytes);
     }
     CK(cudaMemcpyAsync(&w.h_ctrl[slot], &w.d_ctrl[slot], sizeof(SeqCtrl), cudaMemcpyDeviceToHost, w.s_out));
-    if (cx.resilient && part.lost_cap)
+    if (pl.resilient && part.lost_cap)
         CK(cudaMemcpyAsync(part.h_lost, part.d_lost, sizeof(LostUnit) * part.lost_cap, cudaMemcpyDeviceToHost, w.s_out));
     // one event per part for its whole life, re-recorded every round: another waiter may hold the handle
     // (fbr_result_wait blocks on it outside the pool lock), so it must never be destroyed under it
@@ -1179,57 +1340,25 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
     const fbr_map_desc_t& d = st.desc;
     PartCtx& cx = part.cx;
     CK(cudaSetDevice(w.device));
-    cx.R = body.result_bytes;
-    cx.resilient = (d.flags & FBR_RESILIENT) != 0;
-    cx.args_dev = (d.flags & FBR_ARGS_DEVICE) != 0;
-    cx.out_dev = (d.flags & FBR_OUT_DEVICE) != 0;
-    cx.fold = (d.flags & FBR_FOLD) != 0;
-    cx.scan = (d.flags & FBR_SCAN) != 0;
-    cx.keyed = (d.flags & FBR_FOLD_KEYS) != 0;
-    cx.keep_on_device = (d.flags & FBR_RESULTS_ON_DEVICE) != 0 && !cx.fold && !cx.keyed;
-    {
-        // Output resident on worker 0, computed by another worker: kernels storing over NVLink stay below what a
-        // copy engine pushes at the peer-copy rate (TMA bulk or register stores alike).  So the block is
-        // computed into the local out-staging halves and each wave is pushed to the root by this worker's copy engine,
-        // overlapping the next wave's kernel (FBR_PEER_OUT=0: the kernel stores into the root's memory itself).
-        static const bool out_off = getenv("FBR_PEER_OUT") && atoi(getenv("FBR_PEER_OUT")) == 0;
-        cx.peer_out = cx.out_dev && part.worker != 0 && !cx.resilient && !out_off && !(d.flags & FBR_FULL_WINDOW);
+    uint64_t item_bytes_per_task = 0;   // host-resident items: the mean item bytes and offsets of a task, over every stream
+    if ((body.flags & FBR_BODY_ITEMS) && !(d.flags & FBR_ARGS_DEVICE) && part.count) {
+        const StagedStream s = staged_items(st, part);
+        item_bytes_per_task = s.data_bytes(0, part.count) / part.count + s.n * sizeof(uint64_t);
     }
-    {
-        // Bit-packed bool results are small (1/8 B per task): instead of staging them in HBM and copying them out wave
-        // by wave (6 x (2 MB D2H + copy set-up) = the critical path of the e2e step), the dispatch kernel can store them
-        // straight into the pinned host segment (zero copy): the PCIe writes spread over the whole kernel
-        // (FBR_NO_ZERO_COPY selects the staged path).
-        cx.zero_copy = body.result_kind == FBR_RES_BITS8 && !cx.out_dev && !cx.resilient && !cx.keep_on_device &&
-                       !(d.flags & (FBR_FULL_WINDOW | FBR_SHUFFLE | FBR_VIA_RING | FBR_NO_ZERO_COPY)) && st.out != nullptr;
+    cx.plan = plan_block(body, d, p->flags, part.worker, part.first, part.count, st.out != nullptr, w.sm_count, p->ring_bytes,
+                         !p->workers[0].dead, item_bytes_per_task);
+    const BlockPlan& pl = cx.plan;
+    if (pl.args == ArgSource::Pushed && w.s_push == nullptr) {
+        const int root = p->workers[0].device;
+        CK(cudaSetDevice(root));
+        cudaError_t e = cudaStreamCreateWithFlags(&w.s_push, cudaStreamNonBlocking);
+        if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&w.s_push2, cudaStreamNonBlocking);
+        for (int i = 0; i < kRecWindows && e == cudaSuccess; ++i) e = cudaEventCreateWithFlags(&w.ev_push[i], cudaEventDisableTiming);
+        cudaSetDevice(w.device);
+        if (e != cudaSuccess) return fail(FBR_ECUDA, "creating the push stream on device %d failed: %s", root, cudaGetErrorString(e));
+        w.push_root_device = root;
     }
-    cx.full_window = (cx.out_dev && !cx.peer_out) || cx.resilient || cx.keep_on_device || (d.flags & FBR_FULL_WINDOW) || cx.zero_copy ||
-                     cx.fold ||   // a fold block has no output window: nothing is staged or copied out
-                     cx.scan ||   // a scan block's results are rewritten in place once all of them are there
-                     cx.keyed;    // ... and a keyed block's are sorted by key and folded
-    cx.host_args = d.arg_stride != 0 && !cx.args_dev && !cx.resilient;
-    {
-        // device-resident arguments on worker 0, consumed by another worker: stream them through the staging halves,
-        // pushed wave by wave by the root's copy engine (FBR_PEER_PUSH=0: the kernel loads them over NVLink itself)
-        static const bool push_off = getenv("FBR_PEER_PUSH") && atoi(getenv("FBR_PEER_PUSH")) == 0;
-        if (cx.args_dev && d.arg_stride != 0 && part.worker != 0 && !cx.resilient && !push_off && !p->workers[0].dead) {
-            if (w.s_push == nullptr) {
-                const int root = p->workers[0].device;
-                CK(cudaSetDevice(root));
-                cudaError_t e = cudaStreamCreateWithFlags(&w.s_push, cudaStreamNonBlocking);
-                if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&w.s_push2, cudaStreamNonBlocking);
-                for (int i = 0; i < kRecWindows && e == cudaSuccess; ++i) e = cudaEventCreateWithFlags(&w.ev_push[i], cudaEventDisableTiming);
-                cudaSetDevice(w.device);
-                if (e != cudaSuccess) return fail(FBR_ECUDA, "creating the push stream on device %d failed: %s", root, cudaGetErrorString(e));
-                w.push_root_device = root;
-            }
-            cx.peer_push = true;
-            cx.host_args = true;       // same wave / staging machinery as host-resident arguments
-        }
-    }
-    cx.unit = pick_unit(body, map_chunksize(d), part.count, w.sm_count, p->ring_bytes);
-    cx.slot_stride = (uint32_t)round_up((uint64_t)cx.unit * cx.R, 16);
-    const uint32_t unit = cx.unit, R = cx.R;
+    const uint32_t unit = pl.unit, R = pl.R;
     if ((body.flags & FBR_BODY_RECORD) && unit > body.unit_tasks)   // a unit must fit the kernel's shared-memory stage
         return fail(FBR_EINVAL, "record body %s: a claim unit of %u tasks exceeds its stage of %u", body.name.c_str(), unit, body.unit_tasks);
 
@@ -1240,18 +1369,19 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
     part.ctrl_slot = slot;
     CK(cudaMemcpyAsync(&w.d_ctrl[slot], &w.h_ctrl[kCtrlSlots], sizeof(SeqCtrl), cudaMemcpyHostToDevice, w.s_in));
 
-    // shared (broadcast) block
+    // shared (broadcast) block: with FBR_ARGS_DEVICE, d.shared is a device pointer too
     if (d.shared != nullptr && d.shared_bytes) {
+        const bool dev_block = (d.flags & FBR_ARGS_DEVICE) != 0;
         if (d.flags & FBR_SHARED_HANDLE) {
             auto it = p->shared.find((uint64_t)(uintptr_t)d.shared);
             if (it == p->shared.end()) return fail(FBR_ENOENT, "unknown shared handle");
             cx.d_shared = (const uint8_t*)it->second.d_ptr[part.worker];
-        } else if (cx.args_dev && !((uintptr_t)d.shared & 15)) {
+        } else if (dev_block && !((uintptr_t)d.shared & 15)) {
             cx.d_shared = (const uint8_t*)d.shared;
-        } else if (cx.args_dev && (body.flags & FBR_BODY_BROADCAST) && d.shared_bytes <= body.shared_stage_bytes) {
+        } else if (dev_block && (body.flags & FBR_BODY_BROADCAST) && d.shared_bytes <= body.shared_stage_bytes) {
             // staged: the kernel copies whatever is not 16 B aligned into shared memory by hand
             cx.d_shared = (const uint8_t*)d.shared;
-        } else if (cx.args_dev) {
+        } else if (dev_block) {
             // a caller's device block at a base that is not 16 B aligned, read in place by the kernel: a body may load its
             // elements as 8 or 16 B vectors (an alignas(16) struct, doubles), which would fault there.  Read an aligned copy.
             CK(cudaMallocAsync(&part.d_shared_tmp, d.shared_bytes, w.s_in));
@@ -1265,19 +1395,13 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
         }
     }
 
-    if (d.n_items && d.arg_stride && body.result_kind == FBR_RES_BITS8)
-        cx.args_limit_bytes = d.n_items * (uint64_t)(d.arg_stride / 8);   // a byte-task's record is 8 items
     // arguments that stay device-resident for the whole map
-    if (cx.args_dev && !cx.peer_push) {
+    if (pl.args == ArgSource::DeviceInPlace) {
         cx.args_full = (const uint8_t*)d.args;
-    } else if (cx.resilient && d.arg_stride) {
+    } else if (pl.args == ArgSource::Resident) {
         // lost units may be re-dispatched at any time: keep every argument record on the device
         CK(cudaMallocAsync(&part.d_args_full, std::max<uint64_t>(16, st.n_tasks * (uint64_t)d.arg_stride), w.s_in));
-        uint64_t abytes = part.count * (uint64_t)d.arg_stride;
-        if (cx.args_limit_bytes) {
-            const uint64_t start = part.first * (uint64_t)d.arg_stride;
-            abytes = start >= cx.args_limit_bytes ? 0 : std::min(abytes, cx.args_limit_bytes - start);
-        }
+        const uint64_t abytes = pl.arg_bytes(part.first, part.count, d.arg_stride);
         if (abytes)
             CK(cudaMemcpyAsync((uint8_t*)part.d_args_full + part.first * (uint64_t)d.arg_stride,
                                (const uint8_t*)d.args + part.first * (uint64_t)d.arg_stride, abytes, cudaMemcpyHostToDevice, w.s_in));
@@ -1288,116 +1412,61 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
     // items: device-resident ones are read in place.  Host-resident ones (offsets checked by fbr_map_submit_items) stream
     // wave by wave through the worker's d_items staging halves (run_wave); a resilient map may re-dispatch any unit at
     // any time, so it copies its part's whole item span and count + 1 offsets to the device once, like d_args_full
-    if (body.flags & FBR_BODY_ITEMS) {
-        if (cx.args_dev) {
-            for (uint32_t k = 0; k < st.n_item_streams; ++k) {
-                const fbr_items_desc_t& it = st.items[k];
-                cx.items[k] = (const uint8_t*)it.items;
-                cx.item_offs[k] = it.offsets;
-                cx.item_base[k] = 0; cx.item_count[k] = it.n_items;
-            }
-            cx.item_first = 0;
-        } else if (!cx.resilient) {
-            cx.host_items = true;
-            for (int i = 0; i < 2; ++i)
-                if (!w.d_items[i]) CK(cudaMalloc((void**)&w.d_items[i], p->ring_bytes));
-        } else {
-            for (uint32_t k = 0; k < st.n_item_streams; ++k) {
-                const fbr_items_desc_t& it = st.items[k];
-                const uint64_t lo = it.offsets[part.first], hi = it.offsets[part.first + part.count];
-                const uint64_t ibytes = (hi - lo) * it.item_bytes, obytes = (part.count + 1) * sizeof(uint64_t);
-                CK(cudaMallocAsync(&part.d_items[k], std::max<uint64_t>(16, ibytes), w.s_in));
-                CK(cudaMallocAsync(&part.d_item_offs[k], obytes, w.s_in));
-                if (ibytes) CK(cudaMemcpyAsync(part.d_items[k], (const uint8_t*)it.items + lo * it.item_bytes, ibytes, cudaMemcpyHostToDevice, w.s_in));
-                CK(cudaMemcpyAsync(part.d_item_offs[k], it.offsets + part.first, obytes, cudaMemcpyHostToDevice, w.s_in));
-                STAT_ADD(p, h2d_bytes, ibytes + obytes);
-                cx.items[k] = (const uint8_t*)part.d_items[k];
-                cx.item_offs[k] = (const uint64_t*)part.d_item_offs[k];
-                cx.item_base[k] = lo; cx.item_count[k] = hi;
-            }
-            cx.item_first = part.first;
+    if (pl.items == ItemSource::DeviceInPlace) {
+        for (uint32_t k = 0; k < st.n_item_streams; ++k) {
+            const fbr_items_desc_t& it = st.items[k];
+            cx.items[k] = ItemStream{(const uint8_t*)it.items, it.offsets, 0, it.n_items};
         }
+        cx.item_first = 0;
+    } else if (pl.items == ItemSource::Staged) {
+        for (int i = 0; i < 2; ++i)
+            if (!w.d_items[i]) CK(cudaMalloc((void**)&w.d_items[i], p->ring_bytes));
+    } else if (pl.items == ItemSource::Resident) {
+        for (uint32_t k = 0; k < st.n_item_streams; ++k) {
+            const fbr_items_desc_t& it = st.items[k];
+            const uint64_t lo = it.offsets[part.first], hi = it.offsets[part.first + part.count];
+            const uint64_t ibytes = (hi - lo) * it.item_bytes, obytes = (part.count + 1) * sizeof(uint64_t);
+            CK(cudaMallocAsync(&part.d_items[k], std::max<uint64_t>(16, ibytes), w.s_in));
+            CK(cudaMallocAsync(&part.d_item_offs[k], obytes, w.s_in));
+            if (ibytes) CK(cudaMemcpyAsync(part.d_items[k], (const uint8_t*)it.items + lo * it.item_bytes, ibytes, cudaMemcpyHostToDevice, w.s_in));
+            CK(cudaMemcpyAsync(part.d_item_offs[k], it.offsets + part.first, obytes, cudaMemcpyHostToDevice, w.s_in));
+            STAT_ADD(p, h2d_bytes, ibytes + obytes);
+            cx.items[k] = ItemStream{(const uint8_t*)part.d_items[k], (const uint64_t*)part.d_item_offs[k], lo, hi};
+        }
+        cx.item_first = part.first;
     }
 
-    // Opt-in (FBR_POOL_OVERLAP): gather(w) runs on a second, higher-priority stream while the next
-    // wave's / next map's dispatch kernel computes; the ring is then used in alternating halves.
-    // On the pi map (ALU-bound dispatch + HBM-bound gather) the gather is a small share of the step and the
-    // two kernels contend for SM slots, so it is off by default.
-    cx.overlap = cx.full_window && !cx.resilient && (p->flags & FBR_POOL_OVERLAP) != 0;
-    // Direct placement: a contiguous, unshuffled, non-resilient block needs neither task records nor the
-    // ring -- unit t of a wave is tasks [wave_first + t*unit, ...) and its results belong at exactly that
-    // index of the ordered window, so the dispatch kernel stores them there and no gather is launched.
-    // (Shuffled arrival, several attempts per unit and FBR_VIA_RING keep the ring + gather_ordered path.)
-    {
-        const bool unit_ok = ((uint64_t)unit * R) % 16 == 0 || unit == 1;   // full vectors are stored 16 B at a time
-        const bool base_ok = !cx.out_dev || (((uintptr_t)d.out + part.first * R) & 15) == 0;
-        cx.direct = !cx.resilient && !(d.flags & (FBR_SHUFFLE | FBR_VIA_RING)) && unit_ok && base_ok;
-    }
-    // wave capacity in claim units
-    uint64_t units_cap = cx.direct ? (1ull << 31) :   // 32-bit unit counter; a direct wave needs no ring space
-        std::min<uint64_t>(kRecCapacity, (cx.overlap ? p->ring_bytes / 2 : p->ring_bytes) / cx.slot_stride);
-    if (cx.host_args) units_cap = std::min<uint64_t>(units_cap, p->ring_bytes / ((uint64_t)unit * d.arg_stride));
-    if (!cx.full_window) units_cap = std::min<uint64_t>(units_cap, p->ring_bytes / ((uint64_t)unit * R));
-    if (units_cap == 0) return fail(FBR_ENOMEM, "ring_bytes=%llu too small for one claim unit of %u tasks", (unsigned long long)p->ring_bytes, unit);
-    cx.wave_tasks_cap = units_cap * unit;
-    // Host-resident output: cut large maps into ~8 waves (>= 8 MiB of results each) so the D2H of
-    // wave w overlaps the kernels of wave w+1 instead of trailing one monolithic launch.
-    if (!cx.full_window || cx.host_args || cx.host_items) {
-        uint64_t bytes_per_task = std::max<uint64_t>(R, cx.host_args ? d.arg_stride : 0);
-        if (cx.host_items && part.count) {   // the mean item bytes and offsets of a task, over every stream
-            const StagedStream s = staged_items(st, part);
-            const uint64_t mean = s.data_bytes(0, part.count) / part.count;
-            bytes_per_task = std::max<uint64_t>(bytes_per_task, mean + s.n * sizeof(uint64_t));
-        }
-        // a wave must carry enough kernel time to hide its launches: 8 MiB of byte results is tens of us of
-        // pi dispatch; a byte of bit-packed results stands for 8 tasks, so 1 MiB is the same work
-        uint64_t min_wave_bytes = body.result_kind == FBR_RES_BITS8 ? (1ull << 20) : (8ull << 20);
-        if (const char* e = getenv("FBR_MIN_WAVE_KB")) min_wave_bytes = std::max<uint64_t>(4096, (uint64_t)atoll(e) << 10);   // tuning knob
-        const uint64_t min_wave_tasks = round_up(std::max<uint64_t>(1, min_wave_bytes / bytes_per_task), unit);
-        // 8 waves for ~100 MB maps, up to 64 for multi-GB ones (~64 MiB per wave): the first wave's
-        // H2D and the last wave's D2H are the only copies nothing overlaps with
-        uint64_t n_waves = std::min<uint64_t>(64, std::max<uint64_t>(8, part.count * bytes_per_task / (64ull << 20)));
-        // small outputs (bit-packed bools): per-copy set-up weighs more: T_kernel/n + n * T_setup is flattest at a few waves
-        if (body.result_kind == FBR_RES_BITS8 && !cx.host_args) n_waves = 6;
-        if (const char* e = getenv("FBR_WAVES")) n_waves = std::max<uint64_t>(1, (uint64_t)atoll(e));                          // tuning knob
-        const uint64_t share = round_up((part.count + n_waves - 1) / n_waves, unit);
-        cx.wave_tasks_cap = std::min(cx.wave_tasks_cap, std::max(min_wave_tasks, share));
-    }
+    if (pl.wave_tasks_cap == 0) return fail(FBR_ENOMEM, "ring_bytes=%llu too small for one claim unit of %u tasks", (unsigned long long)p->ring_bytes, unit);
 
     // staging
-    if (cx.host_args)
+    if (pl.args_streamed())
         for (int i = 0; i < 2; ++i)
             if (!w.d_args[i]) CK(cudaMalloc((void**)&w.d_args[i], p->ring_bytes));
-    if (!cx.full_window)
+    if (pl.staged())
         for (int i = 0; i < 2; ++i)
             if (!w.d_out[i]) CK(cudaMalloc((void**)&w.d_out[i], p->ring_bytes));
-    if (cx.fold) {
+    if (pl.sink == Sink::FoldPartials) {
         CK(cudaMallocAsync(&part.d_fold, std::max<uint64_t>(16, (part.count + unit - 1) / unit * R), w.s_in));
-    } else if (cx.full_window) {
-        if (cx.out_dev) {
-            cx.window_base = (uint8_t*)d.out + part.first * R;
-        } else if (cx.zero_copy) {
-            cx.window_base = (uint8_t*)st.out + part.first * R;     // pinned host memory, mapped into the device's address space (UVA)
-            STAT_ADD(p, d2h_bytes, part.count * (uint64_t)R);        // these bytes cross PCIe as the kernel's own stores
-        } else {
-            CK(cudaMallocAsync(&part.d_window, std::max<uint64_t>(part.count * R, 16), w.s_in));
-            cx.window_base = (uint8_t*)part.d_window;
-        }
+    } else if (pl.sink == Sink::CallerDevice) {
+        cx.window_base = (uint8_t*)d.out + part.first * R;
+    } else if (pl.sink == Sink::ZeroCopy) {
+        cx.window_base = (uint8_t*)st.out + part.first * R;     // pinned host memory, mapped into the device's address space (UVA)
+        STAT_ADD(p, d2h_bytes, part.count * (uint64_t)R);        // these bytes cross PCIe as the kernel's own stores
+    } else if (pl.engine_window()) {
+        CK(cudaMallocAsync(&part.d_window, std::max<uint64_t>(part.count * R, 16), w.s_in));
+        cx.window_base = (uint8_t*)part.d_window;
     }
-    if (cx.resilient) {
+    if (pl.resilient) {
         part.lost_cap = (uint32_t)std::min<uint64_t>((part.count + unit - 1) / unit, 1u << 22);
         CK(cudaMallocAsync((void**)&part.d_lost, sizeof(LostUnit) * std::max<uint32_t>(1, part.lost_cap), w.s_in));
         CK(cudaHostAlloc((void**)&part.h_lost, sizeof(LostUnit) * std::max<uint32_t>(1, part.lost_cap), cudaHostAllocPortable));
     }
 
-    if (d.flags & FBR_WANT_SUM) {
-        if (!(body.flags & FBR_BODY_SUMMABLE)) return fail(FBR_EINVAL, "body %s results cannot be summed", body.name.c_str());
-        cx.sum_kind = 1;   // the dispatch kernel folds sum(results) while they are in registers
-    }
+    if (pl.sum_kind && !(body.flags & FBR_BODY_SUMMABLE)) return fail(FBR_EINVAL, "body %s results cannot be summed", body.name.c_str());
 
     // before any wave launches: every claim unit of every staged stream must fit one staging half
     std::vector<StagedStream> streams;
-    if (cx.host_items) streams.push_back(staged_items(st, part));
+    if (pl.items == ItemSource::Staged) streams.push_back(staged_items(st, part));
     if (part.emit.h_offs)
         streams.push_back({1, {part.emit.h_offs}, {body.out_bytes}, false,
                            "the claim unit of tasks [%llu, %llu) emits %llu value bytes, more than a staging half of "
@@ -1414,22 +1483,8 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
             if (!w.d_vals[i]) CK(cudaMalloc((void**)&w.d_vals[i], p->ring_bytes));
     uint64_t done_tasks = 0;
     while (done_tasks < part.count) {
-        uint64_t wt = std::min<uint64_t>(cx.wave_tasks_cap, part.count - done_tasks);
-        if (!streams.empty()) {
-            // the most whole units (or the rest of the block) whose wave fits one staging half in every stream, at least
-            // one unit (each fits: checked above), by binary search over the host offsets
-            auto fits = [&](uint64_t tasks) {
-                for (const StagedStream& s : streams)
-                    if (s.staged_bytes(done_tasks, done_tasks + tasks) > p->ring_bytes) return false;
-                return true;
-            };
-            uint64_t lo_u = 0, hi_u = (wt + unit - 1) / unit;               // fits(lo_u units) holds (0 tasks always fit)
-            while (lo_u < hi_u) {
-                const uint64_t mid = (lo_u + hi_u + 1) / 2;
-                if (fits(std::min<uint64_t>(mid * unit, wt))) lo_u = mid; else hi_u = mid - 1;
-            }
-            wt = std::min<uint64_t>(std::max<uint64_t>(lo_u, 1) * unit, wt);
-        }
+        uint64_t wt = std::min<uint64_t>(pl.wave_tasks_cap, part.count - done_tasks);
+        if (!streams.empty()) wt = fit_staged_wave(streams, done_tasks, wt, unit, p->ring_bytes);
         const uint32_t n_units = (uint32_t)((wt + unit - 1) / unit);
         const uint64_t wno = w.wave_no++;
         const int rw = (int)(wno % kRecWindows);
@@ -1448,7 +1503,7 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
                 r.seq = (uint32_t)st.seq;
                 r.count = (uint32_t)std::min<uint64_t>(unit, wt - off);
                 r.first = wave_first + off;
-                r.arg_off = cx.host_args ? off * (uint64_t)d.arg_stride : (wave_first + off) * (uint64_t)d.arg_stride;
+                r.arg_off = pl.args_streamed() ? off * (uint64_t)d.arg_stride : (wave_first + off) * (uint64_t)d.arg_stride;
                 r.func_id = (uint32_t)st.func_id;
                 r.attempt = part.attempt;
             }
@@ -1460,14 +1515,14 @@ static int submit_part(fbr_pool* p, SeqState& st, SeqPart& part, const BodyEntry
         part.wave_cum.push_back(done_tasks);
     }
     // resilient parts copy the window back only once no unit is lost any more (resilient_advance)
-    return finish_round(p, st, part, !cx.resilient);
+    return finish_round(p, st, part, !pl.resilient);
 }
 
 // ResilientZPool semantics (fiber/pool.py:1612-1659): once a round has finished, re-queue the units
 // whose worker died (their slot header carries kUnitLost; gather listed them) with attempt+1, until
 // none is lost; then copy the ordered window back.  Returns 1 while more work was launched.
 static int resilient_advance(fbr_pool* p, SeqState& st, SeqPart& part) {
-    if (!part.cx.resilient || part.finalized) return 0;
+    if (!part.cx.plan.resilient || part.finalized) return 0;
     Worker& w = p->workers[part.worker];
     CK(cudaSetDevice(w.device));
     const BodyEntry& body = *body_of(st.func_id);
@@ -1483,7 +1538,7 @@ static int resilient_advance(fbr_pool* p, SeqState& st, SeqPart& part) {
     // clear the device lost counter (sum/err keep accumulating: lost units were never placed)
     static const uint32_t kZero = 0;
     CK(cudaMemcpyAsync(&w.d_ctrl[part.ctrl_slot].lost_count, &kZero, sizeof(uint32_t), cudaMemcpyHostToDevice, w.s_in));
-    const uint64_t units_cap = std::max<uint64_t>(1, std::min<uint64_t>(kRecCapacity, p->ring_bytes / part.cx.slot_stride));
+    const uint64_t units_cap = part.cx.plan.redispatch_units_cap;
     for (size_t i = 0; i < todo.size(); i += units_cap) {
         const uint32_t n_units = (uint32_t)std::min<uint64_t>(units_cap, todo.size() - i);
         const uint64_t wno = w.wave_no++;
@@ -1542,12 +1597,9 @@ static void cut_blocks(fbr_pool* p, const BodyEntry& body, const fbr_map_desc_t&
                        const std::vector<int>& workers, uint32_t attempt, std::vector<SeqPart>& out) {
     const int nw = (int)workers.size();
     if (nw == 0 || count == 0) return;
-    const uint32_t unit = pick_unit(body, map_chunksize(d), (count + nw - 1) / nw, p->workers[workers[0]].sm_count, p->ring_bytes);
-    const uint64_t units_total = (count + unit - 1) / unit;
-    const uint64_t units_per = (units_total + nw - 1) / nw;
     for (int i = 0; i < nw; ++i) {
-        const uint64_t b0 = std::min<uint64_t>(count, (uint64_t)i * units_per * unit);
-        const uint64_t b1 = std::min<uint64_t>(count, (uint64_t)(i + 1) * units_per * unit);
+        uint64_t b0, b1;
+        cut_block(body, map_chunksize(d), count, nw, i, p->workers[workers[0]].sm_count, p->ring_bytes, &b0, &b1);
         if (b1 <= b0) continue;
         SeqPart part;
         part.worker = workers[i];
@@ -1607,7 +1659,7 @@ static void on_worker_death(fbr_pool* p, int wi, cudaError_t err) {
         for (auto& part : st.parts) {
             if (part.worker != wi) { next.push_back(std::move(part)); continue; }
             cut_blocks(p, body, st.desc, part.first, part.count, live, part.attempt + 1, next);
-            st.redispatched_units += (uint32_t)((part.count + std::max<uint32_t>(1, part.cx.unit) - 1) / std::max<uint32_t>(1, part.cx.unit));
+            st.redispatched_units += (uint32_t)((part.count + std::max<uint32_t>(1, part.cx.plan.unit) - 1) / std::max<uint32_t>(1, part.cx.plan.unit));
             st.graveyard.push_back(std::move(part));
         }
         st.parts.swap(next);
@@ -1953,18 +2005,17 @@ int fbr_plan_query(int func_id, uint64_t n_tasks, uint32_t chunksize, uint64_t r
         return fail(FBR_EINVAL, "bad arguments");
     const BodyEntry& body = *body_of(func_id);
     const uint64_t ring = round_up(ring_bytes ? ring_bytes : (256ull << 20), 4096);
-    const uint32_t cs = chunksize ? chunksize : 32u;
+    fbr_map_desc_t d{};
+    d.chunksize = chunksize;   // map_chunksize: 0 is 32, FBR_PLAN_FOLD cuts as a fold map
     if (sm_count <= 0) sm_count = 132;
-    // the same two steps fbr_map_submit takes: blocks on the map-level unit, then the block's own unit
-    const uint32_t unit = pick_unit(body, cs, (n_tasks + n_workers - 1) / n_workers, sm_count, ring);
-    const uint64_t units_total = (n_tasks + unit - 1) / unit;
-    const uint64_t units_per = (units_total + n_workers - 1) / n_workers;
-    const uint64_t b0 = std::min<uint64_t>(n_tasks, (uint64_t)worker * units_per * unit);
-    const uint64_t b1 = std::min<uint64_t>(n_tasks, (uint64_t)(worker + 1) * units_per * unit);
+    // what fbr_map_submit does: cut_blocks, then plan_block of the worker's block
+    uint64_t b0, b1;
+    cut_block(body, map_chunksize(d), n_tasks, n_workers, worker, sm_count, ring, &b0, &b1);
+    const BlockPlan pl = plan_block(body, d, 0, worker, b0, b1 - b0, true, sm_count, ring, true, 0);
     plan->block_first = b0;
     plan->block_count = b1 - b0;
-    plan->unit_tasks = pick_unit(body, cs, b1 - b0, sm_count, ring);
-    plan->slot_stride = (uint32_t)round_up((uint64_t)plan->unit_tasks * body.result_bytes, 16);
+    plan->unit_tasks = pl.unit;
+    plan->slot_stride = pl.slot_stride;
     plan->n_units = plan->block_count ? (plan->block_count + plan->unit_tasks - 1) / plan->unit_tasks : 0;
     return FBR_OK;
 }
@@ -2960,7 +3011,7 @@ int fbr_result_poll(fbr_pool_t* p, uint64_t seq, uint64_t* n_done) {
         }
         cudaGetLastError();
         const bool part_finished = q == cudaSuccess;
-        if (part.cx.resilient) {
+        if (part.cx.plan.resilient) {
             // results become visible only once no unit is lost any more; polling drives the rounds
             if (part_finished) {
                 if (part.finalized) { done += part.count; continue; }
@@ -2974,7 +3025,7 @@ int fbr_result_poll(fbr_pool_t* p, uint64_t seq, uint64_t* n_done) {
             break;
         }
         uint64_t part_done = 0;
-        if (part.cx.full_window && (part.cx.scan || (!part.cx.out_dev && !part.cx.keep_on_device))) {
+        if (part.cx.plan.final_at_block_end()) {
             // the window reaches the host in one copy at the end, or (a scan block, results on the device too) its prefix
             // folds are written in place behind its last wave: nothing is final before that
             if (part_finished) { done += part.count; continue; }

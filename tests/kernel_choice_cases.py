@@ -1,6 +1,6 @@
 """The kernel choice table: which gather and dispatch kernel each map of the kernel-choice suite is meant to reach.
 
-The engine picks a gather kernel per wave (engine.cu, the ``aligned`` / ``rows_ok`` / ``bulk_ok`` lines of run_wave) and the
+The engine picks a gather kernel per wave (engine.cu ``pick_gather``, from the block's ``BlockPlan``) and the
 payload body picks its dispatch kernel per launch (``launch_payload_map``), from the claim unit, the slot stride, the
 output pointer and the map flags.  ``expected_kernel`` and ``expected_dispatch`` restate those rules;
 ``CASES`` lists the maps, each with the cell (kernel and the edge of its index arithmetic) it is meant to reach; ``CELLS``
@@ -97,7 +97,7 @@ def case_plan(c):
 
 
 def expected_kernel(plan, R, flags, out_ptr):
-    """The kernel that places a wave's results (engine.cu run_wave): "direct" (the dispatch kernel stores at the final
+    """The kernel that places a wave's results (engine.cu pick_gather): "direct" (the dispatch kernel stores at the final
     index, no gather), or the gather kernel "bulk", "rows" or "flat".  out_ptr: the caller's device output (FBR_OUT_DEVICE)
     or 0."""
     unit, slot = plan.unit_tasks, plan.slot_stride

@@ -83,7 +83,7 @@ def test_plan_keeps_every_unit_16_byte_aligned():
 
 
 def _gather_route(slot_stride, unit, R, resilient):
-    """The gather kernel the wave planner picks for a map's full units (engine.cu, the rows_ok / bulk_ok lines):
+    """The gather kernel the wave planner picks for a map's full units (engine.cu, pick_gather):
     gather_bulk_kernel for 16 KB multiples (not on resilient maps), gather_rows_kernel for 4 KB multiples, else
     gather_ordered_kernel (flat)."""
     rows = unit * R == slot_stride and slot_stride % 4096 == 0
