@@ -36,6 +36,7 @@ FBR_FOLD = 0x4000
 FBR_SCAN = 0x8000
 FBR_FOLD_KEYS = 0x10000
 FBR_MAX_KEYS = 65536
+FBR_FOLD_SPARSE_KEYS = 0x20000
 FBR_PLAN_FOLD = 0xFFFFFFFF   # fbr_plan_query's chunksize for the plan of a fold map
 # fbr_task_error
 FBR_TASK_OK, FBR_TASK_OVERFLOW, FBR_TASK_BADARG, FBR_TASK_FAULT = range(4)
@@ -47,7 +48,7 @@ SYMBOLS = [
     "fbr_abi_version", "fbr_last_error", "fbr_device_count",
     "fbr_body_count", "fbr_body_info", "fbr_body_lookup", "fbr_register_body", "fbr_body_shared_info",
     "fbr_body_items_info", "fbr_body_emit_info", "fbr_body_items_streams", "fbr_body_fold_info", "fbr_fold_values",
-    "fbr_scan_values", "fbr_fold_segments",
+    "fbr_scan_values", "fbr_fold_segments", "fbr_result_groups",
     "fbr_pool_create", "fbr_pool_close", "fbr_pool_terminate", "fbr_pool_join", "fbr_pool_destroy",
     "fbr_pool_n_workers", "fbr_pool_worker_device",
     "fbr_map_submit", "fbr_map_submit_items", "fbr_map_submit_items_n", "fbr_shared_put", "fbr_shared_drop", "fbr_plan_query",
@@ -166,6 +167,7 @@ def load():
         "fbr_fold_values": (i32, [vp, i32, vp, u64, vp]),
         "fbr_scan_values": (i32, [vp, i32, vp, u32, vp, u64]),
         "fbr_fold_segments": (i32, [vp, i32, vp, vp, u32, vp]),
+        "fbr_result_groups": (i32, [vp, u64, P(u64), P(vp), P(vp)]),
         "fbr_pool_create": (i32, [i32, P(i32), u64, u32, P(vp)]),
         "fbr_pool_close": (i32, [vp]),
         "fbr_pool_terminate": (i32, [vp]),

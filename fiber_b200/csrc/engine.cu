@@ -294,8 +294,11 @@ struct TimedPair { cudaEvent_t a, b; };
 //   WindowOnDevice  an engine window that stays on the device (FBR_RESULTS_ON_DEVICE)
 //   ScanWindow    an engine window, rewritten into the block's prefix folds after its last round (FBR_SCAN)
 //   KeyedWindow   an engine window, sorted by key and folded per key after its last round (FBR_FOLD_KEYS)
+//   SparseKeyedWindow  an engine window, sorted by key and cut into runs of equal keys after its last round; the runs are
+//                 folded at completion (FBR_FOLD_SPARSE_KEYS)
 //   FoldPartials  each unit's tree, in d_fold: no result leaves the device (FBR_FOLD)
-enum class Sink : uint8_t { Staged, StagedPeer, CallerDevice, ZeroCopy, WindowToHost, WindowOnDevice, ScanWindow, KeyedWindow, FoldPartials };
+enum class Sink : uint8_t { Staged, StagedPeer, CallerDevice, ZeroCopy, WindowToHost, WindowOnDevice, ScanWindow, KeyedWindow,
+                            SparseKeyedWindow, FoldPartials };
 // Where a block's argument records come from: none (range() indices), the caller's device memory read in place
 // (FBR_ARGS_DEVICE), a device copy of the block's records made once (Resident: a resilient unit may be re-dispatched at any
 // time), the host wave by wave through the d_args staging halves, or device memory of worker 0 pushed wave by wave into the
@@ -340,6 +343,7 @@ struct PartCtx {
     uint8_t* fold_total = nullptr;        // FBR_FOLD: the block's total, in the map's pinned segment
     uint8_t* key_totals = nullptr;        // FBR_FOLD_KEYS: the block's n_keys totals and counts, in the map's pinned segment
     uint8_t* key_counts = nullptr;
+    uint64_t* n_groups = nullptr;         // FBR_FOLD_SPARSE_KEYS: the block's D, its word of SeqState::sparse_words
     const uint8_t* d_shared = nullptr;
     uint8_t* window_base = nullptr;       // the block's window (BlockPlan::windowed)
     const uint8_t* args_full = nullptr;   // device-resident arguments of the whole map (DeviceInPlace / Resident)
@@ -385,6 +389,7 @@ struct SeqPart {
     bool finalized = false;               // resilient: window copied back to the host
     bool first_wave_pending = true;       // the block's first wave must wait for what submit_part put on s_in
     void* d_fold = nullptr;               // FBR_FOLD: the partial of each claim unit, by its place in the block
+    void* d_sparse = nullptr;             // FBR_FOLD_SPARSE_KEYS: gathered records, run starts, keys (sparse_keep_layout)
     PartCtx cx;
     EmitBlock emit;
 };
@@ -420,7 +425,12 @@ struct SeqState {
                                            // tree() over the block totals, and a scan map's blocks after the first are wrapped
     std::vector<uint8_t> scan_totals;      // FBR_SCAN, several blocks: every block's total in block order, read before any
                                            // block is wrapped (the wrap rewrites the record that holds it)
-    std::vector<cudaEvent_t> scan_done;    // ... and block b's wrap (and D2H copy) once queued on its worker's s_fold
+    std::vector<cudaEvent_t> block_done;   // ... and block b's wrap (and D2H copy) once queued on its worker's s_fold; a sparse
+                                           // keyed map's block b's run fold and D2H copy (sparse_keyed_finish)
+    uint64_t* sparse_words = nullptr;      // FBR_FOLD_SPARSE_KEYS: each block's D, in pinned memory its run scan writes into
+    std::vector<void*> sparse_host;        // ... block b's totals, keys and run starts once copied out (pinned, block order)
+    std::vector<uint32_t> group_keys;      // ... and the result's distinct keys and counts (fbr_result_groups)
+    std::vector<uint64_t> group_counts;
 };
 
 struct SharedBlock {
@@ -744,7 +754,7 @@ static uint32_t pick_unit(const BodyEntry& b, uint32_t chunksize, uint64_t n_tas
 
 // the chunksize a map's units are picked for: a fold map's units ignore it (FBR_PLAN_FOLD)
 static uint32_t map_chunksize(const fbr_map_desc_t& d) {
-    if (d.flags & (FBR_FOLD | FBR_SCAN | FBR_FOLD_KEYS)) return FBR_PLAN_FOLD;   // scan and keyed maps cut blocks as a fold
+    if (d.flags & (FBR_FOLD | FBR_SCAN | FBR_FOLD_KEYS | FBR_FOLD_SPARSE_KEYS)) return FBR_PLAN_FOLD;   // scan and keyed maps cut blocks as a fold
     return d.chunksize ? d.chunksize : 32u;
 }
 
@@ -769,6 +779,7 @@ static BlockPlan plan_block(const BodyEntry& body, const fbr_map_desc_t& d, uint
                               !(d.flags & (FBR_FULL_WINDOW | FBR_SHUFFLE | FBR_VIA_RING | FBR_NO_ZERO_COPY));
     if (d.flags & FBR_FOLD) pl.sink = Sink::FoldPartials;
     else if (d.flags & FBR_FOLD_KEYS) pl.sink = Sink::KeyedWindow;
+    else if (d.flags & FBR_FOLD_SPARSE_KEYS) pl.sink = Sink::SparseKeyedWindow;
     else if (d.flags & FBR_SCAN) pl.sink = Sink::ScanWindow;
     else if (d.flags & FBR_OUT_DEVICE)
         pl.sink = worker != 0 && !pl.resilient && !out_off && !(d.flags & FBR_FULL_WINDOW) ? Sink::StagedPeer : Sink::CallerDevice;
@@ -1287,6 +1298,94 @@ static int fold_block_by_key(fbr_pool* p, SeqState& st, SeqPart& part) {
     return FBR_OK;
 }
 
+// Where a sparse keyed block keeps its gathered records (at 0), run starts (n + 1 words) and keys (n words) in d_sparse.
+static uint64_t sparse_keep_layout(uint64_t n, uint64_t R, uint64_t* o_starts, uint64_t* o_keys) {
+    *o_starts = round_up(n * R, 256);
+    *o_keys = round_up(*o_starts + 8 * (n + 1), 256);
+    return *o_keys + 4 * n;
+}
+
+// FBR_FOLD_SPARSE_KEYS, a block's last round, queued on its worker's s_out behind its last wave: the body's keys entry with
+// n_keys = 0xFFFFFFFF writes each task's key (the reserved key goes into the block's error word), four LSD radix passes sort
+// the (key, task) pairs -- always four: which digits a block uses is not known on the host without a synchronisation -- and
+// the records are gathered into key order.  run_heads_kernel flags each run of equal keys, the scan of the flags numbers the
+// runs and writes D, their number, into the block's pinned word, and run_starts_kernel writes each run's start and key.  The
+// window and the sort's scratch (about 40 B per task) are freed here; the gathered records, starts and keys stay in
+// part.d_sparse until sparse_keyed_finish folds the runs, since D is known on the host only then.
+static int sparse_block_step(fbr_pool* p, SeqState& st, SeqPart& part) {
+    Worker& w = p->workers[part.worker];
+    const BodyEntry& body = *body_of(st.func_id);
+    const PartCtx& cx = part.cx;
+    const cudaStream_t s = w.s_out;
+    const uint32_t n = (uint32_t)part.count;
+    const uint64_t R = body.result_bytes;
+    const uint32_t n_tiles = (n + keyed::kTile - 1) / keyed::kTile;
+    const uint64_t H = (uint64_t)keyed::kBins * n_tiles, scan_tiles = H / scan::kTile + 1, run_tiles = n / scan::kTile + 1;
+    uint64_t at = 0;
+    auto take = [&](uint64_t bytes) { const uint64_t o = at; at = round_up(at + bytes, 256); return o; };
+    const uint64_t o_keys0 = take(4ull * n), o_keys1 = take(4ull * n), o_idx0 = take(4ull * n), o_idx1 = take(4ull * n),
+                   o_hist = take(8 * H), o_hoffs = take(8 * (H + 1)), o_state = take(8 * (scan_tiles + 2)),
+                   o_head = take(8ull * n), o_run = take(8ull * (n + 1)), o_rstate = take(8 * (run_tiles + 2));
+    uint64_t o_starts, o_dkeys;
+    const uint64_t keep_bytes = sparse_keep_layout(n, R, &o_starts, &o_dkeys);
+    uint8_t *buf = nullptr, *keep = nullptr;
+    cudaError_t e = cudaMallocAsync((void**)&buf, at, s);
+    if (e == cudaSuccess) e = cudaMallocAsync((void**)&keep, keep_bytes, s);
+    if (e != cudaSuccess) {
+        if (buf) cudaFreeAsync(buf, s);
+        cudaGetLastError();
+        return fail(e == cudaErrorMemoryAllocation ? FBR_ENOMEM : FBR_ECUDA, "sparse keyed fold of body %s on worker %d: %llu bytes "
+                    "of device memory: %s", body.name.c_str(), part.worker, (unsigned long long)(at + keep_bytes), cudaGetErrorString(e));
+    }
+    part.d_sparse = keep;
+    uint32_t* keys[2] = {(uint32_t*)(buf + o_keys0), (uint32_t*)(buf + o_keys1)};
+    uint32_t* idx[2] = {(uint32_t*)(buf + o_idx0), (uint32_t*)(buf + o_idx1)};
+    uint64_t* const hist = (uint64_t*)(buf + o_hist);
+    uint64_t* const hoffs = (uint64_t*)(buf + o_hoffs);
+    uint64_t* const state = (uint64_t*)(buf + o_state);   // scan_counts_kernel: tile states, ticket, total
+    uint64_t* const head = (uint64_t*)(buf + o_head);
+    uint64_t* const run = (uint64_t*)(buf + o_run);
+    uint64_t* const rstate = (uint64_t*)(buf + o_rstate);
+    e = (cudaError_t)body.keys(cx.window_base, n, 0xFFFFFFFFu, st.desc.task_index_base + part.first, keys[0],
+                               &w.d_ctrl[part.ctrl_slot].err, (void*)s);
+    const unsigned sort_grid = (unsigned)std::min<uint32_t>(n_tiles, 1u << 16);
+    int cur = 0;
+    for (int pass = 0; pass < 4 && e == cudaSuccess; ++pass, cur ^= 1) {
+        radix_hist_kernel<<<sort_grid, keyed::kThreads, 0, s>>>(keys[cur], n, 8 * pass, hist, n_tiles);
+        e = cudaMemsetAsync(state, 0, 8 * (scan_tiles + 2), s);
+        if (e != cudaSuccess) break;
+        scan_counts_kernel<<<(unsigned)scan_tiles, scan::kThreads, 0, s>>>(hist, H, hoffs, (unsigned long long*)state,
+                                                                          (uint32_t*)(state + scan_tiles), state + scan_tiles + 1);
+        radix_scatter_kernel<<<sort_grid, keyed::kThreads, 0, s>>>(keys[cur], pass ? idx[cur] : nullptr, keys[cur ^ 1], idx[cur ^ 1], n,
+                                                                   8 * pass, hoffs, n_tiles);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) {
+        const uint32_t W = R % 16 == 0 ? 16 : R % 8 == 0 ? 8 : 4;
+        const uint64_t words = R / W, grid = std::min<uint64_t>((n * words + kThreads - 1) / kThreads, 1u << 16);
+        if (W == 16) gather_records_kernel<uint4><<<(unsigned)grid, kThreads, 0, s>>>((const uint4*)cx.window_base, (uint4*)keep, idx[cur], n, (uint32_t)words);
+        else if (W == 8) gather_records_kernel<uint2><<<(unsigned)grid, kThreads, 0, s>>>((const uint2*)cx.window_base, (uint2*)keep, idx[cur], n, (uint32_t)words);
+        else gather_records_kernel<uint32_t><<<(unsigned)grid, kThreads, 0, s>>>((const uint32_t*)cx.window_base, (uint32_t*)keep, idx[cur], n, (uint32_t)words);
+        const unsigned grid_n = (unsigned)std::min<uint64_t>(((uint64_t)n + kThreads - 1) / kThreads, 1u << 16);
+        run_heads_kernel<<<grid_n, kThreads, 0, s>>>(keys[cur], n, head);
+        e = cudaMemsetAsync(rstate, 0, 8 * (run_tiles + 2), s);
+        if (e == cudaSuccess) {
+            scan_counts_kernel<<<(unsigned)run_tiles, scan::kThreads, 0, s>>>(head, n, run, (unsigned long long*)rstate,
+                                                                             (uint32_t*)(rstate + run_tiles), cx.n_groups);
+            run_starts_kernel<<<grid_n, kThreads, 0, s>>>(keys[cur], n, run, (uint64_t*)(keep + o_starts), (uint32_t*)(keep + o_dkeys));
+            e = cudaGetLastError();
+        }
+    }
+    cudaFreeAsync(buf, s);
+    cudaFreeAsync(part.d_window, s);   // the window never leaves the device: the gathered copy replaces it
+    part.d_window = nullptr;
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return fail(FBR_ECUDA, "sparse keyed fold of body %s on worker %d: %s", body.name.c_str(), part.worker, cudaGetErrorString(e));
+    }
+    return FBR_OK;
+}
+
 // Control block (+ lost list) back to the pinned mirror, completion event.
 static int finish_round(fbr_pool* p, SeqState& st, SeqPart& part, bool copy_window) {
     Worker& w = p->workers[part.worker];
@@ -1316,6 +1415,10 @@ static int finish_round(fbr_pool* p, SeqState& st, SeqPart& part, bool copy_wind
         }
         if (pl.sink == Sink::KeyedWindow) {
             const int rc = fold_block_by_key(p, st, part);
+            if (rc != FBR_OK) return rc;
+        }
+        if (pl.sink == Sink::SparseKeyedWindow) {
+            const int rc = sparse_block_step(p, st, part);
             if (rc != FBR_OK) return rc;
         }
     }
@@ -1649,7 +1752,7 @@ static void on_worker_death(fbr_pool* p, int wi, cudaError_t err) {
         // an emit pass's blocks carry the offsets of the workers that counted them, and a fold, scan or keyed map's order depends
         // on its block cut: both are failed, not re-cut
         if (!(st.flags & FBR_RESILIENT) || live.empty() || (on_w0 && p->workers[0].dead) || st.emit_pass ||
-            (st.flags & (FBR_FOLD | FBR_SCAN | FBR_FOLD_KEYS))) {
+            (st.flags & (FBR_FOLD | FBR_SCAN | FBR_FOLD_KEYS | FBR_FOLD_SPARSE_KEYS))) {
             st.dead_worker = wi;
             st.dead_error = (int)err;
             continue;
@@ -1696,10 +1799,10 @@ static void free_emit_block(fbr_pool* p, int worker, EmitBlock& e) {
 
 static void free_seq(fbr_pool* p, SeqState& st) {
     // a scan map's wraps run on s_fold, its windows are freed on s_in: a wrap still in flight finishes first
-    for (cudaEvent_t ev : st.scan_done)
+    for (cudaEvent_t ev : st.block_done)
         if (ev) { cudaEventSynchronize(ev); cudaEventDestroy(ev); }
     cudaGetLastError();
-    st.scan_done.clear();
+    st.block_done.clear();
     for (auto& part : st.graveyard)        // device-side resources died with the worker's context
         if (part.h_lost) cudaFreeHost(part.h_lost);
     st.graveyard.clear();
@@ -1726,12 +1829,18 @@ static void free_seq(fbr_pool* p, SeqState& st) {
         }
         if (part.d_lost) cudaFreeAsync(part.d_lost, w.s_in);
         if (part.d_fold) cudaFreeAsync(part.d_fold, w.s_in);
+        if (part.d_sparse) cudaFreeAsync(part.d_sparse, w.s_in);
         free_emit_block(p, part.worker, part.emit);
         if (part.h_lost) cudaFreeHost(part.h_lost);
         if (part.ctrl_slot >= 0) w.ctrl_free.push_back(part.ctrl_slot);
     }
     if (st.values) pinned_release(p, st.values);
     st.values = nullptr;
+    for (void* h : st.sparse_host)
+        if (h) pinned_release(p, h);
+    st.sparse_host.clear();
+    if (st.sparse_words) pinned_release(p, st.sparse_words);
+    st.sparse_words = nullptr;
     if (st.own_out && st.out && !numa_pinned_release(p, st.out)) pinned_release(p, st.out);
 }
 
@@ -2449,6 +2558,20 @@ static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_ite
     if ((d->flags & FBR_RESULTS_ON_DEVICE) && ((d->flags & FBR_OUT_DEVICE) || d->out))
         return fail(FBR_EINVAL, "FBR_RESULTS_ON_DEVICE owns its output buffer: do not pass out / FBR_OUT_DEVICE");
     if ((d->flags & FBR_RESILIENT) && (d->flags & FBR_SHUFFLE)) return fail(FBR_EINVAL, "FBR_RESILIENT cannot be combined with FBR_SHUFFLE");
+    if (d->flags & FBR_FOLD_SPARSE_KEYS) {
+        if (!(body.flags & FBR_BODY_KEYED))
+            return fail(FBR_EINVAL, "body %s has no key(): its maps cannot fold per key (FBR_FOLD_SPARSE_KEYS needs FBR_BODY_KEYED)", body.name.c_str());
+        if (d->flags & (FBR_FOLD | FBR_SCAN | FBR_FOLD_KEYS))
+            return fail(FBR_EINVAL, "FBR_FOLD_SPARSE_KEYS cannot be combined with FBR_FOLD, FBR_SCAN or FBR_FOLD_KEYS");
+        if (d->out || (d->flags & (FBR_OUT_DEVICE | FBR_WANT_SUM | FBR_NO_ZERO_COPY)))
+            return fail(FBR_EINVAL, "a sparse keyed fold map (FBR_FOLD_SPARSE_KEYS) of body %s owns its result records: no out, "
+                        "FBR_OUT_DEVICE, FBR_WANT_SUM or FBR_NO_ZERO_COPY", body.name.c_str());
+        if (d->n_keys != 0)
+            return fail(FBR_EINVAL, "a sparse keyed fold map (FBR_FOLD_SPARSE_KEYS) takes no n_keys (%u): its keys are any uint32 "
+                        "but 0xFFFFFFFF", d->n_keys);
+        if (d->n_tasks > 0xffffffffull)   // a block's tasks are sorted as uint32 indices
+            return fail(FBR_EINVAL, "a sparse keyed fold map takes fewer than 2^32 tasks (%llu)", (unsigned long long)d->n_tasks);
+    }
     // (before the generic FBR_WANT_SUM check: a scan body is never summable, and the scan map says why)
     if (d->flags & FBR_SCAN) {
         if (!(body.flags & FBR_BODY_SCAN))
@@ -2508,7 +2631,8 @@ static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_ite
         st->n_item_streams = items ? n_streams : 0;
         for (uint32_t k = 0; k < st->n_item_streams; ++k) st->items[k] = items[k];
         const bool fold = (d->flags & FBR_FOLD) != 0, keyed = (d->flags & FBR_FOLD_KEYS) != 0;
-        const bool need_segment = !st->out && d->n_tasks && !(d->flags & FBR_RESULTS_ON_DEVICE) && !fold && !keyed;
+        const bool sparse = (d->flags & FBR_FOLD_SPARSE_KEYS) != 0;
+        const bool need_segment = !st->out && d->n_tasks && !(d->flags & FBR_RESULTS_ON_DEVICE) && !fold && !keyed && !sparse;
         // host allocations fail with the sticky error too once a context of this process has died: tell the two apart
         auto died_meanwhile = [&]() {
             bool any = false;
@@ -2549,6 +2673,12 @@ static int map_submit_pass(fbr_pool_t* p, const fbr_map_desc_t* d, const fbr_ite
                 st->parts[k].cx.key_totals = a;
                 st->parts[k].cx.key_counts = a + K * body.result_bytes;
             }
+        }
+        if (sparse && !st->parts.empty()) {
+            // each block's D, written by its run scan; the result is sized at completion, once every D is known
+            int rc = pinned_acquire(p, st->parts.size() * sizeof(uint64_t), (void**)&st->sparse_words);
+            if (rc != FBR_OK) return rc;
+            for (size_t k = 0; k < st->parts.size(); ++k) st->parts[k].cx.n_groups = st->sparse_words + k;
         }
         if (counted) {
             // the emit pass runs over the blocks the count pass counted
@@ -2712,6 +2842,135 @@ static int keyed_finish(fbr_pool* p, SeqState& st) {
     return FBR_OK;
 }
 
+// Where sparse_keyed_finish puts block b's D totals, D keys and D + 1 run starts in its pinned buffer.
+static uint64_t sparse_host_layout(uint64_t D, uint64_t R, uint64_t* o_keys, uint64_t* o_starts) {
+    *o_keys = round_up(D * R, 8);
+    *o_starts = round_up(*o_keys + 4 * D, 8);
+    return *o_starts + 8 * (D + 1);
+}
+
+// FBR_FOLD_SPARSE_KEYS, once every block is done: block b's D_b is in its pinned word, and its gathered records, run starts
+// and keys are on its worker's device (sparse_block_step).  The first call queues, for each block, the body's fold_segments
+// entry over its D_b runs on its worker's s_fold, then the D2H copy of the D_b totals, keys and starts into pinned memory,
+// behind the event st.block_done[b]; a call that failed part-way resumes at the first block without one.  Once every copy
+// is in, one block's totals are the result.  Several blocks' sorted keys are merged on the host, stable by key with block
+// order inside a key, which gives the key-major sequence of block totals and its offsets: one fold_segments_host folds it
+// and the counts are summed.  The result records are sized exactly here.  With `block` the copies are waited for here;
+// otherwise *ready tells whether they have all finished (fbr_result_wait waits for them outside the lock).
+static int sparse_keyed_finish(fbr_pool* p, SeqState& st, bool block, bool* ready) {
+    const BodyEntry& body = *body_of(st.func_id);
+    const uint64_t R = body.result_bytes;
+    const std::vector<SeqPart*> blocks = parts_in_order(st);
+    const size_t nb = blocks.size();
+    if (st.block_done.empty()) {
+        st.block_done.assign(nb, nullptr);
+        st.sparse_host.assign(nb, nullptr);
+    }
+    for (size_t b = 0; b < nb; ++b) {
+        if (st.block_done[b]) continue;           // queued by an earlier call
+        SeqPart& part = *blocks[b];
+        Worker& w = p->workers[part.worker];
+        if (w.dead) return fail(FBR_ECUDA, "worker %d died before its block of a sparse keyed fold map was folded", part.worker);
+        const uint64_t D = *part.cx.n_groups;
+        uint64_t o_starts, o_dkeys, h_keys, h_starts;
+        sparse_keep_layout(part.count, R, &o_starts, &o_dkeys);
+        const uint64_t hbytes = sparse_host_layout(D, R, &h_keys, &h_starts);
+        if (!st.sparse_host[b]) {
+            const int rc = pinned_acquire(p, hbytes, &st.sparse_host[b]);
+            if (rc != FBR_OK) return rc;
+        }
+        uint8_t* const h = (uint8_t*)st.sparse_host[b];
+        uint8_t* const keep = (uint8_t*)part.d_sparse;
+        uint8_t* totals = nullptr;
+        cudaError_t e = cudaSetDevice(w.device);
+        if (e == cudaSuccess) e = cudaMallocAsync((void**)&totals, D * R, w.s_fold);
+        if (e == cudaSuccess)
+            e = (cudaError_t)body.fold_segments(keep, part.count, (const uint64_t*)(keep + o_starts), (uint32_t)D, totals, (void*)w.s_fold);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(h, totals, D * R, cudaMemcpyDeviceToHost, w.s_fold);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(h + h_keys, keep + o_dkeys, 4 * D, cudaMemcpyDeviceToHost, w.s_fold);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(h + h_starts, keep + o_starts, 8 * (D + 1), cudaMemcpyDeviceToHost, w.s_fold);
+        if (totals) cudaFreeAsync(totals, w.s_fold);
+        cudaEvent_t ev = nullptr;
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventRecord(ev, w.s_fold);
+        if (e != cudaSuccess) {
+            if (ev) cudaEventDestroy(ev);
+            retire_if_dead(p, part.worker);
+            return fail(FBR_ECUDA, "folding the runs of block %zu of a sparse keyed fold map of body %s on worker %d: %s", b,
+                        body.name.c_str(), part.worker, cudaGetErrorString(e));
+        }
+        st.block_done[b] = ev;
+        cudaFreeAsync(part.d_sparse, w.s_fold);   // behind the copies
+        part.d_sparse = nullptr;
+        p->stats.d2h_bytes += D * R + 4 * D + 8 * (D + 1);
+    }
+    for (size_t b = 0; b < nb; ++b) {
+        const int wi = blocks[b]->worker;
+        cudaError_t q = p->workers[wi].dead ? cudaErrorUnknown : cudaSetDevice(p->workers[wi].device);
+        if (q == cudaSuccess) q = block ? cudaEventSynchronize(st.block_done[b]) : cudaEventQuery(st.block_done[b]);
+        if (q == cudaErrorNotReady) { cudaGetLastError(); *ready = false; return FBR_OK; }
+        if (q != cudaSuccess) {
+            retire_if_dead(p, wi);
+            return fail(FBR_ECUDA, "folding the runs of block %zu of a sparse keyed fold map on worker %d: %s", b, wi, cudaGetErrorString(q));
+        }
+    }
+    *ready = true;
+    // block b's totals, keys and counts (differences of its run starts)
+    struct Run { uint32_t key; uint32_t block; uint64_t at; };   // the block's run number
+    std::vector<Run> runs;
+    std::vector<const uint64_t*> starts(nb);
+    for (size_t b = 0; b < nb; ++b) {
+        const uint64_t D = *blocks[b]->cx.n_groups;
+        uint64_t h_keys, h_starts;
+        sparse_host_layout(D, R, &h_keys, &h_starts);
+        const uint8_t* h = (const uint8_t*)st.sparse_host[b];
+        starts[b] = (const uint64_t*)(h + h_starts);
+        for (uint64_t r = 0; r < D; ++r) runs.push_back({((const uint32_t*)(h + h_keys))[r], (uint32_t)b, r});
+    }
+    // stable: within one key the runs stay in block order
+    if (nb > 1) std::stable_sort(runs.begin(), runs.end(), [](const Run& a, const Run& b) { return a.key < b.key; });
+    std::vector<uint32_t> keys;
+    std::vector<uint64_t> counts, offs;
+    for (size_t i = 0; i < runs.size(); ++i) {
+        const Run& r = runs[i];
+        const uint64_t c = starts[r.block][r.at + 1] - starts[r.block][r.at];
+        if (i == 0 || r.key != runs[i - 1].key) {
+            keys.push_back(r.key);
+            counts.push_back(0);
+            offs.push_back(i);
+        }
+        counts.back() += c;
+    }
+    offs.push_back(runs.size());
+    const uint64_t D = keys.size();
+    void* out = nullptr;
+    if (D) {
+        int rc = pinned_acquire(p, D * R, &out);
+        if (rc != FBR_OK) return rc;
+        if (nb == 1) {
+            memcpy(out, st.sparse_host[0], D * R);
+        } else {
+            std::vector<uint8_t> values(runs.size() * R);
+            for (size_t i = 0; i < runs.size(); ++i)
+                memcpy(&values[i * R], (const uint8_t*)st.sparse_host[runs[i].block] + runs[i].at * R, R);
+            rc = fold_segments_host(p, body, values.data(), offs.data(), (uint32_t)D, out);
+            if (rc != FBR_OK) {
+                pinned_release(p, out);
+                return rc;
+            }
+        }
+    }
+    st.out = out;
+    st.own_out = out != nullptr;
+    st.group_keys.swap(keys);
+    st.group_counts.swap(counts);
+    for (void*& h : st.sparse_host) {
+        pinned_release(p, h);
+        h = nullptr;
+    }
+    return FBR_OK;
+}
+
 // Queues on worker w's s_fold the wrap of the n records at `values` (w's device memory, rewritten in place) with the m host
 // records `pieces`, right-nested: the body's scan entry without its prefix step.  With `host`, the wrapped records are then
 // copied there; with `done`, an event is created there and recorded behind it all.  Nothing is waited for, but an upload
@@ -2742,7 +3001,7 @@ static cudaError_t queue_wrap(Worker& w, const BodyEntry& body, const void* piec
 // The caller holds the pool lock.  The first call reads every block's total into st.scan_totals (R bytes per block)
 // before any block is wrapped: a wrap rewrites the record that holds its block's total.  Then, block by block, the pieces
 // are folded from those totals and the wrap is queued on the block's own worker's s_fold (queue_wrap), host results with
-// their one D2H copy into the pinned segment, behind the event st.scan_done[b].  A call that failed part-way resumes at the
+// their one D2H copy into the pinned segment, behind the event st.block_done[b].  A call that failed part-way resumes at the
 // first block without one and folds the same pieces from the kept totals.  With `block` the wraps are waited for here;
 // otherwise *ready tells whether they have all finished (fbr_result_wait waits for them outside the lock).
 static int scan_finish(fbr_pool* p, SeqState& st, bool block, bool* ready) {
@@ -2766,10 +3025,10 @@ static int scan_finish(fbr_pool* p, SeqState& st, bool block, bool* ready) {
             }
         }
         st.scan_totals.swap(totals);
-        st.scan_done.assign(nb, nullptr);
+        st.block_done.assign(nb, nullptr);
     }
     for (size_t b = 1; b < nb; ++b) {
-        if (st.scan_done[b]) continue;            // queued by an earlier call
+        if (st.block_done[b]) continue;            // queued by an earlier call
         SeqPart& part = *blocks[b];
         Worker& w = p->workers[part.worker];
         if (w.dead) return fail(FBR_ECUDA, "worker %d died before its block of a scan map was wrapped", part.worker);
@@ -2783,7 +3042,7 @@ static int scan_finish(fbr_pool* p, SeqState& st, bool block, bool* ready) {
         }
         const uint32_t m = (uint32_t)(pieces.size() / R);
         uint8_t* const host = on_device ? nullptr : (uint8_t*)st.out + part.first * R;
-        const cudaError_t e = queue_wrap(w, body, pieces.data(), m, part.cx.window_base, part.count, host, &st.scan_done[b]);
+        const cudaError_t e = queue_wrap(w, body, pieces.data(), m, part.cx.window_base, part.count, host, &st.block_done[b]);
         if (e != cudaSuccess) {
             retire_if_dead(p, part.worker);
             return fail(FBR_ECUDA, "wrapping block %zu of a scan map of body %s on worker %d: %s", b, body.name.c_str(), part.worker,
@@ -2795,7 +3054,7 @@ static int scan_finish(fbr_pool* p, SeqState& st, bool block, bool* ready) {
     for (size_t b = 1; b < nb; ++b) {
         const int wi = blocks[b]->worker;
         cudaError_t q = p->workers[wi].dead ? cudaErrorUnknown : cudaSetDevice(p->workers[wi].device);
-        if (q == cudaSuccess) q = block ? cudaEventSynchronize(st.scan_done[b]) : cudaEventQuery(st.scan_done[b]);
+        if (q == cudaSuccess) q = block ? cudaEventSynchronize(st.block_done[b]) : cudaEventQuery(st.block_done[b]);
         if (q == cudaErrorNotReady) { cudaGetLastError(); *ready = false; return FBR_OK; }
         if (q != cudaSuccess) {
             retire_if_dead(p, wi);
@@ -2864,6 +3123,7 @@ static int complete_map(fbr_pool* p, SeqState& st, bool block, bool* ready) {
     if (st.flags & FBR_FOLD) rc = fold_host_records(p, body, (const uint8_t*)st.out + body.result_bytes, st.parts.size(), st.out);
     else if (st.flags & FBR_SCAN) rc = scan_finish(p, st, block, ready);
     else if ((st.flags & FBR_FOLD_KEYS) && st.parts.size() > 1) rc = keyed_finish(p, st);
+    else if (st.flags & FBR_FOLD_SPARSE_KEYS) rc = sparse_keyed_finish(p, st, block, ready);
     if (rc != FBR_OK) return st.dead_worker >= 0 ? dead_map_error(p, st) : rc;
     st.completed = *ready;
     return FBR_OK;
@@ -2908,10 +3168,11 @@ static int result_wait_locked_out(fbr_pool_t* p, uint64_t seq, int timeout_ms, f
             SeqState& st = *it->second;
             if (st.dead_worker >= 0) return dead_map_error(p, st);
             for (auto& part : st.parts) evs.push_back({part.worker, p->workers[part.worker].device, part.done});
-            // FBR_SCAN: the wraps of blocks after the first, once queued (scan_done[b] belongs to the b-th block by start)
+            // FBR_SCAN: the wraps of blocks after the first; FBR_FOLD_SPARSE_KEYS: every block's run fold -- once queued
+            // (block_done[b] belongs to the b-th block by start)
             const std::vector<SeqPart*> blocks = parts_in_order(st);
-            for (size_t b = 1; b < st.scan_done.size() && b < blocks.size(); ++b)
-                if (st.scan_done[b]) evs.push_back({blocks[b]->worker, p->workers[blocks[b]->worker].device, st.scan_done[b]});
+            for (size_t b = 0; b < st.block_done.size() && b < blocks.size(); ++b)
+                if (st.block_done[b]) evs.push_back({blocks[b]->worker, p->workers[blocks[b]->worker].device, st.block_done[b]});
         }
         // block outside the pool lock so other threads can keep submitting
         bool again = false;
@@ -3039,7 +3300,7 @@ int fbr_result_poll(fbr_pool_t* p, uint64_t seq, uint64_t* n_done) {
         done += part_done;
         if (part_done < part.count) break;
     }
-    if (st.flags & (FBR_FOLD | FBR_SCAN | FBR_FOLD_KEYS)) {   // results are final once the map is complete: 0 tasks done until then
+    if (st.flags & (FBR_FOLD | FBR_SCAN | FBR_FOLD_KEYS | FBR_FOLD_SPARSE_KEYS)) {   // final once the map is complete: 0 tasks done until then
         bool ready = false;
         if (done >= st.n_tasks) {                 // every part is done: fold and scan blocks count only then (above)
             const int rc = complete_map(p, st, false, &ready);
@@ -3111,6 +3372,9 @@ int fbr_result_fetch(fbr_pool_t* p, uint64_t seq, uint64_t first, uint64_t count
     if (st.flags & FBR_FOLD) return fail(FBR_EINVAL, "seq %llu is a fold map: its one result record is fbr_result_t.data", (unsigned long long)seq);
     if (st.flags & FBR_FOLD_KEYS)
         return fail(FBR_EINVAL, "seq %llu is a keyed fold map: its records and counts are fbr_result_t.data", (unsigned long long)seq);
+    if (st.flags & FBR_FOLD_SPARSE_KEYS)
+        return fail(FBR_EINVAL, "seq %llu is a sparse keyed fold map: its records are fbr_result_t.data, its keys and counts "
+                    "fbr_result_groups", (unsigned long long)seq);
     if (!(st.flags & FBR_RESULTS_ON_DEVICE)) return fail(FBR_EINVAL, "seq %llu does not keep its results on the device", (unsigned long long)seq);
     if (first + count > st.n_tasks) return fail(FBR_EINVAL, "range out of bounds");
     const uint64_t R = st.result_bytes;
@@ -3138,6 +3402,22 @@ int fbr_result_fetch(fbr_pool_t* p, uint64_t seq, uint64_t first, uint64_t count
         CK(cudaSetDevice(p->workers[part.worker].device));
         CK(cudaStreamSynchronize(p->workers[part.worker].s_out));
     }
+    return FBR_OK;
+}
+
+int fbr_result_groups(fbr_pool_t* p, uint64_t seq, uint64_t* n_groups, const uint32_t** keys, const uint64_t** counts) {
+    if (!p || !n_groups || !keys || !counts) return fail(FBR_EINVAL, "NULL argument");
+    std::lock_guard<std::mutex> g(p->mu);
+    auto it = p->seqs.find(seq);
+    if (it == p->seqs.end()) return fail(FBR_ENOENT, "unknown seq %llu", (unsigned long long)seq);
+    const SeqState& st = *it->second;
+    if (!(st.flags & FBR_FOLD_SPARSE_KEYS))
+        return fail(FBR_EINVAL, "seq %llu is not a sparse keyed fold map (FBR_FOLD_SPARSE_KEYS)", (unsigned long long)seq);
+    if (!st.completed || st.err_code)
+        return fail(FBR_EINVAL, "seq %llu has no groups before fbr_result_wait has succeeded", (unsigned long long)seq);
+    *n_groups = st.group_keys.size();
+    *keys = st.group_keys.data();
+    *counts = st.group_counts.data();
     return FBR_OK;
 }
 

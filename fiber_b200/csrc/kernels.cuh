@@ -1940,6 +1940,26 @@ __global__ void __launch_bounds__(kThreads) key_offsets_kernel(const uint32_t* s
     }
 }
 
+// Sparse keyed folds (FBR_FOLD_SPARSE_KEYS): the runs of equal keys of the n sorted keys.  run_heads_kernel flags the first
+// task of each run; the exclusive scan of the flags (scan_counts_kernel) gives each head its run number and D, the number of
+// runs, as its total; run_starts_kernel then writes run r's first place and key, and starts[D] = n.
+__global__ void __launch_bounds__(kThreads) run_heads_kernel(const uint32_t* sorted, uint32_t n, uint64_t* head) {
+    for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads)
+        head[i] = i == 0 || sorted[i] != sorted[i - 1];
+}
+
+__global__ void __launch_bounds__(kThreads) run_starts_kernel(const uint32_t* sorted, uint32_t n, const uint64_t* run_of,
+                                                              uint64_t* starts, uint32_t* keys) {
+    for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads) {
+        const uint32_t k = sorted[i];
+        if (i == 0 || k != sorted[i - 1]) {
+            starts[run_of[i]] = i;
+            keys[run_of[i]] = k;
+        }
+        if (i == 0) starts[run_of[n]] = n;
+    }
+}
+
 // dst record j <- src record perm[j], records of `words` W-byte words (W = 16, 8 or 4, the widest that divides R)
 template <class W>
 __global__ void __launch_bounds__(kThreads) gather_records_kernel(const W* src, W* dst, const uint32_t* perm, uint64_t n,

@@ -297,12 +297,48 @@ class KeyedResultArray(ResultArray):
         return "KeyedResultArray(%s%s, n_keys=%d, body=%s)" % (self[:6], "..." if len(self) > 6 else "", len(self), self._spec.name)
 
 
+class SparseKeyedResultArray(ResultArray):
+    """The result of a sparse keyed fold (``Pool.fold_by_sparse_key``): one record per distinct key some task produced, in
+    ascending key order, read like a map result; ``keys`` (uint32) are those keys and ``counts`` (uint64) their tasks."""
+
+    def __init__(self, spec, array, keys, counts):
+        super().__init__(spec, array)
+        self._keys, self._counts = keys, counts
+
+    @property
+    def keys(self):
+        return self._keys
+
+    @property
+    def counts(self):
+        return self._counts
+
+    def get(self, key, default=None):
+        """The record of ``key``, or ``default`` when no task produced it."""
+        i = int(np.searchsorted(self._keys, key))
+        return self[i] if i < len(self._keys) and int(self._keys[i]) == key else default
+
+    def __repr__(self):
+        return "SparseKeyedResultArray(%s%s, n_groups=%d, body=%s)" % (self[:6], "..." if len(self) > 6 else "", len(self),
+                                                                      self._spec.name)
+
+
 def host_result(spec, kind, data, n=0, total=None, values=None):
     """What a finished map whose results are in host memory returns, in either isolation.  ``kind`` is "plain", "bits"
-    (one bit per bool result), "emit" (variable-length results), "fold" or "keyed"; ``spec`` is the body the caller mapped;
-    ``n`` the number of results the caller sees (a keyed fold's n_keys).  ``data`` holds the result records as uint8 (the
-    bit-packed bytes, the end offsets of an emit map, a fold's one record, a keyed fold's n records then n uint64 counts),
-    or is None for a map over no tasks; ``values`` are an emit map's values; ``total`` is the device-side sum, or None."""
+    (one bit per bool result), "emit" (variable-length results), "fold", "keyed" or "sparse"; ``spec`` is the body the
+    caller mapped; ``n`` the number of results the caller sees (a keyed fold's n_keys, a sparse keyed fold's D).  ``data``
+    holds the result records as uint8 (the bit-packed bytes, the end offsets of an emit map, a fold's one record, a keyed
+    fold's n records then n uint64 counts, a sparse keyed fold's n records, n uint64 counts, then n uint32 keys), or is None
+    for a map over no tasks; ``values`` are an emit map's values; ``total`` is the device-side sum, or None."""
+    if kind == "sparse":
+        dtype, sub = spec.result_dtype()
+        R = spec.result_bytes
+        if data is None:        # no task: no key
+            return SparseKeyedResultArray(spec, np.empty((0,) + sub, dtype), np.empty(0, np.uint32), np.empty(0, np.uint64))
+        records = data[:n * R]
+        counts = data[n * R:n * (R + 8)].copy().view(np.uint64)
+        keys = data[n * (R + 8):n * (R + 12)].copy().view(np.uint32)
+        return SparseKeyedResultArray(spec, records.view(dtype).reshape((n,) + sub), keys, counts)
     if kind == "fold":
         return spec.unpack_result(fold_identity(spec) if data is None else bytes(data))
     if kind == "keyed":
@@ -340,7 +376,9 @@ def _n_keys(n_keys):
 def _raise_task_error(name, code, task, emit_count=None, n_keys=None):
     """Raise the exception of a map's first failed task (``err_code`` / ``err_task`` of its fbr_result_t) for body
     ``name``; ``emit_count(task)`` gives the number of values an emit body's task was counted to push, and ``n_keys`` is a
-    keyed fold's number of keys."""
+    keyed fold's number of keys (0 for a sparse keyed fold)."""
+    if code == _abi.FBR_TASK_KEY and not n_keys:
+        raise ValueError("%s: key() of task %d is 0xffffffff, which fold_by_sparse_key reserves" % (name, task))
     if code == _abi.FBR_TASK_KEY:
         raise ValueError("%s: key() of task %d is not below n_keys=%d" % (name, task, n_keys))
     if code == _abi.FBR_TASK_EMIT:
@@ -367,6 +405,7 @@ class MapResult:
         self._n_items = n if n_items is None else n_items      # the items the caller mapped
         self._n_keys = n_keys
         self._kind = "fold" if flags & _abi.FBR_FOLD else "keyed" if flags & _abi.FBR_FOLD_KEYS else \
+            "sparse" if flags & _abi.FBR_FOLD_SPARSE_KEYS else \
             "bits" if user_spec is not None else "emit" if spec.flags & _abi.FBR_BODY_EMIT else "plain"
         self._result = None
         self._exc = None              # a task error is raised again by every later get()
@@ -391,6 +430,14 @@ class MapResult:
         elif self._kind == "keyed":         # n_keys records, then n_keys uint64 counts
             self.raw = ctypes.string_at(res.data, self._n_keys * (res.result_bytes + 8))
             self._result = host_result(self._spec, "keyed", np.frombuffer(self.raw, np.uint8), self._n_keys)
+        elif self._kind == "sparse":        # D records (fbr_result_t.data), then D counts and D keys (fbr_result_groups)
+            eng, d = self._engine, ctypes.c_uint64(0)
+            keys, counts = ctypes.c_void_p(), ctypes.c_void_p()
+            _abi.check(eng.lib.fbr_result_groups(eng.handle, self._seq, ctypes.byref(d), ctypes.byref(keys), ctypes.byref(counts)))
+            D = d.value
+            self.raw = ctypes.string_at(res.data, D * res.result_bytes) + ctypes.string_at(counts, 8 * D) + \
+                ctypes.string_at(keys, 4 * D)
+            self._result = host_result(self._spec, "sparse", np.frombuffer(self.raw, np.uint8), D)
         elif self._flags & _abi.FBR_RESULTS_ON_DEVICE:
             self._result = self._device_result(res, dsum)
         else:
@@ -534,6 +581,15 @@ class KeyedFoldResult(MapResult):
 
     def _iter_ready(self):
         raise TypeError("%s: a keyed fold has one result per key, not one per task: use get()" % self._spec.name)
+
+
+class SparseKeyedFoldResult(MapResult):
+    """Handle of an asynchronous sparse keyed fold (``Pool.fold_by_sparse_key_async``): ``get()`` returns a
+    SparseKeyedResultArray of one record per distinct key, with its keys and counts (FBR_FOLD_SPARSE_KEYS in
+    include/fiber_b200.h)."""
+
+    def _iter_ready(self):
+        raise TypeError("%s: a sparse keyed fold has one result per distinct key, not one per task: use get()" % self._spec.name)
 
 
 class ApplyResult(MapResult):
@@ -815,14 +871,14 @@ class Pool:
         return registry.spec(registry.body_name_of(func))
 
     def _start(self, func, iterable, *, star, mode, chunksize=None, streaming=False, n_keys=0):
-        """The one submission path of maps (``mode`` "map"), folds, keyed folds ("fold_by_key") and accumulates of ``func``
-        over ``iterable``, whose items are argument tuples with ``star``: a MapResult, a FoldResult for a fold, or a
-        KeyedFoldResult for a keyed fold."""
+        """The one submission path of maps (``mode`` "map"), folds, keyed folds ("fold_by_key"), sparse keyed folds
+        ("fold_by_sparse_key") and accumulates of ``func`` over ``iterable``, whose items are argument tuples with ``star``:
+        a MapResult, a FoldResult for a fold, a KeyedFoldResult for a keyed fold or a SparseKeyedFoldResult for a sparse one."""
         self._check_running()
         if chunksize is None:
             chunksize = DEFAULT_CHUNKSIZE if mode == "map" else 0     # a fold's order does not depend on a chunksize
         spec = self._spec_of(func) if mode == "map" else \
-            self._fold_spec(func, scan=mode == "accumulate", keyed=mode == "fold_by_key")
+            self._fold_spec(func, scan=mode == "accumulate", keyed=mode in ("fold_by_key", "fold_by_sparse_key"))
         if mode == "fold_by_key":
             n_keys = _n_keys(n_keys)
         if not hasattr(iterable, "__len__"):
@@ -835,6 +891,7 @@ class Pool:
         cls, want_sum, flags = {"map": (MapResult, True, _abi.FBR_NO_ZERO_COPY if streaming else 0),
                                 "fold": (FoldResult, False, _abi.FBR_FOLD),
                                 "fold_by_key": (KeyedFoldResult, False, _abi.FBR_FOLD_KEYS),
+                                "fold_by_sparse_key": (SparseKeyedFoldResult, False, _abi.FBR_FOLD_SPARSE_KEYS),
                                 "accumulate": (MapResult, False, _abi.FBR_SCAN)}[mode]
         if mode != "map" and len(iterable) == 0:          # identity() / no prefixes: nothing to bind or submit
             return cls(self, self._engine, spec, 0, 0, None, flags, n_keys=n_keys)
@@ -850,7 +907,7 @@ class Pool:
 
     def _submit_proc(self, spec, kind, items, chunksize, n_keys=0):
         """Process-isolated workers: the map is cut into blocks that worker processes pull (procpool.py).  ``kind`` is the
-        block kind: "map", "apply", "fold", "fold_by_key" (with ``n_keys``) or "accumulate", with "star" in front for
+        block kind: "map", "apply", "fold", "fold_by_key" (with ``n_keys``), "fold_by_sparse_key" or "accumulate", with "star" in front for
         argument tuples."""
         if (kind.startswith("star") and not isinstance(items, registry.Columns)) or \
                 not isinstance(items, (range, list, np.ndarray, registry.Ragged, registry.Columns)):
@@ -926,6 +983,26 @@ class Pool:
 
     def starfold_by_key(self, func, iterable, n_keys):
         return self.starfold_by_key_async(func, iterable, n_keys).get()
+
+    # -- sparse keyed folds: a fold per distinct uint32 key() of the results, on the device -----------------------------
+    def fold_by_sparse_key_async(self, func, iterable):
+        """A fold of the results of each distinct key: a SparseKeyedFoldResult whose ``get()`` gives a
+        SparseKeyedResultArray with one record per key some task produced, in ascending key order -- record k the fold of
+        the results whose body ``key()`` is k in the order of FBR_FOLD_SPARSE_KEYS (include/fiber_b200.h), on one worker
+        ``fold(func, [x for x in iterable if key(func(x)) == k])`` bit for bit -- with ``keys`` and ``counts``.  Keys are
+        any uint32 but 0xFFFFFFFF, which is reserved: a task whose key is 0xFFFFFFFF raises ValueError.  There is no
+        chunksize, as for ``fold``."""
+        return self._start(func, iterable, star=False, mode="fold_by_sparse_key")
+
+    def fold_by_sparse_key(self, func, iterable):
+        return self.fold_by_sparse_key_async(func, iterable).get()
+
+    def starfold_by_sparse_key_async(self, func, iterable):
+        """``fold_by_sparse_key_async`` over argument tuples, bound as ``starmap`` binds them."""
+        return self._start(func, iterable, star=True, mode="fold_by_sparse_key")
+
+    def starfold_by_sparse_key(self, func, iterable):
+        return self.starfold_by_sparse_key_async(func, iterable).get()
 
     # -- accumulates: every prefix of a fold, on the device ------------------------------------------------------------
     def accumulate_async(self, func, iterable):

@@ -183,6 +183,9 @@ def gpu_worker_main(device, conn, results, sys_path, init=None):
         if msg[0] == "keyed":
             _fold_keyed_totals_in_worker(pool, conn, segments, msg)
             continue
+        if msg[0] == "sparse":
+            _fold_sparse_totals_in_worker(pool, conn, msg)
+            continue
         _, job, blk, body, kind, chunksize, payload, shm_name, off, attempt, module = msg
         with _reporting(conn, job, blk):
             _register(body, module)
@@ -199,6 +202,10 @@ def gpu_worker_main(device, conn, results, sys_path, init=None):
             else:
                 handle = pool._start(f, items, star=mode != kind, mode=mode, chunksize=chunksize)
             res = handle._wait()
+            if mode == "fold_by_sparse_key":                       # D records, counts and keys, in a file of the block's own
+                put_values(values_name(shm_name, blk), np.frombuffer(handle.raw, np.uint8))
+                conn.send(("done", job, blk, None))
+                continue
             if mode in ("fold", "fold_by_key"):                    # the block's total (R bytes), or its n_keys totals and counts
                 raw = np.frombuffer(handle.raw, np.uint8)
             else:
@@ -304,6 +311,49 @@ def _fold_keyed_totals_in_worker(pool, conn, segments, msg):
         conn.send(("folded", job))
 
 
+def sparse_area(data, R):
+    """A sparse keyed fold's block (or result) as written by its worker: D records of R bytes, D uint64 counts, then D
+    uint32 keys (uint8) -> (keys, records as uint8 [D, R], counts)."""
+    D = len(data) // (R + 12)
+    return (np.array(data[D * (R + 8):D * (R + 12)]).view(np.uint32), np.asarray(data[:D * R]).reshape(D, R),
+            np.array(data[D * R:D * (R + 8)]).view(np.uint64))
+
+
+def sparse_keyed_sequence(keys, records, counts):
+    """The input of the last step of a sparse keyed fold: the key-major sequence of the block totals, stable by key with
+    block order inside each key (uint8), its D + 1 run offsets, the D distinct keys in ascending order and their summed
+    counts.  ``keys``, ``records`` ([D_b, R] uint8) and ``counts`` are the blocks' in block order."""
+    allk = np.concatenate(keys) if keys else np.zeros(0, np.uint32)
+    order = np.argsort(allk, kind="stable")
+    sk = allk[order]
+    head = np.flatnonzero(np.concatenate([[True], sk[1:] != sk[:-1]])) if len(sk) else np.zeros(0, np.int64)
+    offsets = np.concatenate([head, [len(sk)]]).astype(np.uint64)
+    values = np.concatenate(records)[order].reshape(-1) if len(sk) else np.zeros(0, np.uint8)
+    summed = np.add.reduceat(np.concatenate(counts)[order], head).astype(np.uint64) if len(sk) else np.zeros(0, np.uint64)
+    return values, offsets, sk[head], summed
+
+
+def _fold_sparse_totals_in_worker(pool, conn, msg):
+    """A sparse keyed fold map's last step, in the worker the master picked: the blocks' files (sparse_area) become the
+    result file -- record k is tree() over the totals of the blocks where key k has tasks, in block order
+    (fbr_fold_segments), and count k the sum of the blocks' counts -- and D is reported."""
+    from fiber_b200 import registry
+    _, job, n_blocks, body, shm_name, module = msg
+    with _reporting(conn, job, -1):
+        _register(body, module)
+        spec = registry.spec(body)
+        R = spec.result_bytes
+        areas = [sparse_area(np.fromfile(os.path.join("/dev/shm", values_name(shm_name, b)), np.uint8), R) for b in range(n_blocks)]
+        values, offsets, keys, counts = sparse_keyed_sequence(*zip(*areas)) if areas else sparse_keyed_sequence([], [], [])
+        out = np.zeros(len(keys) * R, np.uint8)
+        values = np.ascontiguousarray(values)
+        if len(keys):
+            _abi.check(pool._engine.lib.fbr_fold_segments(pool._engine.handle, spec.func_id, values.ctypes.data,
+                                                          offsets.ctypes.data, len(keys), out.ctypes.data))
+        put_values(values_name(shm_name, n_blocks), np.concatenate([out, counts.view(np.uint8), keys.view(np.uint8)]))
+        conn.send(("folded", job, len(keys)))
+
+
 # ------------------------------------------------------------------------------------------------
 # master side
 # ------------------------------------------------------------------------------------------------
@@ -326,6 +376,10 @@ class _Job:
         self.n_keys = n_keys
         if self.keyed:
             self.chunksize = n_keys
+        # sparse keyed fold maps: each block writes its records, counts and keys to a file of its own (values_name), and
+        # the last step writes the result to the file after them and reports D (n_groups)
+        self.sparse = kind in ("fold_by_sparse_key", "starfold_by_sparse_key")
+        self.n_groups = 0
         # accumulate maps: each block places its own prefix folds like a map; blocks after the first are wrapped at the end
         self.scan = kind in ("accumulate", "staraccumulate")
         self.scan_wrapped = set()                     # blocks (b > 0) already wrapped and placed
@@ -337,15 +391,16 @@ class _Job:
         self.n_blocks, self.done_blocks = len(blocks), 0
         self.payload_of, self.module = payload_of, module
         nbytes = ((n + 7) // 8) if bits else ((1 + len(blocks)) * result_bytes if self.fold else
-                                              (1 + len(blocks)) * n_keys * (result_bytes + 8) if self.keyed else n * result_bytes)
+                                              (1 + len(blocks)) * n_keys * (result_bytes + 8) if self.keyed else
+                                              1 if self.sparse else n * result_bytes)
         self.shm = SharedSegment("fbr_%d_%d_%d" % (os.getpid(), jid, int(time.time() * 1e6) & 0xFFFFFF), nbytes) if n else None
         self.nbytes = nbytes
         self.sum, self.error = 0, None
         self.event = threading.Event()
         if self.shm is not None:            # the /dev/shm name never outlives the job object (fire-and-forget maps, failed maps)
             weakref.finalize(self, _release_shm, self.shm)
-            if out_dtype is not None:
-                weakref.finalize(self, _unlink_values, self.shm.name, len(blocks))
+            if out_dtype is not None or self.sparse:
+                weakref.finalize(self, _unlink_values, self.shm.name, len(blocks) + self.sparse)
 
     def offset(self, lo, blk):
         if self.fold:
@@ -411,16 +466,20 @@ class ProcessResult:
                 raise TimeoutError("map %d not finished" % job.id)
             if job.error is not None:
                 raise job.error
-            kind = "fold" if job.fold else "keyed" if job.keyed else "emit" if job.out_dtype is not None else \
-                "bits" if job.bits else "plain"
+            kind = "fold" if job.fold else "keyed" if job.keyed else "sparse" if job.sparse else \
+                "emit" if job.out_dtype is not None else "bits" if job.bits else "plain"
             data = values = None
             if kind == "emit" and job.n:
                 data, values = self._emit_parts()
+            elif kind == "sparse" and job.n:
+                data = np.fromfile(os.path.join("/dev/shm", values_name(job.shm.name, job.n_blocks)), np.uint8)
+                _unlink_values(job.shm.name, job.n_blocks + 1)
             elif job.n:
                 data = job.shm.array[:job.result_bytes if job.fold else
                                      job.n_keys * (job.result_bytes + 8) if job.keyed else job.nbytes]
             total = job.sum if (self._spec.flags & _abi.FBR_BODY_SUMMABLE) else None
-            result = host_result(self._spec, kind, data, job.n_keys if job.keyed else job.n, total, values)
+            result = host_result(self._spec, kind, data, job.n_keys if job.keyed else job.n_groups if job.sparse else job.n,
+                                 total, values)
             if job.shm is not None:
                 if not job.fold:
                     result._shm = job.shm    # the mapping lives as long as the result; workers are done with the name
@@ -500,6 +559,12 @@ class ProcessPool:
         n_keys totals and counts; once every block is in, one live worker folds each key's non-empty totals in block order
         (fbr_fold_segments) and sums the counts."""
         return self.submit(spec, None, "fold_by_key" if kind == "map" else "starfold_by_key", items, 0, n_keys=n_keys)
+
+    def submit_fold_by_sparse_key(self, spec, kind, items):
+        """A sparse keyed fold map (``kind`` "map" or "starmap"): each block runs ``Pool.fold_by_sparse_key`` in its worker
+        and writes its records, counts and keys to a file of its own; once every block is in, one live worker merges the
+        blocks' keys, folds each key's totals in block order (fbr_fold_segments) and sums the counts."""
+        return self.submit(spec, None, "fold_by_sparse_key" if kind == "map" else "starfold_by_sparse_key", items, 0)
 
     def submit(self, spec, twin, kind, items, chunksize, single=False, n_keys=0):
         """items: a ``range`` or a list/array of per-task items (tuples for starmap).  ``n_keys``: a keyed fold's keys."""
@@ -628,13 +693,14 @@ class ProcessPool:
                     if w.block is not None and w.block[0] is job:
                         inflight -= 1
                     self._on_death(w, dead_reason)
-        if (job.fold or job.keyed or (job.scan and job.n_blocks > 1)) and job.n and job.error is None:
+        if (job.fold or job.keyed or job.sparse or (job.scan and job.n_blocks > 1)) and job.n and job.error is None:
             self._fold_totals(job)
         job.event.set()
 
     def _fold_totals(self, job):
         """A fold map whose blocks have all placed their totals: one live worker folds them in block order into the result
-        record; a keyed fold map's per key (_fold_keyed_totals_in_worker); an accumulate map's wraps every block after the
+        record; a keyed fold map's per key (_fold_keyed_totals_in_worker); a sparse keyed fold map's per distinct key
+        (_fold_sparse_totals_in_worker); an accumulate map's wraps every block after the
         first (_scan_blocks_in_worker).  This runs after close()
         too, like the blocks of queued maps; terminate() abandons it.  A worker that dies meanwhile is replaced and the fold goes to the next live one, as a block would be re-queued: without error_handling
         the first death fails the map, and MAX_ATTEMPTS deaths fail it in any case.  The map always ends folded or failed."""
@@ -662,6 +728,8 @@ class ProcessPool:
                     w.conn.send(("scan", job.id, job.ranges, todo, job.scan_totals, job.body, job.shm.name, job.module))
                 elif job.keyed:
                     w.conn.send(("keyed", job.id, job.n_blocks, job.n_keys, job.body, job.shm.name, job.module))
+                elif job.sparse:
+                    w.conn.send(("sparse", job.id, job.n_blocks, job.body, job.shm.name, job.module))
                 else:
                     w.conn.send(("fold", job.id, job.n_blocks, job.body, job.shm.name, job.module))
             except (OSError, ValueError):
@@ -674,6 +742,8 @@ class ProcessPool:
                     if msg[0] == "scanned":
                         job.scan_wrapped.add(msg[2])
                     elif msg[0] == "folded":
+                        if job.sparse:
+                            job.n_groups = msg[2]
                         return
                     elif msg[0] == "error":
                         self._fail(job, _ERRORS.get(msg[3], RuntimeError)(msg[4]))

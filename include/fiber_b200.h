@@ -287,6 +287,26 @@ int fbr_pool_worker_device(fbr_pool_t* pool, int worker, int* device_id);
                                    its n_keys totals and counts cross PCIe.  fbr_result_poll reports 0 tasks done until the
                                    whole map is, fbr_result_fetch refuses the map, and a worker that dies under it fails it */
 #define FBR_MAX_KEYS 65536u
+#define FBR_FOLD_SPARSE_KEYS 0x20000u  /* fold per distinct key (FBR_BODY_KEYED bodies), for any uint32 key() but 0xFFFFFFFF:
+                                   fbr_result_t.data holds D records, one per distinct key some task produced, in ascending
+                                   key order; fbr_result_groups gives D, the keys and the tasks per key.  Record k is
+                                   FBR_FOLD_KEYS' record k with the keys without tasks left out: each block's total for k is
+                                   tree() of its own x_k, record k tree() over the totals of the blocks where k has a task, in
+                                   block order, under the fold plan's block cut (FBR_PLAN_FOLD).  One worker gives tree(x_k);
+                                   with every key below K <= 65536 the records, keys and counts are FBR_FOLD_KEYS' over K keys
+                                   without its empty keys, bit for bit.  Nothing else -- chunksize, unit size, ring_bytes,
+                                   waves, FBR_SHUFFLE, FBR_VIA_RING, re-dispatched units -- changes a bit.  desc.n_keys must
+                                   be 0, and a block holds fewer than 2^32 tasks.  Refused with FBR_FOLD, FBR_SCAN,
+                                   FBR_FOLD_KEYS, out, FBR_OUT_DEVICE, FBR_WANT_SUM or FBR_NO_ZERO_COPY; FBR_RESULTS_ON_DEVICE
+                                   changes nothing.  The key 0xFFFFFFFF is reserved: a task whose key() is 0xFFFFFFFF fails the
+                                   map with FBR_TASK_KEY (the engine calls the body's keys entry with n_keys = 0xFFFFFFFF).
+                                   Each block is a full-window map; after its last round it sorts its tasks by key on the
+                                   device (four 8-bit LSD radix passes), gathers its records into key order and finds the
+                                   runs of equal keys; its D, known only then, sizes the result at completion, where each
+                                   block's runs are folded and, with several blocks, the blocks' sorted keys are merged on the
+                                   host.  Only the D records, keys and run starts of each block cross PCIe.
+                                   fbr_result_poll reports 0 tasks done until the whole map is, fbr_result_fetch refuses the
+                                   map, and a worker that dies under it fails it */
 
 typedef struct fbr_map_desc {
     int32_t func_id;
@@ -405,10 +425,13 @@ typedef enum fbr_task_error {
     FBR_TASK_BADARG = 2,
     FBR_TASK_FAULT = 3,      /* injected fault (resilient-pool tests) */
     FBR_TASK_EMIT = 4,       /* an emit body's task pushed another number of values than its count pass gave */
-    FBR_TASK_KEY = 5         /* FBR_FOLD_KEYS: the task's key() is not below n_keys */
+    FBR_TASK_KEY = 5         /* FBR_FOLD_KEYS: the task's key() is not below n_keys; FBR_FOLD_SPARSE_KEYS: it is 0xFFFFFFFF */
 } fbr_task_error;
 
 int fbr_result_wait(fbr_pool_t* pool, uint64_t seq, int timeout_ms, fbr_result_t* res);
+/* A FBR_FOLD_SPARSE_KEYS map once fbr_result_wait has succeeded: *n_groups = D, the number of its records; *keys = its D
+ * distinct keys in ascending order and *counts = the tasks of each (host memory owned by the map until its release). */
+int fbr_result_groups(fbr_pool_t* pool, uint64_t seq, uint64_t* n_groups, const uint32_t** keys, const uint64_t** counts);
 int fbr_result_poll(fbr_pool_t* pool, uint64_t seq, uint64_t* n_done);
 /* Address of the map's ordered-result buffer without waiting: tasks [0, n_done) of it are final. */
 int fbr_result_data(fbr_pool_t* pool, uint64_t seq, void** data);

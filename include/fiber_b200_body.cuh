@@ -79,6 +79,12 @@
 // key() is not below n_keys fails the map with FBR_TASK_KEY.  FBR_EXPORT_RECORD_BODY exports the keys entry (keys_kernel)
 // and the fold_segments entry (a segmented tree()) after scan.
 //
+// The same body also folds by any 32-bit key: Pool.fold_by_sparse_key(f, xs) returns one record per distinct key that some
+// task produced, in ascending key order, with its key and its count (FBR_FOLD_SPARSE_KEYS).  Record k is fold_by_key's
+// record k with the keys without tasks left out, so one worker again gives Pool.fold(f, [x for x in xs if key(f(x)) == k]).
+// The key 0xFFFFFFFF is reserved: the engine calls the keys entry with n_keys = 0xFFFFFFFF, and a task whose key() is
+// 0xFFFFFFFF fails the map with FBR_TASK_KEY.  No other body code is needed.
+//
 // A record body may also read one array every task of a map shares (the pool initializer's initargs, or the same array
 // in every task tuple): it declares the array's element type and a shared-memory budget, and run() gets the block
 // after the result:
